@@ -3,7 +3,7 @@
 synthetic graph (232 965 V, 114.6 M power-law edges + self loops, LAYERS 602-128-41, fp32), N GPUs of one node.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
-                    [--workload reddit|products|papers100m|tiny] [--toolkit gcn|gcn_eager|gat]
+                    [--workload reddit|products|papers100m|tiny] [--toolkit gcn|gcn_eager|gat] [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...        (N > 1: one rank per GPU, NCCL)
 
 One step = one training epoch through the reference-shaped API (toolkits.GCNImpl <-> toolkits/GCN.hpp):
@@ -15,11 +15,18 @@ through the peer-memory engine (csrc/nts_exchange.cu).  `--workload products` / 
 Prints ONE JSON line (rank 0).  `value` = aggregated edges per second over the whole job (3*E / epoch time) with
 inputs resident in HBM; `e2e` = the same with the feature matrix coming from pinned host memory every step and the
 loss read back; `roofline` = the layer-0 forward aggregation kernel timed live with CUDA events (`frac` algorithmic
-bytes, `frac_dram` ncu DRAM bytes of the committed capture of the same kernel, `frac_min` compulsory bytes);
+bytes, `frac_min` compulsory bytes);
 `parity` (N > 1) = the benchmarked distributed operator against a float64 reference on this box; `exchange_timeline`
 (N > 1) = per-phase device time of one forward exchange; `cpu_baseline` / `--impl reference` = the UNMODIFIED
-reference CPU GCN (toolkits/GCN_CPU.hpp via oracle/_ref, built from /root/reference by oracle/Makefile) on this box's
-usable host threads - on the workload itself when it fits the time budget, else on a stated 1/div scale model.
+reference CPU GCN (toolkits/GCN_CPU.hpp via oracle/_ref, built from the reference sources by oracle/Makefile) on the
+host's usable threads - on the workload itself when it fits the time budget, else on a stated 1/div scale model;
+null when oracle/_ref was not built.
+
+`--dump-outputs DIR` writes what the last timed step computed: the loss `run_epoch` returns (`loss.npy`) and the last
+layer's output rows it was computed from (`output.npy`; float32, a fixed seeded sample of rows with their ids in
+`output_rows.npy` when the matrix would exceed 64 MB); ranks > 0 of a multi-GPU run add `_rank<r>` to each name.
+The weights are left out: Adam turns last-bit differences of near-zero gradients into steps of the learning rate.  Inputs are generated
+from fixed seeds, so two builds run with the same arguments can be compared file by file.
 """
 import argparse
 import json
@@ -65,6 +72,8 @@ def parse_args():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-ref-gpu", action="store_true", help="skip timing the reference's own CUDA kernels")
     ap.add_argument("--zipf-s", type=float, default=1.0, help="endpoint skew (1.0 = SURVEY 8d power law, 0 = uniform)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step to DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -160,8 +169,8 @@ def reference_cpu_epochs(V, layers, edges_u32, steps, warmup, threads=None):
     E = int(edges_u32.shape[0])
     if not os.path.exists(binary):
         # never substitute the port silently: a "port" number must not be mistaken for the reference
-        raise SystemExit("bench.py: oracle/_ref/nts_ref_main is missing - build it with `make -C oracle ref` in the "
-                         "build container (it travels to the GPU box with the snapshot)")
+        raise SystemExit("bench.py: oracle/_ref/nts_ref_main is missing - build it with `make -C oracle ref` "
+                         "(needs the reference sources)")
     work = tempfile.mkdtemp(prefix="nts_bench_ref_")
     try:
         efile = os.path.join(work, "g.edge")
@@ -363,6 +372,7 @@ def main():
 
         class _AsGcn:                      # same (loss, acc) return and X[0] slot as the GCN toolkits
             X = gat_model.X
+            gat = gat_model
 
             @staticmethod
             def run_epoch():
@@ -404,6 +414,8 @@ def main():
     torch.cuda.nvtx.range_pop()
     ms_total = ev0.elapsed_time(ev1)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, model, rank, world)
     launches = lib.nts_kernel_launch_count() - launches0
     ops.set_kernel_timer(None)
     ksum = timer.summary()
@@ -477,14 +489,12 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        which = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s"
+        peak = float(peaks.get("hbm_gbs", 3350.0))
+        which = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet 3.35 TB/s"
         # algorithmic bytes (SURVEY 8d): E*(4 idx + 4 w + 4F row) + V_out*4F + (V_out+1)*4, summed over launches
         b_alg = k["edges"] * (8 + 4 * F0) + k["rows"] * 4 * F0 + (k["rows"] + k["calls"]) * 4
         achieved = b_alg / (k["ms"] * 1e-3) / 1e9
         t_launch = k["ms"] / k["calls"] * 1e-3
-        traffic = _ncu_traffic(F0) if (args.workload == "reddit" and world == 1 and args.zipf_s == 1.0
-                                       and not eager and ops._plan_mode != "off") else None
         # compulsory traffic (SURVEY 8d): every feature row once in, every output row once out, the graph arrays once
         b_min = (k["rows"] * 4 * F0 * 2 + k["edges"] * 8 + (k["rows"] + k["calls"]) * 4) / k["calls"]
         roof = {"bound": "hbm",
@@ -493,10 +503,7 @@ def main():
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_source": which,
                 "frac_note": "achieved = ALGORITHMIC bytes / time (SURVEY 8d: every gathered row counted as if it "
                              "came from HBM); > 1 means L1/L2 reuse, it is NOT a physical HBM fraction - see "
-                             "frac_dram (ncu dram bytes of the same kernel / time) and frac_min (compulsory bytes)",
-                "traffic": traffic["bytes"] if traffic else None,
-                "traffic_source": traffic["source"] if traffic else None,
-                "frac_dram": (traffic["bytes"] / t_launch / 1e9 / peak) if traffic else None,
+                             "frac_min (compulsory bytes)",
                 "frac_min": b_min / t_launch / 1e9 / peak,
                 "launches": k["calls"], "avg_ms_per_launch": k["ms"] / k["calls"],
                 "algorithmic_bytes_per_launch": b_alg / k["calls"], "compulsory_bytes_per_launch": b_min}
@@ -518,7 +525,8 @@ def main():
                 "note": "CUDA-event time of the aggregation launches only (rank 0), SURVEY 8d"}
     if rank == 0:
         cpu = None
-        if not args.no_cpu_baseline and world == 1 and not eager and not gat:   # the CPU arm is ALGORITHM:GCNCPU
+        ref_built = os.path.exists(os.path.join(ROOT, "oracle", "_ref", "nts_ref_main"))
+        if not args.no_cpu_baseline and world == 1 and not eager and not gat and ref_built:   # ALGORITHM:GCNCPU
             cores = usable_cores()
             div, probe = pick_cpu_sample(V, E_rand, layers, args.cpu_sample_div, min(args.cpu_budget_s, 25.0), 3, cores)
             Vs, edges = _scale_model(V, E_rand, div)
@@ -677,7 +685,7 @@ def exchange_timeline(ex, feats, layers, world, dev):
 
 
 def reference_gpu_kernels(pg, feats, layers, torch):
-    """Time the UNMODIFIED reference CUDA kernels (cuda/ntsCUDAFuseKernel.cuh, compiled for sm_100a into
+    """Time the UNMODIFIED reference CUDA kernels (cuda/ntsCUDAFuseKernel.cuh, compiled for sm_90a into
     oracle/_ref/libnts_refcuda.so) on the same chunk and inputs: 1 warm-up + 2 timed launches per width, CUDA events
     on the reference's own stream.  Also cross-checks their output against ours.  Bench-only baseline."""
     import ctypes as C
@@ -739,6 +747,30 @@ def reference_gpu_kernels(pg, feats, layers, torch):
     return out
 
 
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(d, model, rank, world):
+    """What the last timed step computed: its loss and the last layer's output rows (float32).  An output matrix too
+    large for this rank's share of DUMP_BYTES is cut to a fixed seeded sample of rows (their ids in output_rows.npy)."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    sfx = "_rank%d" % rank if rank else ""
+    loss = model.loss if hasattr(model, "loss") else model.gat.loss
+    arrays = {"loss": np.array([float(loss.detach().item())], dtype=np.float32)}
+    out = model.X[-1].detach().float()
+    room = DUMP_BYTES // world - 4096   # (4 KB: the .npy headers and the loss)
+    if out.numel() * 4 > room:
+        n = room // (out.shape[1] * 4 + 8)
+        rows = np.sort(np.random.default_rng(0x5EED0004).choice(out.shape[0], size=n, replace=False))
+        arrays["output_rows"] = rows.astype(np.float64)
+        out = out[torch.from_numpy(rows).to(out.device)]
+    arrays["output"] = out.cpu().numpy()
+    for name, a in arrays.items():
+        np.save(os.path.join(d, name + sfx + ".npy"), a)
+
+
 def _gat_roofline(k, ksum, F, H):
     """K7 forward (segment_gather_sum_kernel in head mode 2): per edge one slot index, one [H] source-score row and
     one F-wide mirror row; per destination its F-wide output and three [H] rows (score, max, sum)."""
@@ -747,12 +779,12 @@ def _gat_roofline(k, ksum, F, H):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
     b_alg = k["edges"] * (4 + 4 * H + 4 * F) + k["rows"] * (4 * F + 12 * H) + (k["rows"] + k["calls"]) * 4
     achieved = b_alg / (k["ms"] * 1e-3) / 1e9
     out = {"bound": "hbm", "kernel": "segment_gather_sum_kernel<HM=2> (fused GAT attention forward, F=%d, %d heads)" % (F, H),
            "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-           "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s",
+           "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet 3.35 TB/s",
            "frac_note": "algorithmic bytes / time; > 1 means L1/L2 reuse of the gathered rows", "traffic": None,
            "launches": k["calls"], "avg_ms_per_launch": k["ms"] / k["calls"],
            "algorithmic_bytes_per_launch": b_alg / k["calls"]}
@@ -773,8 +805,8 @@ def _config(args, V, E_total, layers):
             "aggregations_per_epoch": 2 * n_layers if eager else 2 * n_layers - 1, "drop_rate": args.drop_rate,
             "zipf_s": args.zipf_s,
             "l2": "%s: features %.0f MB + graph arrays %.0f MB (all ranks), no flush between steps" % (
-                "inputs larger than L2" if V * layers[0] * 4 + E_total * 16 > 2 * 126e6 else
-                "inputs NOT larger than the 126 MB L2 (a test workload, not a bench line)",
+                "inputs larger than L2" if V * layers[0] * 4 + E_total * 16 > 2 * 50e6 else
+                "inputs NOT larger than the 50 MB L2 (a test workload, not a bench line)",
                 V * layers[0] * 4 / 1e6, E_total * 16 / 1e6)}
 
 
@@ -819,20 +851,6 @@ def _workload_name(name, V, E, layers, args=None):
         model = "%d-layer GAT, %d heads" % (len(layers) - 1, args.heads)
     return "%s-shaped synthetic power-law graph: %d V, %d E (incl. self loops), %s %s fp32" % (
         name, V, E, model, "-".join(str(x) for x in layers))
-
-
-def _ncu_traffic(F):
-    """dram bytes per call of the dominant kernel from the committed ncu capture of THIS round's kernel
-    (profiles/traffic.json: {"fwd_F602": {"bytes": ..., "kernel": ..., "source": ...}}), or None.  CUDA has no way to
-    read DRAM counters outside a profiler, so this is the one number of the line that is not measured live."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        d = json.load(open(p)).get("fwd_F%d" % F)
-        if d and "planned_gather_sum_kernel" in d.get("kernel", ""):
-            return {"bytes": float(d["bytes"]), "source": d.get("source")}
-    except Exception:
-        pass
-    return None
 
 
 if __name__ == "__main__":

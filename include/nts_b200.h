@@ -1,5 +1,5 @@
 /* nts_b200.h - C ABI of libnts_b200.so: NeutronStar's sparse neighbour-aggregation hot path,
- * hand-written for NVIDIA B200 (sm_100a).
+ * hand-written for NVIDIA H100 (sm_90a).
  *
  * This is the drop-in boundary.  Every entry point replaces one member of the reference's device
  * interface `cuda/ntsCUDA.hpp` (free functions :25-47, `deviceCSC` :49-95, `Cuda_Stream` :97-217,
@@ -285,7 +285,7 @@ int nts_aggregate_records(float *aggregate, const float *records, nts_vid_t n_re
                           nts_vid_t feature_size, nts_vid_t partition_start,
                           nts_vid_t partition_end, void *stream);
 
-/* ---- dense-row exchange helpers of the B200 engine (replace the record format on NVLink) -------------- */
+/* ---- dense-row exchange helpers of the exchange engine (replace the record format on NVLink) ----------- */
 /* dst[k,:] = src[rows[k],:]   (sender-side compaction of mirror rows / pull from a peer's mapped buffer) */
 int nts_gather_rows(float *dst, const float *src, const nts_vid_t *rows, nts_vid_t n_rows,
                     nts_vid_t feature_size, void *stream);

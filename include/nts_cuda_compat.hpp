@@ -6,7 +6,7 @@
 // (:97-217).  This header re-declares that surface - same names, same parameter order and meaning, same
 // "print and exit(1)" error convention (cuda/ntsCUDAGraphOP.cu:13-19) - as thin inline forwards to the C ABI of
 // libnts_b200.so (include/nts_b200.h), so that reference translation units compile and link unchanged while
-// every kernel they launch is the sm_100a implementation of this repository.
+// every kernel they launch is the sm_90a implementation of this repository.
 //
 // Not reproduced on purpose:
 //   * the reference's "_Optim" kernels overwrite instead of accumulate and overrun rows by one

@@ -1,9 +1,9 @@
-"""Build libnts_b200.so (hand-written sm_100a kernels + C ABI) in-tree with nvcc.
+"""Build libnts_b200.so (hand-written sm_90a kernels for H100 + C ABI) in-tree with nvcc.
 
     python -m neutronstarlite_b200.build [--force] [--verbose]
 
-The shared object lands in neutronstarlite_b200/lib/ (git-ignored, but it travels to the GPU box with the
-repository snapshot).  nvcc cross-compiles for sm_100a without a GPU.
+The shared object lands in neutronstarlite_b200/lib/ (git-ignored build product).  nvcc cross-compiles for sm_90a
+without a GPU.
 """
 from __future__ import annotations
 
@@ -23,8 +23,8 @@ CU_SOURCES = ["nts_runtime.cu", "nts_aggregate.cu", "nts_plan.cu", "nts_edge_ops
 CXX_SOURCES = ["nts_graph_host.cpp"]
 HEADERS = [os.path.join(CSRC, "nts_common.cuh"), os.path.join(ROOT, "include", "nts_b200.h")]
 
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + [
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "-Xcompiler", "-fopenmp",
@@ -59,7 +59,7 @@ def _run(cmd, verbose, log):
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA/C++ source for sm_100a and link libnts_b200.so. Returns the library path."""
+    """Compile every CUDA/C++ source for sm_90a and link libnts_b200.so. Returns the library path."""
     os.makedirs(OBJDIR, exist_ok=True)
     nvcc = _nvcc()
     log = []
@@ -81,7 +81,7 @@ def build(force=False, verbose=False):
                   "-c", s, "-o", o], verbose, log)
             relink = True
     if relink or not os.path.exists(LIB):
-        _run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB] + objs +
+        _run([nvcc] + ARCH + ["-shared", "-o", LIB] + objs +
              ["-Xcompiler", "-fopenmp", "-lgomp"], verbose, log)
     with open(os.path.join(LIBDIR, "build.log"), "a") as f:
         f.write("\n".join(log))

@@ -1,4 +1,4 @@
-// Segmented weighted gather-sum (the SpMM-like neighbour aggregation) for sm_100a.
+// Segmented weighted gather-sum (the SpMM-like neighbour aggregation) for sm_90a.
 //
 //   out[r,:] += sum_{e in [off[r], off[r+1])} in[src(e),:] * w[e]
 //
@@ -19,15 +19,15 @@
 //   variant 1 (shuffle): each lane loads one edge's (index, weight) coalesced, broadcast by __shfl.
 //   variant 2 (bulk):    one thread per CTA issues `cp.async.bulk` (TMA, SASS UBLKCP) copies of the
 //                        CTA's index and weight tiles into shared memory, completion on an mbarrier;
-//                        warps then read (index, weight) with broadcast LDS.  DEFAULT (15.5 vs 31.3 ms
-//                        on the F=602 Reddit-shaped launch; profiles/README.md).
+//                        warps then read (index, weight) with broadcast LDS.  DEFAULT (H100, F=602
+//                        Reddit-shaped launch: 26.4 vs 27.7 ms; F=128: 4.77 vs 4.93 ms).
 //
 // Template parameters of segment_gather_sum_kernel<VEC,K,U,BULK,MINB,HM>: VEC floats per lane load, K vector
 // chunks per lane (a warp covers 32*VEC*K columns per tile), U edges whose loads are issued before their FMAs,
 // BULK = variant 2, MINB = __launch_bounds__ min CTAs/SM (register cap), HM = head mode: 0 one weight per edge,
 // 1 the weight array is [E,H] and each lane picks its column's head, 2 the weight is recomputed on the fly from the
 // per-vertex attention scores and softmax statistics (the fused GAT layer, nts_edge_ops.cu K7).
-// (U, MINB) per shape come from the sweeps in profiles/tune_r1_*.jsonl; NTS_AGG_TUNE / NTS_AGG_TILES are
+// (U, MINB) per shape come from tools/tune_aggregate.py sweeps; NTS_AGG_TUNE / NTS_AGG_TILES are
 // measurement hooks read once at first launch, not product configuration.
 #include "nts_common.cuh"
 
@@ -174,7 +174,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MINB)
   // quantum / column tile owned by this warp.
   //   interleaved (tile_major = 0): consecutive warps = the column tiles of one quantum (they share index loads)
   //   tile-major  (tile_major = 1): all quanta of tile 0 first, then tile 1, ...: at any moment the CTAs in flight
-  //     touch one column slab of the feature matrix, which is sized to stay resident in the 126 MB L2.
+  //     touch one column slab of the feature matrix, which is sized to stay resident in the 50 MB L2.
   //     Warps per tile are padded to a multiple of the CTA size so a CTA never straddles two tiles.
   const uint64_t gwarp = (uint64_t)blockIdx.x * kVW + warp_in_block;
   // the launch covers edges [e_begin, n_edges64) of the arrays (e_begin = off[0]; 0 except for row-range launches)
@@ -440,14 +440,15 @@ static LaunchShape pick_shape(const float *in, const float *out, uint32_t F, uin
   s.tile_vecs = (nvec + s.tiles - 1) / s.tiles;
   s.k = (int)((s.tile_vecs + 31) / 32);
   s.tiles = (nvec + s.tile_vecs - 1) / s.tile_vecs;
-  // (U, min CTAs/SM): measured on B200 for the headline shapes (profiles/tune_r1_*.jsonl), generic rule otherwise
+  // (U, min CTAs/SM): measured on an H100 for the headline shapes (NTS_PLAN=0 tools/tune_aggregate.py, the
+  // Reddit-shaped graph), generic rule otherwise
   s.minb = 1;
   int budget = 40 / (s.k * s.vec);
   s.u = budget >= 8 ? 8 : (budget >= 4 ? 4 : 2);
-  if (s.vec == 2 && s.k == 5) { // F=602: 15.5 ms vs 16.4 (U=4) / 16.1 (U=2, 3 CTAs) on the Reddit-shaped graph
+  if (s.vec == 2 && s.k == 5) { // F=602: 26.4 ms vs 26.2 (U=4, 1 CTA) / 26.3 (U=4, 2 CTAs) / 27.1 (U=2, 3 CTAs)
     s.u = 2;
     s.minb = 2;
-  } else if (s.vec == 4 && s.k == 1) { // F=128: 3.48 ms vs 3.76 (U=8, 3 CTAs) / 4.65 (U=8, unconstrained)
+  } else if (s.vec == 4 && s.k == 1) { // F=128: 4.77 ms vs 6.0 (U=8, 4 CTAs) / 6.1 (U=8, 1 CTA) / 6.7 (U=16, 2)
     s.u = 4;
     s.minb = 4;
   }
@@ -568,7 +569,7 @@ static int segment_gather_sum(const float *in, float *out, const float *w, const
     if (att && s.k == 1 && s.tiles == 1 && F / s.vec <= 16 && !s.tile_major && !getenv("NTS_AGG_NO_SUBWARP"))
       s.g = 2;
   }
-  // edges per warp: multiple of 32; shrink for small inputs so the grid still fills 148 SMs
+  // edges per warp: multiple of 32; shrink for small inputs so the grid still fills every SM
   uint32_t Q = g_edges_per_warp > 0 ? (uint32_t)g_edges_per_warp : 512u / (uint32_t)s.g;
   if (g_edges_per_warp <= 0) {
     const uint64_t want_warps = (uint64_t)sm_count() * 64;
@@ -578,7 +579,7 @@ static int segment_gather_sum(const float *in, float *out, const float *w, const
   Q = (Q + 31u) & ~31u;
   if (s.g > 1 && Q * s.g > 1024) // the CTA's staged index span must keep fitting shared memory
     Q = (1024u / s.g) & ~31u;
-  int variant = g_variant == 0 ? 2 : g_variant; // measured on B200: bulk-staged indices are ~15-20% faster
+  int variant = g_variant == 0 ? 2 : g_variant; // measured on an H100: bulk-staged indices are ~3-5% faster
   bool bulk = variant == 2 && (att || heads <= 1); // [E, H] weight matrices are not bulk-staged
   // the bulk copies need 16-byte aligned index/weight arrays (cudaMalloc gives 256)
   if (bulk && !(aligned_to(idx, 16) && (!w || aligned_to(w, 16)))) {

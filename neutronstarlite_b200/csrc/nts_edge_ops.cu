@@ -1,4 +1,4 @@
-// Edge-granular operators of the GAT path for sm_100a: mirror/destination <-> edge-message copies,
+// Edge-granular operators of the GAT path for sm_90a: mirror/destination <-> edge-message copies,
 // per-destination edge softmax (multi-column, max-subtracted) and the fused-aggregation backward.
 //
 // Replaces cuda/ntsCUDADistKernel.cuh:23-95,166-260 and the `scatter_grad_back_to_messaage` kernel

@@ -72,7 +72,7 @@ struct nts_exchange {
   size_t bsend_cap = 0;
   cudaStream_t comm = nullptr;
   std::vector<cudaStream_t> dma;      // [P] one stream per peer for copy-engine pushes: the copies to different peers
-  std::vector<cudaEvent_t> ev_dma;    //     run on different copy engines at once (one engine alone reaches ~350 GB/s)
+  std::vector<cudaEvent_t> ev_dma;    //     run on different copy engines at once (one engine alone does not fill NVLink)
   std::vector<char> dma_used;         //     streams used by the current call (joined back into `comm` at its end)
   cudaEvent_t ev_main = nullptr, ev_comm = nullptr;
   std::vector<cudaEvent_t> ev_peer;   // backward: partial of chunk i finished
@@ -416,10 +416,11 @@ template <class Fn> static int time_launches(Fn run, cudaStream_t st, float *ms)
 }
 
 // Pipeline or merged?  One launch per source partition hides the transfer behind the earlier chunks, but small
-// launches run at a fraction of the large-launch rate (config B at 8 GPUs: 1.8 M-edge chunks take 2x their share);
+// launches run at a fraction of the large-launch rate (config B at 8 GPUs: 1.8 M-edge chunks);
 // one merged launch is efficient but can only start when ALL rows have landed.  Decided once per (direction, width)
 // from MEASURED launch times on scratch inputs (L = local chunk, c_i = remote chunks, M = merged launch) and the
-// transfer time T of the bytes this rank receives (forward) / sends (backward) at 600 GB/s:
+// transfer time T of the bytes this rank receives (forward) / sends (backward) at 300 GB/s
+// (two thirds of NVLink 4's 450 GB/s per direction on H100):
 //   forward : pipeline ~ L + max(sum c_i, T - L)        merged ~ max(L, T) + M
 //   backward: pipeline ~ sum c_i + max(L, T / (P-1))    merged ~ M + max(L, T)
 // Each rank decides for itself (it only changes how a rank consumes its own window / fills its own staging).
@@ -496,7 +497,7 @@ static int decide_mode(nts_exchange *ex, bool forward, uint32_t F, cudaStream_t 
     return rc;
   if (!ex->chunks[p].edges)
     L = 0.f;
-  const float T = (float)((double)(forward ? ex->recv_total : ex->recv_total) * F * 4.0 / 600e9 * 1e3); // ms
+  const float T = (float)((double)(forward ? ex->recv_total : ex->recv_total) * F * 4.0 / 300e9 * 1e3); // ms
   if (forward) {
     m.pipeline_ms = L + std::max(sum_c, T - L);
     m.merged_ms = std::max(L, T) + M;
@@ -969,7 +970,7 @@ static int return_impl(nts_exchange *ex, const float *gm, float *dx, nts_vid_t F
   return 0;
 }
 
-// Per-phase device timeline of forward calls (evidence for profiles/): enable, run ONE forward, read.
+// Per-phase device timeline of forward calls (bench.py exchange_timeline): enable, run ONE forward, read.
 int nts_exchange_set_trace(nts_exchange *ex, int enable) {
   NTS_ARG_CHECK(ex != nullptr, "null engine");
   if (enable && ex->tev.empty()) {

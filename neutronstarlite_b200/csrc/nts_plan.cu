@@ -4,12 +4,12 @@
 //   out[r,:] += sum_{e in [off[r], off[r+1])} in[row(e),:] * w[e]
 //
 // i.e. Cuda_Stream::Gather_By_Dst_From_Src / Gather_By_Src_From_Dst (cuda/ntsCUDAGraphOP.cu:157-281) - but with the
-// three things the ncu captures of round 1 asked for (profiles/README.md: the kernel is bound by the L1 data stage
-// every gathered byte crosses, and re-reads the feature matrix from DRAM 26 times):
+// three things a profile of that kernel asks for (it is bound by the L1 data stage every gathered byte crosses, and
+// re-reads the feature matrix from DRAM many times over):
 //
 //   1. source-slab bucketing.  Edges are regrouped by (slab of the gathered row, output row): slab s holds the
 //      edges whose gathered row lies in rows [s*slab_rows, (s+1)*slab_rows) of the input matrix, sized so that one
-//      slab of the matrix stays resident in the 126 MB L2.  One launch per slab, in stream order, so at any moment
+//      slab of the matrix stays resident in the 50 MB L2.  One launch per slab, in stream order, so at any moment
 //      the CTAs in flight gather from ONE slab; the output row of a (slab, row) segment is finished with a plain
 //      read-modify-write exactly like the unbucketed kernel (launches never overlap, so no extra atomics).
 //      The bucketing is a stable sort by (slab, row): inside a segment the edges keep the order of the reference
@@ -19,8 +19,7 @@
 //      interleaved, so the per-edge broadcast read from shared memory is ONE 8-byte LDS instead of two 4-byte ones,
 //      and the TMA bulk copy (cp.async.bulk -> SASS UBLKCP) stages one array per CTA instead of two.
 //   3. 16-byte feature loads for every width.  Rows whose byte length is not a multiple of 16 (F = 602: 2408 B) are
-//      copied once per call into a workspace with rows padded to a multiple of 4 floats (0.2 ms of HBM time at
-//      config B), so the gather always uses float4 loads on 16-byte aligned rows and one warp covers up to 640
+//      copied once per call into a workspace with rows padded to a multiple of 4 floats, so the gather always uses float4 loads on 16-byte aligned rows and one warp covers up to 640
 //      columns: 19 + 1 data-stage wavefronts per edge at F = 602 instead of 21.6 + 4.
 //
 // Plan construction (hand-written kernels + one CUB radix sort) replaces nothing in the reference: its chunks are
@@ -375,7 +374,8 @@ struct PlanShape;
 // each warp issues one cp.async.bulk (SASS UBLKCP) per edge that copies the row's tile (16-byte aligned thanks to the
 // padded workspace) into a per-warp ring of STAGES shared-memory buffers, completion on one mbarrier per stage; the
 // warp waits, reads its chunks with 16-byte LDS, accumulates, and re-arms the stage for edge e + STAGES.
-// Kept as variant 1 of nts_gather_plan_set_variant for measurement (profiles/): bulk copies bypass L1, which serves
+// Kept as variant 1 of nts_gather_plan_set_variant for measurement (tools/k1_sweep.py --tma; 3-10x slower than
+// variant 0 on an H100): bulk copies bypass L1, which serves
 // the hub rows of a skewed graph, and every gathered byte still crosses the shared-memory data stage once.
 template <int K, int STAGES, int OUTV, int MINB>
 __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
@@ -633,9 +633,9 @@ static int run_plan(nts_gather_plan *pl, const float *input, float *output, uint
     sh.g = 1;
   // (U, min CTAs/SM): U*K 16-byte loads in flight per lane
   // defaults = the largest U that compiles without spills at the occupancy point (ptxas -v); measured points for
-  // the headline shapes in profiles/ (tools/k1_sweep.py)
-  // (k = 5, F = 602: U=4 at 2 CTAs/SM 12.75 ms vs U=2 13.9 / U=1 at 3 CTAs 13.5; k = 1, F = 128: U=4 at 4 CTAs 2.90 ms
-  // vs U=8 at 3 CTAs 3.07 - profiles/k1_sweep_r2a.jsonl)
+  // the headline shapes measured on an H100 with tools/k1_sweep.py (unbucketed, Zipf graph of config B):
+  // k = 5, F = 602: U=4 at 2 CTAs/SM 24.9 ms vs U=1 at 3 CTAs 25.1 / U=4 at 1 CTA 27.1 / U=2 at 3 CTAs 32.7;
+  // k = 1, F = 128: U=4 at 4 CTAs 3.98 ms vs U=8 at 3 CTAs 4.37 / U=16 at 2 CTAs 5.5
   sh.minb = sh.k >= 3 ? 2 : (sh.k == 2 ? 3 : 4);
   sh.u = sh.k == 4 ? 2 : 4;
   {
@@ -713,7 +713,7 @@ extern "C" {
 int nts_gather_plan_pick_slabs(nts_vid_t gather_rows, uint64_t n_edges, nts_vid_t n_rows, nts_vid_t feature_size,
                                uint64_t l2_budget_bytes) {
   if (!l2_budget_bytes)
-    l2_budget_bytes = 40ull << 20; // a slab that stays resident next to the streamed outputs and index tiles
+    l2_budget_bytes = 16ull << 20; // a third of the 50 MB L2: the slab stays resident next to the streamed outputs
   const uint64_t bytes = (uint64_t)gather_rows * ((feature_size + 3u) & ~3u) * 4ull;
   uint64_t s = (bytes + l2_budget_bytes - 1) / l2_budget_bytes;
   // every (slab, row) segment costs one read-modify-write of the output row: keep >= 16 edges per segment on average
@@ -974,8 +974,8 @@ nts_gather_plan *nts_gather_plan_create_parts(const nts_plan_part *parts, int n_
 float nts_gather_plan_tuned_ms(const nts_gather_plan *pl) { return pl ? pl->tuned_ms : 0.f; }
 
 // Slab count by measurement.  Whether bucketing pays depends on how skewed the gathered rows are (hub sources stay in
-// L1/L2 by themselves: on the Zipf graph of config B one launch at F=602 takes 12.8 ms unbucketed, 20.9 ms with 14
-// slabs; with uniform endpoints 35.3 ms vs 16.9 ms) and on the degree distribution of the output rows (every non-empty
+// L1/L2 by themselves: on an H100, the Zipf graph of config B at F=602 takes 24.8 ms unbucketed, 19.5 ms with 4 slabs
+// and 25.5 ms with 16; with uniform endpoints 87.1 ms vs 39.0 ms at 16 slabs) and on the degree distribution of the output rows (every non-empty
 // (slab, row) segment costs a read-modify-write of the output row) - so the candidates 1, 2, 4, ... up to the
 // size-based bound are built and timed on the real arrays (zero features: the access pattern does not depend on the
 // values), 1 warm + 2 timed launches each, and the fastest is kept.  One-time cost per (chunk, direction, width).

@@ -28,11 +28,11 @@ int sm_count() {
   static int cached[64] = {0};
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64)
-    return 148;
+    return 132;
   if (cached[dev] == 0) {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148; // B200
+      n = 132; // H100 SXM
     cached[dev] = n;
   }
   return cached[dev];

@@ -1,4 +1,4 @@
-"""Device-resident partition-boundary exchange: the B200 replacement for the reference's host-staged MPI ring
+"""Device-resident partition-boundary exchange: the replacement for the reference's host-staged MPI ring
 (`Graph::sync_compute_decoupled` / `compute_sync_decoupled`, core/graph.hpp:3455-3719, and `NtsGraphCommunicator`,
 comm/network.cpp:159-844).
 

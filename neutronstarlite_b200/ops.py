@@ -3,7 +3,7 @@ constructed from `(PartitionedGraph, active)`, `forward(x)` / `forward(x, w)`, `
 `get_additional_grad()`; outputs are freshly allocated zero tensors the kernels accumulate into
 (NtsScheduler::NewKeyTensor / NewLeafTensor, core/NtsScheduler.hpp:378-394).
 
-Every operator calls the sm_100a kernels through the C ABI (`_lib.call`); tensors only provide device
+Every operator calls the sm_90a kernels through the C ABI (`_lib.call`); tensors only provide device
 memory and the current CUDA stream.  There is no CPU path: a CPU tensor raises.
 """
 from __future__ import annotations

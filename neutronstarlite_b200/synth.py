@@ -12,8 +12,10 @@ WORKLOADS = {
     # name: (V, E_random, layers)            SURVEY.md 8 preamble / 8d
     "reddit": (232965, 114615892, [602, 128, 41]),
     "products": (2449029, 61859140, [100, 128, 47]),
-    "papers100m": (111059956, 1615685872, [128, 128, 172]),   # config E: generated per partition (zipf_edges_owned)
-    "papers_eighth": (13882494, 201960734, [128, 128, 172]),  # one GPU's share of config E as a stand-alone graph
+    # config E: ogbn-papers100M's degree and widths at half its vertices and edges, so that one partition of 8 fits an
+    # 80 GB H100 next to its receive window (tools/plan_memory.py); generated per partition (zipf_edges_owned)
+    "papers100m": (55529978, 807842936, [128, 128, 172]),
+    "papers_eighth": (6941247, 100980367, [128, 128, 172]),   # one GPU's share of config E as a stand-alone graph
     "cora_sized": (2708, 10858, [1433, 128, 7]),
     "tiny": (20000, 400000, [602, 128, 41]),
 }

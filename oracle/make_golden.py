@@ -1,11 +1,12 @@
 #!/usr/bin/env python3
-"""TEST INFRASTRUCTURE ONLY - regenerate tests/golden/*.npz from the UNMODIFIED reference.
+"""TEST INFRASTRUCTURE ONLY - regenerate the golden vectors under tests/golden/ from the UNMODIFIED reference.
 
-Runs oracle/_ref/nts_ref_driver (built by `make -C oracle ref` from /root/reference) on
+Runs oracle/_ref/nts_ref_driver (built by `make -C oracle ref` from the reference sources) on
   * the reference's own Cora fixture (data/cora.2708.edge.self) at P = 1, 2, 4 ranks and
   * a small synthetic multigraph (hubs, duplicates, self loops, isolated vertices) at P = 1, 2, 3, 4, 8
-and packs every dumped artefact into one .npz per case.  Only runs in the build container
-(/root/reference must exist); the .npz files are committed so the GPU box never needs it.
+and packs every dumped artefact into tests/golden/<case>/, split over a few .npz parts (save_case) so that no
+stored file exceeds 1 MB.  Needs the reference sources (oracle/Makefile REF); the outputs are committed, so the
+tests never do.
 
     python oracle/make_golden.py            # all cases
 """
@@ -27,6 +28,33 @@ INT_U32 = {"partition_offset", "out_degree", "in_degree", "mirror_index", "whole
            "column_offset", "row_indices", "row_offset", "column_indices"}
 U8 = {"source_active", "has_mirror_at"}
 COPY_ONLY = {"scatter_src_msg", "scatter_dst_msg", "aggregate_dst_dmsg"}
+INPUTS = {"X", "G", "dep_Gm", "Ge", "softmax_in", "softmax_gout"}
+
+
+def _part(key):
+    base = key.split("/")[-1]
+    base = base.split("_", 1)[1] if base.startswith("chunk") else base
+    if key in ("edges", "case") or base in INT_U32 or base in U8 or base == "meta" or base.startswith("edge_weight"):
+        return "topology"
+    if base in INPUTS:
+        return "inputs"
+    return "copies" if base in COPY_ONLY else "outputs"
+
+
+def save_case(name, data):
+    """tests/golden/<name>/{topology,inputs,outputs,copies}.npz (tests/golden_store.py reads them back)."""
+    d = os.path.join(GOLD, name)
+    os.makedirs(d, exist_ok=True)
+    for f in os.listdir(d):
+        if f.endswith(".npz"):
+            os.remove(os.path.join(d, f))
+    parts = {}
+    for k, v in data.items():
+        parts.setdefault(_part(k), {})[k] = v
+    for part, arrays in parts.items():
+        dst = os.path.join(d, part + ".npz")
+        np.savez_compressed(dst, **arrays)
+        print("wrote", dst, "%.1f KB" % (os.path.getsize(dst) / 1024))
 
 
 def synth_edges(V=9216, E=20000, seed=0x5EED0001):
@@ -112,9 +140,7 @@ def run_case(name, edges, V, P, F, keep_copy_only, threads):
         data = parse_dump(out, P, F, keep_copy_only)
         data["edges"] = edges.astype(np.uint32)
         data["case"] = np.array([V, edges.shape[0], P, F], dtype=np.int64)
-        dst = os.path.join(GOLD, "%s_P%d_F%d.npz" % (name, P, F))
-        np.savez_compressed(dst, **data)
-        print("wrote", dst, "%.1f KB" % (os.path.getsize(dst) / 1024))
+        save_case("%s_P%d_F%d" % (name, P, F), data)
     finally:
         shutil.rmtree(work, ignore_errors=True)
 

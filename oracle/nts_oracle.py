@@ -6,7 +6,7 @@ This module is the *checker*.  Nothing under ``neutronstarlite_b200/`` imports i
 Every function restates one piece of iDC-NEU/NeutronStarLite (paths relative to the reference
 root) and cites the file:line it follows.  Parity is PINNED: ``tests/test_oracle_golden.py``
 checks every function here against golden vectors produced by the *unmodified* reference CPU
-operators (``oracle/_ref/nts_ref_driver``, built by ``oracle/Makefile`` from /root/reference,
+operators (``oracle/_ref/nts_ref_driver``, built by ``oracle/Makefile`` from the reference sources,
 run at P = 1, 2, 4, 8 ranks under the MPI stand-in of ``oracle/shim``) and committed under
 ``tests/golden/`` by ``oracle/make_golden.py``.
 

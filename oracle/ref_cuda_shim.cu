@@ -1,6 +1,6 @@
 // TEST / BENCH INFRASTRUCTURE ONLY.  extern "C" handles around the UNMODIFIED reference CUDA launchers
-// (cuda/ntsCUDAGraphOP.cu, compiled from /root/reference for sm_100a by oracle/Makefile into
-// oracle/_ref/libnts_refcuda.so) so that bench.py can time "the reference's own GPU kernels on a B200"
+// (cuda/ntsCUDAGraphOP.cu, compiled from the reference sources for sm_90a by oracle/Makefile into
+// oracle/_ref/libnts_refcuda.so) so that bench.py can time "the reference's own GPU kernels on an H100"
 // next to ours (BASELINE.md section 3, item 7).  Nothing here is part of the product.
 #define CUDA_ENABLE 1
 #include "ntsCUDA.hpp"

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY.  Op-level driver around the UNMODIFIED reference CPU
-// path.  It is compiled against the headers where they lie in /root/reference
+// path.  It is compiled against the reference headers where they lie (REF of oracle/Makefile)
 // (nothing is copied into this repository) by oracle/Makefile, output goes to
 // oracle/_ref/.  It loads an edge file exactly as toolkits/main.cpp:44-54 does,
 // builds the PartitionedGraph exactly as toolkits/GAT_CPU_DIST.hpp:67-74 does,

@@ -1,9 +1,7 @@
 """pytest configuration: markers, import path, golden-vector loader."""
-import glob
 import os
 import sys
 
-import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -13,26 +11,25 @@ ORACLE_DIR = os.path.join(ROOT, "oracle")
 if ORACLE_DIR not in sys.path:
     sys.path.insert(0, ORACLE_DIR)
 
-GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
+import golden_store  # noqa: E402
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 class Golden:
     """One reference run: integer artefacts and operator results of P ranks (oracle/make_golden.py)."""
 
-    def __init__(self, path):
-        self.path = path
-        self.name = os.path.basename(path)[:-4]
-        z = np.load(path)
+    def __init__(self, name):
+        z = golden_store.load(name)
+        self.name = z.name
         self._z = z
         self.V, self.E, self.P, self.F = (int(x) for x in z["case"])
         self.edges = z["edges"]
 
     def has(self, rank, key):
-        return ("r%d/%s" % (rank, key)) in self._z.files
+        return ("r%d/%s" % (rank, key)) in self._z
 
     def get(self, rank, key):
         return self._z["r%d/%s" % (rank, key)]
@@ -46,10 +43,6 @@ class Golden:
         return self.get(0, "partition_offset")
 
 
-def golden_paths():
-    return sorted(glob.glob(os.path.join(GOLDEN_DIR, "*.npz")))
-
-
-@pytest.fixture(params=golden_paths(), ids=lambda p: os.path.basename(p)[:-4])
+@pytest.fixture(params=golden_store.case_names())
 def golden(request):
     return Golden(request.param)

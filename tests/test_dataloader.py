@@ -1,19 +1,28 @@
-"""GNNDatum host loader (SURVEY 8 f3) on the reference's own Cora tables (oracle/_ref/data, copied there from
-/root/reference/data by oracle/Makefile): the parallel parser must give exactly what a record-by-record read of the
+"""GNNDatum host loader (SURVEY 8 f3) on the reference's own Cora tables (stored gzipped under tests/golden/cora_tables,
+unpacked into a temporary directory): the parallel parser must give exactly what a record-by-record read of the
 text tables gives (the contract of core/ntsDataloador.hpp:156-221), for the whole graph and for a partition's rows; a
 packed binary table must round-trip."""
+import gzip
 import os
+import shutil
 
 import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DATA = os.path.join(ROOT, "oracle", "_ref", "data")
-needs_data = pytest.mark.skipif(not os.path.exists(os.path.join(DATA, "cora.featuretable")),
-                                reason="oracle/_ref/data absent (make -C oracle ref copies the reference's Cora fixture)")
+TABLES = os.path.join(ROOT, "tests", "golden", "cora_tables")
 
 
-def _reference_read(V, F):
+@pytest.fixture(scope="module")
+def cora_dir(tmp_path_factory):
+    d = tmp_path_factory.mktemp("cora")
+    for name in ("cora.featuretable", "cora.labeltable", "cora.mask"):
+        with gzip.open(os.path.join(TABLES, name + ".gz"), "rb") as src, open(d / name, "wb") as dst:
+            shutil.copyfileobj(src, dst)
+    return str(d)
+
+
+def _reference_read(DATA, V, F):
     """Record by record, like the reference's three istreams."""
     feats = np.zeros((V, F), dtype=np.float32)
     labels = np.zeros(V, dtype=np.int64)
@@ -32,11 +41,11 @@ def _reference_read(V, F):
     return feats, labels, masks
 
 
-@needs_data
-def test_text_tables_match_a_record_by_record_read():
+def test_text_tables_match_a_record_by_record_read(cora_dir):
     from neutronstarlite_b200.dataloader import GNNDatum
+    DATA = cora_dir
     V, F = 2708, 1433
-    feats, labels, masks = _reference_read(V, F)
+    feats, labels, masks = _reference_read(DATA, V, F)
     d = GNNDatum(F, 7, 0, V).readFeature_Label_Mask(os.path.join(DATA, "cora.featuretable"),
                                                     os.path.join(DATA, "cora.labeltable"),
                                                     os.path.join(DATA, "cora.mask"))

@@ -7,6 +7,7 @@ the reference run at the same P.  The CUDA data path itself is covered by tests/
 import os
 import sys
 
+import golden_store
 import numpy as np
 import pytest
 import torch
@@ -14,7 +15,6 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
 
 
 def _gather_sum(offsets, idx, w, X, n_rows):
@@ -115,7 +115,7 @@ def _worker(rank, world, port, case, q):
     try:
         from neutronstarlite_b200.exchange import ExchangePlan
         from neutronstarlite_b200.graph import HostGraph, PartitionedGraph
-        z = np.load(os.path.join(GOLD, case))
+        z = golden_store.load(case)
         V, E, P, F = (int(x) for x in z["case"])
         assert P == world
         hg = HostGraph(z["edges"], V)

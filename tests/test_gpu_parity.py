@@ -1,4 +1,4 @@
-"""Parity of the sm_100a kernels, called through the C ABI, against
+"""Parity of the sm_90a kernels, called through the C ABI, against
   (1) the golden vectors of the UNMODIFIED reference CPU operators (tests/golden, P = 1, 2, 4, 8),
   (2) the C / numpy oracle on seeded random multigraphs (hubs, empty rows, duplicates; every vector-width class),
   (3) size-independent properties at larger sizes (exact in-degree counts, linearity).

@@ -119,9 +119,9 @@ def test_gat_epoch_matches_torch_autograd(heads, fused_kernel):
     model.Update()
 
 
-def test_bench_prints_the_contract_line_on_a_tiny_workload():
+def test_bench_prints_the_contract_line_on_a_tiny_workload(tmp_path):
     """`bench.py` (our arm) end to end on the tiny workload: one JSON line with every key of the bench contract,
-    kernels of libnts_b200 actually launched, roofline and e2e present."""
+    kernels of libnts_b200 actually launched, roofline and e2e present, and the last timed step's outputs dumped."""
     import json
     import os
     import subprocess
@@ -129,7 +129,8 @@ def test_bench_prints_the_contract_line_on_a_tiny_workload():
     dev()
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     out = subprocess.run([sys.executable, os.path.join(root, "bench.py"), "--workload", "tiny", "--steps", "3",
-                          "--warmup", "3", "--no-cpu-baseline", "--no-ref-gpu"], stdout=subprocess.PIPE,
+                          "--warmup", "3", "--no-cpu-baseline", "--no-ref-gpu", "--dump-outputs", str(tmp_path)],
+                         stdout=subprocess.PIPE,
                          stderr=subprocess.PIPE, text=True, timeout=600)
     assert out.returncode == 0, out.stderr[-1500:]
     line = json.loads(out.stdout.strip().splitlines()[-1])
@@ -139,3 +140,8 @@ def test_bench_prints_the_contract_line_on_a_tiny_workload():
     assert line["gpu_launches"] >= 9 and line["value"] > 0
     assert line["e2e"]["h2d_bytes_per_step"] > 0 and line["e2e"]["d2h_bytes_per_step"] > 0
     assert line["roofline"]["bound"] == "hbm" and line["roofline"]["achieved"] > 0
+    import numpy as np
+    out = np.load(tmp_path / "output.npy")
+    loss = np.load(tmp_path / "loss.npy")
+    assert out.shape == (20000, 41) and out.dtype == np.float32 and np.isfinite(out).all()
+    assert loss.shape == (1,) and np.isfinite(loss).all() and loss[0] > 0

@@ -1,5 +1,5 @@
 """The numpy restatement (oracle/nts_oracle.py) against the golden vectors dumped by the UNMODIFIED
-reference CPU operators (tests/golden/*.npz, produced by oracle/make_golden.py at P = 1, 2, 4, 8).
+reference CPU operators (tests/golden/<case>/, produced by oracle/make_golden.py at P = 1, 2, 4, 8).
 Integer artefacts must be bit-exact; float results within 2e-6 relative of the reference's own
 CPU result (same summation order, FMA contraction is the only freedom)."""
 import numpy as np

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Per-GPU HBM budget of the distributed aggregation path for a graph shape (no GPU needed): which arrays live on a
-rank, how large they are, and whether the shape fits 180 GB.  Upper bounds where the exact number depends on the graph
+rank, how large they are, and whether the shape fits an 80 GB H100.  Upper bounds where the exact number depends on the graph
 (distinct remote sources of a rank <= V - V_p).
 
     python tools/plan_memory.py --V 111059956 --E 1616000000 --layers 128-128-172 --gpus 8
@@ -9,7 +9,7 @@ import argparse
 import json
 
 
-def plan(V, E, layers, P, hbm_gb=180.0, slabs=1, n_buffers=2):
+def plan(V, E, layers, P, hbm_gb=80.0, slabs=1, n_buffers=2):
     Vp = -(-V // P)                      # vertices of a rank (balanced by the partitioner up to 1024-alignment)
     Ep = -(-(E + V) // P)                # in-edges of a rank incl. self loops (mean; skew adds up to ~1.25x at P=8)
     local = Ep // P                      # edges whose source is local (uniform estimate)
