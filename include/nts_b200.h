@@ -119,8 +119,18 @@ int nts_gather_plan_pick_slabs(nts_vid_t gather_rows, uint64_t n_edges, nts_vid_
 nts_gather_plan *nts_gather_plan_create(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
                                         const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows,
                                         uint64_t n_edges, nts_vid_t gather_rows, int n_slabs, void *stream);
+/* The same with up to two dense FP32 hub blocks beside the slab-bucketed residual: the n_hub_cols most referenced
+ * gathered rows (ties: smaller id) become a column block [n_rows x n_hub_cols] that takes every edge gathering one of
+ * them, the n_hub_rows longest output rows a row block [n_hub_rows x gather_rows] that takes their remaining edges;
+ * each dense cell holds the sum of its edges' weights.  A run computes the blocks as GEMMs before the slab launches.
+ * Counts above the rows available are clamped (nts_gather_plan_hubs reports the result); 0, 0 = nts_gather_plan_create. */
+nts_gather_plan *nts_gather_plan_create_hybrid(const nts_vid_t *offsets, const nts_vid_t *indices,
+                                               const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
+                                               nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows, int n_slabs,
+                                               int n_hub_cols, int n_hub_rows, void *stream);
 /* slab count chosen by MEASUREMENT on the real arrays at this feature width (candidates 1, 2, 4, ... built and timed
- * once; hub-dominated graphs prefer no bucketing, uniform ones 8-16 slabs) */
+ * once; hub-dominated graphs prefer no bucketing, uniform ones 8-16 slabs), then the hub counts of
+ * nts_gather_plan_create_hybrid the same way among rows dense enough to be candidates (NTS_PLAN_HUBS=0: none) */
 nts_gather_plan *nts_gather_plan_create_tuned(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
                                               const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows,
                                               uint64_t n_edges, nts_vid_t gather_rows, nts_vid_t feature_size,
@@ -140,6 +150,7 @@ nts_gather_plan *nts_gather_plan_create_parts(const nts_plan_part *parts, int n_
 float nts_gather_plan_tuned_ms(const nts_gather_plan *plan); /* time of the winning candidate of a measured plan */
 int nts_gather_plan_destroy(nts_gather_plan *plan);
 int nts_gather_plan_slabs(const nts_gather_plan *plan);
+int nts_gather_plan_hubs(const nts_gather_plan *plan, int *cols, int *rows); /* hub columns / rows of the plan */
 uint64_t nts_gather_plan_bytes(const nts_gather_plan *plan);
 /* output[r,:] += sum_e input[row(e),:] * w(e)   (accumulates; one launch per non-empty slab, in stream order) */
 int nts_gather_plan_run(nts_gather_plan *plan, const float *input, float *output, nts_vid_t feature_size,

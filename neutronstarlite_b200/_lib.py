@@ -51,11 +51,13 @@ SIGNATURES = {
     "nts_segment_gather_sum_range": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _u64, _u64, _u32, _vp]),
     "nts_gather_plan_pick_slabs": (_int, [_u32, _u64, _u32, _u32, _u64]),
     "nts_gather_plan_create": (_vp, [_vp, _vp, _vp, _vp, _u32, _u32, _u64, _u32, _int, _vp]),
+    "nts_gather_plan_create_hybrid": (_vp, [_vp, _vp, _vp, _vp, _u32, _u32, _u64, _u32, _int, _int, _int, _vp]),
     "nts_gather_plan_create_tuned": (_vp, [_vp, _vp, _vp, _vp, _u32, _u32, _u64, _u32, _u32, _vp]),
     "nts_gather_plan_create_parts": (_vp, [_vp, _int, _u32, _u32, _int, _u32, _vp]),
     "nts_gather_plan_tuned_ms": (C.c_float, [_vp]),
     "nts_gather_plan_destroy": (_int, [_vp]),
     "nts_gather_plan_slabs": (_int, [_vp]),
+    "nts_gather_plan_hubs": (_int, [_vp, C.POINTER(_int), C.POINTER(_int)]),
     "nts_gather_plan_bytes": (_u64, [_vp]),
     "nts_gather_plan_run": (_int, [_vp, _vp, _vp, _u32, _vp]),
     "nts_gather_plan_last_launch": (_int, [_vp] + [C.POINTER(_int)] * 5),

@@ -380,8 +380,11 @@ static int aggregate_chunk(nts_exchange *ex, int i, bool forward, const float *i
       pl = nts_gather_plan_create_tuned(off, idx, w, nullptr, base, n_rows, c.edges, gather_rows, F, st);
       if (!pl)
         return -1;
-      for (auto &e : plans) // another width settled on the same slab count: share its arrays
-        if (nts_gather_plan_slabs(e.second) == nts_gather_plan_slabs(pl)) {
+      int hc = 0, hr = 0, ehc = 0, ehr = 0;
+      nts_gather_plan_hubs(pl, &hc, &hr);
+      for (auto &e : plans) // another width settled on the same slab and hub counts: share its arrays
+        if (nts_gather_plan_slabs(e.second) == nts_gather_plan_slabs(pl) &&
+            nts_gather_plan_hubs(e.second, &ehc, &ehr) == 0 && ehc == hc && ehr == hr) {
           nts_gather_plan_destroy(pl);
           pl = e.second;
           break;

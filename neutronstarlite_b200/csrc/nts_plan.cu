@@ -42,6 +42,13 @@ struct nts_gather_plan {
   std::vector<uint64_t> slab_edge; // [slabs + 1] host copy of voff[s * n_rows]
   float *workspace = nullptr;  // padded copy of the input when its rows are not 16-byte multiples / aligned
   size_t workspace_floats = 0;
+  // dense hub blocks (nts_gather_plan_create_hybrid); the slab-bucketed pairs hold the remaining edges only
+  int hub_cols = 0, hub_rows = 0;
+  uint32_t *hub_col_ids = nullptr; // [hub_cols] gathered rows of the column block, most referenced first
+  uint32_t *hub_row_ids = nullptr; // [hub_rows] output rows of the row block, longest segment first
+  uint32_t lda_c = 0, lda_r = 0;   // n_rows / hub_rows rounded up to a multiple of 4 (16-byte operand rows)
+  float *dense = nullptr;          // D_c^T [hub_cols x lda_c], then D_r^T [gather_rows x lda_r]: summed edge weights
+  size_t dense_floats = 0;
   int last_grid = 0, last_launches = 0, last_k = 0, last_u = 0, last_outv = 0;
   float tuned_ms = 0.f;        // nts_gather_plan_create_tuned: time of the winning candidate
 };
@@ -120,18 +127,84 @@ __global__ void plan_permute_pairs_kernel(const uint32_t *__restrict__ perm, con
 }
 
 // voff[k] = number of sorted keys < k, k in [0, n_keys]
-__global__ void plan_offsets_kernel(const uint32_t *__restrict__ sorted_key, uint32_t n_edges, uint32_t n_keys,
+template <class KeyT>
+__global__ void plan_offsets_kernel(const KeyT *__restrict__ sorted_key, uint32_t n_edges, uint32_t n_keys,
                                     uint32_t *__restrict__ voff) {
   for (uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; k <= n_keys; k += (uint64_t)gridDim.x * blockDim.x) {
     uint32_t lo = 0, hi = n_edges; // first position with key >= k
     while (lo < hi) {
       uint32_t mid = lo + ((hi - lo) >> 1);
-      if (__ldg(sorted_key + mid) < (uint32_t)k)
+      if (__ldg(sorted_key + mid) < (KeyT)k)
         lo = mid + 1;
       else
         hi = mid;
     }
     voff[k] = lo;
+  }
+}
+
+// ---- hub blocks (nts_gather_plan_create_hybrid) --------------------------------------------------------------------
+constexpr uint32_t kNoHub = 0xffffffffu;
+
+// cnt[g] = number of edges that gather row g (integer atomics: the counts are exact and order-independent)
+__global__ void plan_ref_count_kernel(const uint32_t *__restrict__ idx, const uint32_t *__restrict__ slot_of,
+                                      uint32_t base, uint32_t n_edges, uint32_t *__restrict__ cnt) {
+  for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n_edges; e += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t id = __ldg(idx + e);
+    atomicAdd(cnt + (slot_of ? __ldg(slot_of + id) : id - base), 1u);
+  }
+}
+
+// 64-bit key per edge: an edge whose gathered row is a hub column goes to cell (slot, row) of the column block D_c^T
+// [hub_cols x lda_c]; else an edge of a hub row goes to cell (gathered row, slot) of the row block D_r^T
+// [gather_rows x lda_r]; both as n_keys + the cell's offset in the dense buffer, so they sort past every residual
+// (slab, row) key and voff[n_keys] is the residual edge count.
+__global__ void plan_hybrid_keys_kernel(const uint32_t *__restrict__ off, const uint32_t *__restrict__ idx,
+                                        const uint32_t *__restrict__ slot_of, uint32_t base, uint32_t n_rows,
+                                        uint32_t n_edges, uint32_t slab_rows, uint32_t slabs,
+                                        const uint32_t *__restrict__ col_slot, const uint32_t *__restrict__ row_slot,
+                                        uint32_t lda_c, uint64_t dc_cells, uint32_t lda_r, uint64_t *__restrict__ key,
+                                        uint32_t *__restrict__ val) {
+  const uint64_t n_keys = (uint64_t)slabs * n_rows;
+  for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n_edges; e += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t r = plan_find_row(off, n_rows, (uint32_t)e);
+    const uint32_t id = __ldg(idx + e);
+    const uint32_t g = slot_of ? __ldg(slot_of + id) : id - base;
+    const uint32_t cs = __ldg(col_slot + g), rs = __ldg(row_slot + r);
+    uint64_t k;
+    if (cs != kNoHub) {
+      k = n_keys + (uint64_t)cs * lda_c + r;
+    } else if (rs != kNoHub) {
+      k = n_keys + dc_cells + (uint64_t)g * lda_r + rs;
+    } else {
+      uint32_t s = g / slab_rows;
+      if (s >= slabs)
+        s = slabs - 1;
+      k = (uint64_t)s * n_rows + r;
+    }
+    key[e] = k;
+    val[e] = (uint32_t)e;
+  }
+}
+
+// One warp per run of equal dense keys (a cell): dense[key - n_keys] = sum of the run's weights, lane-strided partial
+// sums then a fixed butterfly, so two builds give bit-identical cells.
+__global__ void plan_cell_sum_kernel(const uint64_t *__restrict__ cell_key, const uint32_t *__restrict__ run_start,
+                                     const uint32_t *__restrict__ run_len, uint32_t n_runs,
+                                     const uint32_t *__restrict__ perm, const float *__restrict__ w, uint64_t n_keys,
+                                     float *__restrict__ dense) {
+  const uint32_t lane = threadIdx.x & 31;
+  for (uint64_t run = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; run < n_runs;
+       run += ((uint64_t)gridDim.x * blockDim.x) >> 5) {
+    const uint32_t b = __ldg(run_start + run), n = __ldg(run_len + run);
+    float s = 0.f;
+    for (uint32_t j = lane; j < n; j += 32)
+      s += w ? __ldg(w + __ldg(perm + b + j)) : 1.f;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1)
+      s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0)
+      dense[__ldg(cell_key + run) - n_keys] = s;
   }
 }
 
@@ -597,6 +670,134 @@ static int launch_planned_tma(nts_gather_plan *pl, const PlanShape &sh, const fl
     return launch_planned<K_, U_, 1, B_>(pl, sh, in4, ld4, out, F, Q, st);                                           \
   }
 
+// ---- dense hub blocks: FP32 SIMT GEMM (FFMA only, no tensor cores) ----------------------------------------------------
+//   out[rowmap(m), n] += sum_{k in this CTA's K range} At[k, m] * B[colmap(k), n]      m < M, n < F
+// At is the block stored K-major ([K x lda], lda % 4 == 0, columns M..lda zero), B rows are ldb floats, 16-byte
+// aligned and zero past F (the input or the padded workspace), so both operand tiles are rows of 16-byte chunks that
+// cp.async copies straight into double-buffered shared memory (zero-filled past the edges).  128 x 128 x 16 tiles,
+// 256 threads, 8 x 8 outputs per thread.  Column block: colmap = hub columns, rowmap = identity, one CTA per output
+// tile -> plain read-modify-write.  Row block: colmap = identity, rowmap = hub rows, split-K -> vector red.
+// blockIdx.x = (split * m_tiles + m_tile) * n_tiles + n_tile: the N tiles of one A tile run back to back (A from L2).
+constexpr int kHubBM = 128, kHubBN = 128, kHubBK = 16, kHubThreads = 256;
+
+__device__ __forceinline__ void p_cp_async16(void *smem_dst, const void *gmem_src, bool full) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(p_smem_u32(smem_dst)), "l"(gmem_src),
+               "r"(full ? 16 : 0)
+               : "memory");
+}
+
+template <int OUTV, bool SPLIT>
+__global__ void __launch_bounds__(kHubThreads, 2)
+    hub_block_gemm_kernel(const float *__restrict__ At, uint32_t lda, uint32_t M, uint32_t K, uint32_t k_split,
+                          const float *__restrict__ B, uint32_t ldb, const uint32_t *__restrict__ colmap,
+                          float *__restrict__ out, uint32_t F, const uint32_t *__restrict__ rowmap, uint32_t m_tiles,
+                          uint32_t n_tiles) {
+  __shared__ __align__(16) float As[2][kHubBK][kHubBM];
+  __shared__ __align__(16) float Bs[2][kHubBK][kHubBN];
+  const uint32_t t = threadIdx.x;
+  const uint32_t n_tile = blockIdx.x % n_tiles, rest = blockIdx.x / n_tiles;
+  const uint32_t m0 = (rest % m_tiles) * kHubBM, n0 = n_tile * kHubBN;
+  const uint32_t k_begin = (rest / m_tiles) * k_split;
+  const uint32_t k_end = min(K, k_begin + k_split);
+  if (k_begin >= k_end)
+    return;
+  const uint32_t n_kt = (k_end - k_begin + kHubBK - 1) / kHubBK;
+
+  auto load = [&](uint32_t kt, int buf) {
+#pragma unroll
+    for (int i = 0; i < 2; i++) { // 512 16-byte chunks per operand tile, 2 per thread
+      const uint32_t c = t + i * kHubThreads, kk = c >> 5, c4 = (c & 31) * 4;
+      const uint32_t k = k_begin + kt * kHubBK + kk;
+      const bool kin = k < k_end;
+      const bool a_ok = kin && m0 + c4 < lda;
+      p_cp_async16(&As[buf][kk][c4], a_ok ? At + (size_t)k * lda + m0 + c4 : At, a_ok);
+      const bool b_ok = kin && n0 + c4 < ldb;
+      const uint32_t brow = b_ok ? (colmap ? __ldg(colmap + k) : k) : 0;
+      p_cp_async16(&Bs[buf][kk][c4], B + (size_t)brow * ldb + (b_ok ? n0 + c4 : 0), b_ok);
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+
+  const uint32_t tx = t & 15, ty = t >> 4;
+  float acc[8][8];
+#pragma unroll
+  for (int i = 0; i < 8; i++)
+#pragma unroll
+    for (int j = 0; j < 8; j++)
+      acc[i][j] = 0.f;
+
+  load(0, 0);
+  for (uint32_t kt = 0; kt < n_kt; kt++) {
+    const int buf = kt & 1;
+    if (kt + 1 < n_kt) {
+      load(kt + 1, buf ^ 1);
+      asm volatile("cp.async.wait_group 1;" ::: "memory");
+    } else {
+      asm volatile("cp.async.wait_group 0;" ::: "memory");
+    }
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < kHubBK; kk++) {
+      const float4 a0 = *reinterpret_cast<const float4 *>(&As[buf][kk][ty * 4]);
+      const float4 a1 = *reinterpret_cast<const float4 *>(&As[buf][kk][64 + ty * 4]);
+      const float4 b0 = *reinterpret_cast<const float4 *>(&Bs[buf][kk][tx * 4]);
+      const float4 b1 = *reinterpret_cast<const float4 *>(&Bs[buf][kk][64 + tx * 4]);
+      const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+      const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+      for (int i = 0; i < 8; i++)
+#pragma unroll
+        for (int j = 0; j < 8; j++)
+          acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+    }
+    __syncthreads();
+  }
+
+#pragma unroll
+  for (int i = 0; i < 8; i++) {
+    const uint32_t m = m0 + (i >> 2) * 64 + ty * 4 + (i & 3);
+    if (m >= M)
+      continue;
+    float *orow = out + (size_t)(rowmap ? __ldg(rowmap + m) : m) * F;
+#pragma unroll
+    for (int j = 0; j < 2; j++) {
+      const uint32_t col = n0 + j * 64 + tx * 4;
+      if (col < F)
+        flush_chunk<OUTV, SPLIT>(orow, col, F,
+                                 make_float4(acc[i][j * 4], acc[i][j * 4 + 1], acc[i][j * 4 + 2], acc[i][j * 4 + 3]));
+    }
+  }
+}
+
+template <int OUTV>
+static int launch_hub_blocks(nts_gather_plan *pl, const float *in, uint32_t ldb, float *out, uint32_t F,
+                             cudaStream_t st) {
+  const uint32_t n_tiles = (F + kHubBN - 1) / kHubBN;
+  if (pl->hub_cols) { // column block: M = n_rows, K = hub_cols
+    const uint32_t m_tiles = (pl->n_rows + kHubBM - 1) / kHubBM;
+    const uint64_t blocks = (uint64_t)m_tiles * n_tiles;
+    NTS_ARG_CHECK(blocks <= 0x7fffffffull, "hub column block grid too large");
+    hub_block_gemm_kernel<OUTV, false><<<(unsigned)blocks, kHubThreads, 0, st>>>(
+        pl->dense, pl->lda_c, pl->n_rows, (uint32_t)pl->hub_cols, (uint32_t)pl->hub_cols, in, ldb, pl->hub_col_ids, out,
+        F, nullptr, m_tiles, n_tiles);
+    NTS_LAUNCH_CHECK();
+  }
+  if (pl->hub_rows) { // row block: M = hub_rows, K = gather_rows, split so that about 4 waves of CTAs fill the SMs
+    const uint32_t m_tiles = (pl->hub_rows + kHubBM - 1) / kHubBM;
+    const uint32_t K = pl->gather_rows;
+    const uint64_t want = (uint64_t)sm_count() * 2 * 4;
+    uint64_t splits = (want + (uint64_t)m_tiles * n_tiles - 1) / ((uint64_t)m_tiles * n_tiles);
+    uint32_t k_split = (uint32_t)((K + splits - 1) / splits);
+    k_split = std::max<uint32_t>((k_split + kHubBK - 1) / kHubBK * kHubBK, 16 * kHubBK);
+    splits = (K + k_split - 1) / k_split;
+    hub_block_gemm_kernel<OUTV, true><<<(unsigned)(splits * m_tiles * n_tiles), kHubThreads, 0, st>>>(
+        pl->dense + (size_t)pl->hub_cols * pl->lda_c, pl->lda_r, (uint32_t)pl->hub_rows, K, k_split, in, ldb, nullptr,
+        out, F, pl->hub_row_ids, m_tiles, n_tiles);
+    NTS_LAUNCH_CHECK();
+  }
+  return 0;
+}
+
 static int run_plan(nts_gather_plan *pl, const float *input, float *output, uint32_t F, cudaStream_t st) {
   if (pl->n_rows == 0 || pl->n_edges == 0 || F == 0)
     return 0;
@@ -628,6 +829,13 @@ static int run_plan(nts_gather_plan *pl, const float *input, float *output, uint
   sh.k = (int)((sh.tile_vecs + 31) / 32);
   sh.tiles = (ld4 + sh.tile_vecs - 1) / sh.tile_vecs;
   sh.outv = (F % 4 == 0 && aligned_to(output, 16)) ? 4 : ((F % 2 == 0 && aligned_to(output, 8)) ? 2 : 1);
+  if (pl->hub_cols || pl->hub_rows) { // dense blocks first, then the residual edges' slab launches (stream order)
+    const int rc = sh.outv == 4   ? launch_hub_blocks<4>(pl, in, ld, output, F, st)
+                   : sh.outv == 2 ? launch_hub_blocks<2>(pl, in, ld, output, F, st)
+                                  : launch_hub_blocks<1>(pl, in, ld, output, F, st);
+    if (rc)
+      return rc;
+  }
   sh.g = ld4 <= 8 ? 4 : (ld4 <= 16 ? 2 : 1); // rows narrower than half / a quarter of a warp: virtual warps
   if (g_plan_variant == 1 || getenv("NTS_PLAN_NO_SUBWARP"))
     sh.g = 1;
@@ -652,7 +860,7 @@ static int run_plan(nts_gather_plan *pl, const float *input, float *output, uint
   }
   uint32_t Q = g_plan_q > 0 ? (uint32_t)g_plan_q : 512u / sh.g; // the CTA's staged span stays 8 * 512 pairs
   if (g_plan_q <= 0) { // shrink for small inputs so every slab launch still fills the SMs
-    const uint64_t per_slab = pl->n_edges / (uint64_t)pl->slabs + 1;
+    const uint64_t per_slab = pl->slab_edge[pl->slabs] / (uint64_t)pl->slabs + 1; // residual edges (no hub blocks)
     const uint64_t want_warps = (uint64_t)sm_count() * 64 * sh.g;
     while (Q > 32 && ((per_slab + Q - 1) / Q) * sh.tiles < want_warps)
       Q >>= 1;
@@ -725,9 +933,162 @@ int nts_gather_plan_pick_slabs(nts_vid_t gather_rows, uint64_t n_edges, nts_vid_
   return s < 1 ? 1 : (int)s;
 }
 
+// Exact reference counts of the gathered rows and segment lengths of the output rows, on the host.
+static bool hub_counts(const nts_vid_t *offsets, const nts_vid_t *indices, const nts_vid_t *slot_of, nts_vid_t base,
+                       uint32_t n_rows, uint32_t E, uint32_t gather_rows, std::vector<uint32_t> &col_cnt,
+                       std::vector<uint32_t> &seg, cudaStream_t st) {
+  uint32_t *cnt = nullptr;
+  std::vector<uint32_t> off(n_rows + 1);
+  col_cnt.assign(gather_rows, 0);
+  const unsigned blocks = (unsigned)std::min<uint64_t>(((uint64_t)E + 255) / 256, (uint64_t)sm_count() * 32);
+  bool ok = cudaMalloc(reinterpret_cast<void **>(&cnt), (size_t)gather_rows * 4) == cudaSuccess &&
+            cudaMemsetAsync(cnt, 0, (size_t)gather_rows * 4, st) == cudaSuccess;
+  if (ok && E) {
+    plan_ref_count_kernel<<<blocks, 256, 0, st>>>(indices, slot_of, base, E, cnt);
+    count_launch();
+  }
+  ok = ok && cudaMemcpyAsync(col_cnt.data(), cnt, (size_t)gather_rows * 4, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+       cudaMemcpyAsync(off.data(), offsets, ((size_t)n_rows + 1) * 4, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+       cudaStreamSynchronize(st) == cudaSuccess;
+  cudaFree(cnt);
+  seg.resize(n_rows);
+  for (uint32_t r = 0; r < n_rows; r++)
+    seg[r] = off[r + 1] - off[r];
+  return ok;
+}
+
+// The h ids of largest count, ties broken by the smaller id (deterministic), largest first.
+static std::vector<uint32_t> top_ids(const std::vector<uint32_t> &cnt, size_t h) {
+  std::vector<uint32_t> ids(cnt.size());
+  for (size_t i = 0; i < ids.size(); i++)
+    ids[i] = (uint32_t)i;
+  h = std::min(h, ids.size());
+  std::partial_sort(ids.begin(), ids.begin() + h, ids.end(),
+                    [&](uint32_t a, uint32_t b) { return cnt[a] != cnt[b] ? cnt[a] > cnt[b] : a < b; });
+  ids.resize(h);
+  return ids;
+}
+
+// Hybrid construction: hub columns / hub rows are picked, the edges split into the two dense blocks and the residual
+// by one stable 64-bit radix sort, the residual bucketed as usual and each dense cell the sum of its edges' weights.
+static bool build_hybrid(nts_gather_plan *pl, const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
+                         const nts_vid_t *slot_of, nts_vid_t index_base, int n_hub_cols, int n_hub_rows,
+                         cudaStream_t st) {
+  const uint32_t E = (uint32_t)pl->n_edges, n_rows = pl->n_rows, G = pl->gather_rows;
+  std::vector<uint32_t> col_cnt, seg;
+  if (!hub_counts(offsets, indices, slot_of, index_base, n_rows, E, G, col_cnt, seg, st))
+    return false;
+  const std::vector<uint32_t> cols = top_ids(col_cnt, (size_t)n_hub_cols), rows = top_ids(seg, (size_t)n_hub_rows);
+  pl->hub_cols = (int)cols.size();
+  pl->hub_rows = (int)rows.size();
+  pl->lda_c = (n_rows + 3u) & ~3u;
+  pl->lda_r = ((uint32_t)pl->hub_rows + 3u) & ~3u;
+  const uint64_t dc_cells = (uint64_t)pl->hub_cols * pl->lda_c;
+  pl->dense_floats = dc_cells + (pl->hub_rows ? (uint64_t)G * pl->lda_r : 0);
+  std::vector<uint32_t> col_slot(G, kNoHub), row_slot(n_rows, kNoHub);
+  for (size_t i = 0; i < cols.size(); i++)
+    col_slot[cols[i]] = (uint32_t)i;
+  for (size_t i = 0; i < rows.size(); i++)
+    row_slot[rows[i]] = (uint32_t)i;
+
+  const uint64_t n_keys = (uint64_t)pl->slabs * n_rows;
+  int bits = 1;
+  while (bits < 64 && (1ull << bits) < n_keys + pl->dense_floats)
+    bits++;
+  uint64_t *key_in = nullptr, *key_out = nullptr;
+  uint32_t *val_in = nullptr, *val_out = nullptr, *d_col_slot = nullptr, *d_row_slot = nullptr, *d_runs = nullptr;
+  void *tmp = nullptr;
+  size_t tmp_bytes = 0;
+  bool ok =
+      cudaMalloc(reinterpret_cast<void **>(&pl->pairs), (size_t)E * sizeof(uint2)) == cudaSuccess &&
+      cudaMalloc(reinterpret_cast<void **>(&pl->voff), ((size_t)n_keys + 1) * 4) == cudaSuccess &&
+      cudaMalloc(reinterpret_cast<void **>(&pl->dense), pl->dense_floats * 4) == cudaSuccess &&
+      cudaMalloc(reinterpret_cast<void **>(&pl->hub_col_ids), cols.size() * 4 + 4) == cudaSuccess &&
+      cudaMalloc(reinterpret_cast<void **>(&pl->hub_row_ids), rows.size() * 4 + 4) == cudaSuccess &&
+      cudaMalloc(reinterpret_cast<void **>(&d_col_slot), (size_t)G * 4 + 4) == cudaSuccess &&
+      cudaMalloc(reinterpret_cast<void **>(&d_row_slot), (size_t)n_rows * 4 + 4) == cudaSuccess &&
+      cudaMalloc(reinterpret_cast<void **>(&key_in), (size_t)E * 8) == cudaSuccess &&
+      cudaMalloc(reinterpret_cast<void **>(&key_out), (size_t)E * 8) == cudaSuccess &&
+      cudaMalloc(reinterpret_cast<void **>(&val_in), (size_t)E * 4) == cudaSuccess &&
+      cudaMalloc(reinterpret_cast<void **>(&val_out), (size_t)E * 4) == cudaSuccess &&
+      cudaMalloc(reinterpret_cast<void **>(&d_runs), 4) == cudaSuccess &&
+      cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, key_in, key_out, val_in, val_out, (int64_t)E, 0, bits, st) ==
+          cudaSuccess &&
+      cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 16) == cudaSuccess &&
+      cudaMemcpyAsync(pl->hub_col_ids, cols.data(), cols.size() * 4, cudaMemcpyHostToDevice, st) == cudaSuccess &&
+      cudaMemcpyAsync(pl->hub_row_ids, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, st) == cudaSuccess &&
+      cudaMemcpyAsync(d_col_slot, col_slot.data(), (size_t)G * 4, cudaMemcpyHostToDevice, st) == cudaSuccess &&
+      cudaMemcpyAsync(d_row_slot, row_slot.data(), (size_t)n_rows * 4, cudaMemcpyHostToDevice, st) == cudaSuccess &&
+      cudaMemsetAsync(pl->dense, 0, pl->dense_floats * 4, st) == cudaSuccess;
+  const unsigned blocks = (unsigned)std::min<uint64_t>(((uint64_t)E + 255) / 256, (uint64_t)sm_count() * 32);
+  if (ok) {
+    plan_hybrid_keys_kernel<<<blocks, 256, 0, st>>>(offsets, indices, slot_of, index_base, n_rows, E, pl->slab_rows,
+                                                    (uint32_t)pl->slabs, d_col_slot, d_row_slot, pl->lda_c, dc_cells,
+                                                    pl->lda_r, key_in, val_in);
+    count_launch();
+    // LSD radix sort: stable, so edges of one (slab, row) segment or one dense cell keep their original order
+    ok = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, key_in, key_out, val_in, val_out, (int64_t)E, 0, bits, st) ==
+         cudaSuccess;
+  }
+  if (ok) {
+    const unsigned kb = (unsigned)std::min<uint64_t>((n_keys + 256) / 256, (uint64_t)sm_count() * 32);
+    plan_offsets_kernel<uint64_t><<<kb, 256, 0, st>>>(key_out, E, (uint32_t)n_keys, pl->voff);
+    count_launch();
+    std::vector<uint32_t> h(pl->slabs + 1);
+    ok = cudaStreamSynchronize(st) == cudaSuccess;
+    for (int s = 0; s <= pl->slabs && ok; s++)
+      ok = cudaMemcpy(&h[s], pl->voff + (size_t)s * n_rows, 4, cudaMemcpyDeviceToHost) == cudaSuccess;
+    for (int s = 0; s <= pl->slabs; s++)
+      pl->slab_edge[s] = h[s];
+  }
+  const uint32_t n_res = (uint32_t)pl->slab_edge[pl->slabs], n_dense = E - n_res;
+  if (ok && n_res) {
+    plan_pairs_kernel<<<blocks, 256, 0, st>>>(val_out, indices, weight, slot_of, index_base, n_res, pl->pairs);
+    count_launch();
+  }
+  if (ok && n_dense) { // runs of equal cell keys: (key, length), start = exclusive sum of the lengths (integers)
+    uint32_t n_runs = 0;
+    size_t b1 = 0, b2 = 0;
+    ok = cub::DeviceRunLengthEncode::Encode(nullptr, b1, key_out + n_res, key_in, val_in, d_runs, (int64_t)n_dense,
+                                            st) == cudaSuccess &&
+         cub::DeviceScan::ExclusiveSum(nullptr, b2, val_in, d_col_slot, (int64_t)n_dense, st) == cudaSuccess;
+    if (ok && std::max(b1, b2) > tmp_bytes) {
+      cudaFree(tmp);
+      tmp_bytes = std::max(b1, b2);
+      ok = cudaMalloc(&tmp, tmp_bytes) == cudaSuccess;
+    }
+    uint32_t *run_start = nullptr;
+    ok = ok && cudaMalloc(reinterpret_cast<void **>(&run_start), (size_t)n_dense * 4) == cudaSuccess &&
+         cub::DeviceRunLengthEncode::Encode(tmp, b1, key_out + n_res, key_in, val_in, d_runs, (int64_t)n_dense, st) ==
+             cudaSuccess &&
+         cudaMemcpyAsync(&n_runs, d_runs, 4, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+         cudaStreamSynchronize(st) == cudaSuccess &&
+         cub::DeviceScan::ExclusiveSum(tmp, b2, val_in, run_start, (int64_t)n_runs, st) == cudaSuccess;
+    if (ok) {
+      const unsigned rb = (unsigned)std::min<uint64_t>(((uint64_t)n_runs * 32 + 255) / 256, (uint64_t)sm_count() * 32);
+      plan_cell_sum_kernel<<<rb, 256, 0, st>>>(key_in, run_start, val_in, n_runs, val_out + n_res, weight, n_keys,
+                                               pl->dense);
+      count_launch();
+      ok = cudaStreamSynchronize(st) == cudaSuccess;
+    }
+    cudaFree(run_start);
+  }
+  cudaFree(key_in), cudaFree(key_out), cudaFree(val_in), cudaFree(val_out), cudaFree(tmp);
+  cudaFree(d_col_slot), cudaFree(d_row_slot), cudaFree(d_runs);
+  return ok;
+}
+
 nts_gather_plan *nts_gather_plan_create(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
                                         const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows,
                                         uint64_t n_edges, nts_vid_t gather_rows, int n_slabs, void *stream) {
+  return nts_gather_plan_create_hybrid(offsets, indices, weight, slot_of, index_base, n_rows, n_edges, gather_rows,
+                                       n_slabs, 0, 0, stream);
+}
+
+nts_gather_plan *nts_gather_plan_create_hybrid(const nts_vid_t *offsets, const nts_vid_t *indices,
+                                               const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
+                                               nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows, int n_slabs,
+                                               int n_hub_cols, int n_hub_rows, void *stream) {
   auto bad = [](const char *m) -> nts_gather_plan * {
     fail(-1, m, __FILE__, __LINE__);
     return nullptr;
@@ -736,6 +1097,8 @@ nts_gather_plan *nts_gather_plan_create(const nts_vid_t *offsets, const nts_vid_
     return bad("chunk edge count must fit uint32 offsets");
   if (n_rows && n_edges && !(offsets && indices))
     return bad("null graph array");
+  if (n_hub_cols < 0 || n_hub_rows < 0)
+    return bad("negative hub count");
   if (n_slabs < 1)
     n_slabs = 1;
   if (gather_rows == 0)
@@ -756,10 +1119,14 @@ nts_gather_plan *nts_gather_plan_create(const nts_vid_t *offsets, const nts_vid_
   const uint32_t n_keys = (uint32_t)n_slabs * n_rows;
   uint32_t *key_in = nullptr, *key_out = nullptr, *val_in = nullptr, *val_out = nullptr;
   void *tmp = nullptr;
-  bool ok = cudaMalloc(reinterpret_cast<void **>(&pl->pairs), (size_t)E * sizeof(uint2)) == cudaSuccess &&
-            cudaMalloc(reinterpret_cast<void **>(&pl->voff), ((size_t)n_keys + 1) * sizeof(uint32_t)) == cudaSuccess;
+  const bool hubs = gather_rows > 0 && (n_hub_cols > 0 || n_hub_rows > 0);
+  bool ok = hubs || (cudaMalloc(reinterpret_cast<void **>(&pl->pairs), (size_t)E * sizeof(uint2)) == cudaSuccess &&
+                     cudaMalloc(reinterpret_cast<void **>(&pl->voff), ((size_t)n_keys + 1) * sizeof(uint32_t)) ==
+                         cudaSuccess);
   const unsigned blocks = (unsigned)std::min<uint64_t>(((uint64_t)E + 255) / 256, (uint64_t)sm_count() * 32);
-  if (ok && n_slabs == 1) {
+  if (hubs) {
+    ok = build_hybrid(pl, offsets, indices, weight, slot_of, index_base, n_hub_cols, n_hub_rows, st);
+  } else if (ok && n_slabs == 1) {
     plan_pairs_kernel<<<blocks, 256, 0, st>>>(nullptr, indices, weight, slot_of, index_base, E, pl->pairs);
     count_launch();
     ok = cudaMemcpyAsync(pl->voff, offsets, ((size_t)n_rows + 1) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st) ==
@@ -790,7 +1157,7 @@ nts_gather_plan *nts_gather_plan_create(const nts_vid_t *offsets, const nts_vid_
       plan_pairs_kernel<<<blocks, 256, 0, st>>>(val_out, indices, weight, slot_of, index_base, E, pl->pairs);
       count_launch();
       const unsigned kb = (unsigned)std::min<uint64_t>(((uint64_t)n_keys + 256) / 256, (uint64_t)sm_count() * 32);
-      plan_offsets_kernel<<<kb, 256, 0, st>>>(key_out, E, n_keys, pl->voff);
+      plan_offsets_kernel<uint32_t><<<kb, 256, 0, st>>>(key_out, E, n_keys, pl->voff);
       count_launch();
       std::vector<uint32_t> h(n_slabs + 1);
       ok = cudaStreamSynchronize(st) == cudaSuccess;
@@ -804,9 +1171,8 @@ nts_gather_plan *nts_gather_plan_create(const nts_vid_t *offsets, const nts_vid_
     ok = cudaStreamSynchronize(st) == cudaSuccess && cudaGetLastError() == cudaSuccess;
   cudaFree(key_in), cudaFree(key_out), cudaFree(val_in), cudaFree(val_out), cudaFree(tmp);
   if (!ok) {
+    nts_gather_plan_destroy(pl);
     fail(-1, "nts_gather_plan_create: device allocation or preprocessing failed", __FILE__, __LINE__);
-    cudaFree(pl->pairs), cudaFree(pl->voff);
-    delete pl;
     return nullptr;
   }
   return pl;
@@ -882,7 +1248,7 @@ static nts_gather_plan *build_plan_parts(const nts_plan_part *parts, int n_parts
     plan_permute_pairs_kernel<<<blocks, 256, 0, st>>>(val_out, unsorted, E, pl->pairs);
     count_launch();
     const unsigned kb = (unsigned)std::min<uint64_t>(((uint64_t)n_keys + 256) / 256, (uint64_t)sm_count() * 32);
-    plan_offsets_kernel<<<kb, 256, 0, st>>>(key_out, E, n_keys, pl->voff);
+    plan_offsets_kernel<uint32_t><<<kb, 256, 0, st>>>(key_out, E, n_keys, pl->voff);
     count_launch();
     std::vector<uint32_t> h(n_slabs + 1);
     ok = cudaStreamSynchronize(st) == cudaSuccess;
@@ -979,15 +1345,29 @@ float nts_gather_plan_tuned_ms(const nts_gather_plan *pl) { return pl ? pl->tune
 // (slab, row) segment costs a read-modify-write of the output row) - so the candidates 1, 2, 4, ... up to the
 // size-based bound are built and timed on the real arrays (zero features: the access pattern does not depend on the
 // values), 1 warm + 2 timed launches each, and the fastest is kept.  One-time cost per (chunk, direction, width).
+//
+// Then the dense hub blocks, by coordinate descent from the best plain plan: hub columns 32, 64, ... with no hub rows,
+// then hub rows 32, 64, ... with the chosen columns (each stops at the first candidate that is not faster), then the
+// slab count of the residual at half and twice the plain plan's: at most 12 more timed builds.  NTS_PLAN_HUBS=0
+// (measurement override) skips this.  Only rows with more than kHubFloor edges per cell of their column / row of the
+// block are candidates, which keeps uniform and sparse inputs hub-free without any timing: on an H100 SXM (700 W) the
+// F=602 gather of config B averages ~170 ps per edge (19.4 ms for 114.8 M edges), a dense cell costs 2 * 608 flop,
+// ~18 ps at the 67 TFLOP/s FP32 data-sheet rate, so below ~0.1 edge per cell a column cannot pay for itself even at
+// peak; 0.05 leaves a factor of two for the timed search to settle.
+static constexpr double kHubFloor = 0.05;
+static constexpr int kHubMax = 512;
+
 nts_gather_plan *nts_gather_plan_create_tuned(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
                                               const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows,
                                               uint64_t n_edges, nts_vid_t gather_rows, nts_vid_t feature_size,
                                               void *stream) {
   cudaStream_t st = as_stream(stream);
   const int s_max = nts_gather_plan_pick_slabs(gather_rows, n_edges, n_rows, feature_size, 16ull << 20);
+  const char *hub_env = getenv("NTS_PLAN_HUBS");
+  const bool try_hubs = !(hub_env && strcmp(hub_env, "0") == 0) && n_rows > 0 && gather_rows > 0;
   nts_gather_plan *best = nts_gather_plan_create(offsets, indices, weight, slot_of, index_base, n_rows, n_edges,
                                                  gather_rows, 1, stream);
-  if (!best || s_max <= 1 || n_edges == 0 || feature_size == 0)
+  if (!best || (s_max <= 1 && !try_hubs) || n_edges == 0 || feature_size == 0)
     return best;
   float *x = nullptr, *y = nullptr;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
@@ -1011,26 +1391,54 @@ nts_gather_plan *nts_gather_plan_create_tuned(const nts_vid_t *offsets, const nt
   };
   float best_ms = 0.f;
   ok = ok && time_plan(best, &best_ms);
-  for (int s = 2; ok; s *= 2) {
-    const int cand = s > s_max ? s_max : s;
-    nts_gather_plan *pl = nts_gather_plan_create(offsets, indices, weight, slot_of, index_base, n_rows, n_edges,
-                                                 gather_rows, cand, stream);
-    float ms = 0.f;
-    if (!pl || !time_plan(pl, &ms)) {
+  // build and time one candidate, keep it if it is faster: 1 = kept, 0 = not kept (*ms its time), -1 = failed
+  auto consider = [&](int s, int hc, int hr, float *ms) -> int {
+    nts_gather_plan *pl = nts_gather_plan_create_hybrid(offsets, indices, weight, slot_of, index_base, n_rows, n_edges,
+                                                        gather_rows, s, hc, hr, stream);
+    if (!pl || !time_plan(pl, ms)) {
       nts_gather_plan_destroy(pl);
-      break;
+      return -1;
     }
-    if (ms < best_ms) {
+    if (*ms < best_ms) {
       nts_gather_plan_destroy(best);
       best = pl;
-      best_ms = ms;
-    } else {
-      nts_gather_plan_destroy(pl);
-      if (ms > 1.1f * best_ms) // getting worse: larger slab counts only add read-modify-writes
-        break;
+      best_ms = *ms;
+      return 1;
     }
+    nts_gather_plan_destroy(pl);
+    return 0;
+  };
+  for (int s = 2; ok && s_max > 1; s *= 2) {
+    const int cand = s > s_max ? s_max : s;
+    float ms = 0.f;
+    const int r = consider(cand, 0, 0, &ms);
+    if (r < 0 || (r == 0 && ms > 1.1f * best_ms)) // getting worse: larger slab counts only add read-modify-writes
+      break;
     if (cand == s_max)
       break;
+  }
+  if (ok && try_hubs) {
+    std::vector<uint32_t> col_cnt, seg;
+    ok = hub_counts(offsets, indices, slot_of, index_base, n_rows, (uint32_t)n_edges, gather_rows, col_cnt, seg, st);
+    int n_c = 0, n_r = 0;
+    for (uint32_t c : col_cnt)
+      n_c += c > kHubFloor * n_rows;
+    for (uint32_t s : seg)
+      n_r += s > kHubFloor * gather_rows;
+    const int plain_slabs = best->slabs;
+    float ms = 0.f;
+    for (int c = 32; ok && c <= std::min(n_c, kHubMax); c *= 2)
+      if (consider(best->slabs, c, 0, &ms) != 1)
+        break;
+    for (int r = 32; ok && r <= std::min(n_r, kHubMax); r *= 2)
+      if (consider(best->slabs, best->hub_cols, r, &ms) != 1)
+        break;
+    if (best->hub_cols || best->hub_rows) {
+      const int hc = best->hub_cols, hr = best->hub_rows;
+      for (int s : {plain_slabs / 2, std::min(plain_slabs * 2, s_max)})
+        if (s >= 1 && s != plain_slabs && s != best->slabs)
+          consider(s, hc, hr, &ms);
+    }
   }
   cudaFree(x), cudaFree(y);
   if (e0)
@@ -1047,16 +1455,29 @@ int nts_gather_plan_destroy(nts_gather_plan *pl) {
   cudaFree(pl->pairs);
   cudaFree(pl->voff);
   cudaFree(pl->workspace);
+  cudaFree(pl->dense);
+  cudaFree(pl->hub_col_ids);
+  cudaFree(pl->hub_row_ids);
   delete pl;
   return 0;
 }
 
 int nts_gather_plan_slabs(const nts_gather_plan *pl) { return pl ? pl->slabs : 0; }
 
+int nts_gather_plan_hubs(const nts_gather_plan *pl, int *cols, int *rows) {
+  NTS_ARG_CHECK(pl != nullptr, "null plan");
+  if (cols)
+    *cols = pl->hub_cols;
+  if (rows)
+    *rows = pl->hub_rows;
+  return 0;
+}
+
 uint64_t nts_gather_plan_bytes(const nts_gather_plan *pl) {
   if (!pl)
     return 0;
-  return pl->n_edges * 8ull + ((uint64_t)pl->slabs * pl->n_rows + 1) * 4ull + pl->workspace_floats * 4ull;
+  return pl->n_edges * 8ull + ((uint64_t)pl->slabs * pl->n_rows + 1) * 4ull + pl->workspace_floats * 4ull +
+         pl->dense_floats * 4ull + ((uint64_t)pl->hub_cols + pl->hub_rows) * 4ull;
 }
 
 int nts_gather_plan_last_launch(const nts_gather_plan *pl, int *launches, int *grid, int *k, int *u, int *outv) {

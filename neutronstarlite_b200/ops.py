@@ -8,6 +8,9 @@ memory and the current CUDA stream.  There is no CPU path: a CPU tensor raises.
 """
 from __future__ import annotations
 
+import ctypes as C
+import time as _time
+
 import torch
 
 from . import _lib
@@ -93,22 +96,33 @@ class GatherPlan:
     source-slab bucketing (L2 residency), interleaved (row, weight) pairs, 16-byte aligned gathers."""
 
     def __init__(self, offsets, indices, weight, index_base, n_rows, n_edges, gather_rows, slabs, slot_of=None,
-                 tune_for=0):
-        """slabs > 0: that many source slabs; slabs == 0: the slab count is MEASURED for feature width `tune_for`
-        (nts_gather_plan_create_tuned)."""
+                 tune_for=0, hubs=(0, 0)):
+        """slabs > 0: that many source slabs and hubs = (hub columns, hub rows) dense blocks
+        (nts_gather_plan_create_hybrid); slabs == 0: slab and hub counts are MEASURED for feature width `tune_for`
+        (nts_gather_plan_create_tuned).  build_s is the one-time construction (and tuning) time."""
         L = _lib.load()
+        t0 = _time.perf_counter()
         if slabs > 0:
-            self.handle = L.nts_gather_plan_create(_ptr(offsets), _ptr(indices), _ptr(weight), _ptr(slot_of),
-                                                   int(index_base), int(n_rows), int(n_edges), int(gather_rows),
-                                                   int(slabs), _stream())
+            self.handle = L.nts_gather_plan_create_hybrid(_ptr(offsets), _ptr(indices), _ptr(weight), _ptr(slot_of),
+                                                          int(index_base), int(n_rows), int(n_edges),
+                                                          int(gather_rows), int(slabs), int(hubs[0]), int(hubs[1]),
+                                                          _stream())
         else:
             self.handle = L.nts_gather_plan_create_tuned(_ptr(offsets), _ptr(indices), _ptr(weight), _ptr(slot_of),
                                                          int(index_base), int(n_rows), int(n_edges),
                                                          int(gather_rows), int(tune_for), _stream())
+        self.build_s = _time.perf_counter() - t0      # create synchronises the stream
         if not self.handle:
             raise _lib.NtsError("nts_gather_plan_create failed: " + L.nts_last_error().decode(errors="replace"))
         self.slabs = int(L.nts_gather_plan_slabs(self.handle))
+        hc, hr = C.c_int(0), C.c_int(0)
+        _lib.call("nts_gather_plan_hubs", self.handle, C.byref(hc), C.byref(hr))
+        self.hub_cols, self.hub_rows = hc.value, hr.value
         self.n_rows, self.n_edges = int(n_rows), int(n_edges)
+
+    def key(self):
+        """What decides the plan's arrays besides the chunk direction: plans with equal keys are interchangeable."""
+        return (self.slabs,) + ((self.hub_cols, self.hub_rows) if self.hub_cols or self.hub_rows else ())
 
     def run(self, x, out):
         _lib.call("nts_gather_plan_run", self.handle, _ptr(x), _ptr(out), int(x.shape[1]), _stream())
@@ -152,7 +166,7 @@ def _chunk_plan(chunk, direction, F):
         n_rows, gather_rows = chunk.batch_size_forward, chunk.batch_size_backward
     else:
         n_rows, gather_rows = chunk.batch_size_backward, chunk.batch_size_forward
-    plans = chunk.__dict__.setdefault("_gather_plans", {})      # (direction, slabs) -> plan
+    plans = chunk.__dict__.setdefault("_gather_plans", {})      # (direction, slabs[, hub cols, hub rows]) -> plan
     tuned = chunk.__dict__.setdefault("_gather_plan_for", {})   # (direction, F) -> plan picked by measurement
     key = (direction, _plan_slabs) if _plan_slabs else (direction, "F", int(F))
     plan = plans.get(key) if _plan_slabs else tuned.get(key)
@@ -163,9 +177,10 @@ def _chunk_plan(chunk, direction, F):
         else:
             plan = GatherPlan(chunk.row_offset_gpu, chunk.column_indices_gpu, chunk.edge_weight_backward_gpu,
                               chunk.dst_range[0], n_rows, chunk.edge_size, gather_rows, _plan_slabs, tune_for=int(F))
-        if (direction, plan.slabs) in plans:     # another width already settled on this slab count: share the arrays
-            plan = plans[(direction, plan.slabs)]
-        plans[(direction, plan.slabs)] = plan
+        share = (direction,) + plan.key()
+        if share in plans:     # another width already settled on these slab and hub counts: share the arrays
+            plan = plans[share]
+        plans[share] = plan
         if not _plan_slabs:
             tuned[key] = plan
     return plan
