@@ -156,6 +156,21 @@ uint64_t nts_gather_plan_bytes(const nts_gather_plan *plan);
 int nts_gather_plan_run(nts_gather_plan *plan, const float *input, float *output, nts_vid_t feature_size,
                         void *stream);
 int nts_gather_plan_last_launch(const nts_gather_plan *plan, int *launches, int *grid, int *k, int *u, int *outv);
+/* BF16 gathers with FP32 accumulation: output[r,:] += sum_e w(e) * float(bf16(input[row(e),:])).  bf16() rounds to
+ * nearest even (what torch's x.to(torch.bfloat16) computes, incl. inf, NaN and subnormals); weights, accumulation
+ * and output stay FP32.  An NTS_DTYPE_F32 input is converted once per call into the plan's BF16 workspace (rows
+ * padded to a multiple of 8 values); an NTS_DTYPE_BF16 input is gathered in place when feature_size % 8 == 0 and it
+ * is 16-byte aligned, else re-strided into the workspace.  Hub blocks read BF16 rows and compute in FP32.  Returns an
+ * error under nts_gather_plan_set_variant(1) (the TMA row-staging variant is FP32 only). */
+enum { NTS_DTYPE_F32 = 0, NTS_DTYPE_BF16 = 1 };
+int nts_gather_plan_run_bf16(nts_gather_plan *plan, const void *input, int input_dtype, float *output,
+                             nts_vid_t feature_size, void *stream);
+/* nts_gather_plan_create_tuned with the candidates timed as BF16 gathers (and the L2 slab bound counting 2-byte rows):
+ * the slab and hub counts that suit BF16 rows of this width */
+nts_gather_plan *nts_gather_plan_create_tuned_bf16(const nts_vid_t *offsets, const nts_vid_t *indices,
+                                                   const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
+                                                   nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows,
+                                                   nts_vid_t feature_size, void *stream);
 int nts_gather_plan_set_tuning(int u, int min_blocks, int edges_per_warp); /* measurement hook, 0 = default */
 /* 0 = gathered rows through registers (default); 1 = rows staged in shared memory by per-row cp.async.bulk (TMA) into
  * a per-warp ring, U of set_tuning = ring depth - the north star's "feature tiles via TMA", kept for measurement */
@@ -372,6 +387,9 @@ nts_exchange *nts_exchange_create(const nts_exchange_desc *desc);
 int nts_exchange_destroy(nts_exchange *ex);
 /* floats ONE epoch buffer of the receive window needs at this width; take the MAX over ranks before reserving */
 uint64_t nts_exchange_required_floats(const nts_exchange *ex, nts_vid_t feature_size);
+/* window floats per epoch buffer for BF16 calls of width F (BF16 rows at stride ceil(F/8)*8 forward, FP32 partials
+ * backward): reserve this much before nts_exchange_forward_bf16 / nts_exchange_backward_bf16 */
+uint64_t nts_exchange_required_floats_bf16(const nts_exchange *ex, nts_vid_t feature_size);
 uint64_t nts_exchange_capacity_floats(const nts_exchange *ex);
 /* Replacing the exported window is COLLECTIVE and must not race with peers that still map or write it.  On every
  * rank: nts_exchange_release_peers (drains this rank's device work, closes its mappings of the peers' windows) ->
@@ -387,6 +405,14 @@ int nts_exchange_open_peers(nts_exchange *ex, const unsigned char *window_handle
 int nts_exchange_forward(nts_exchange *ex, const float *x, float *y, nts_vid_t feature_size, void *stream);
 /* dX_p += sum_j A_{j<-p}^T dY_j (ForwardGPUfuseOp::backward, :75-90); dx zeroed by caller */
 int nts_exchange_backward(nts_exchange *ex, const float *g, float *dx, nts_vid_t feature_size, void *stream);
+/* BF16 gathers with FP32 accumulation (the contract of nts_gather_plan_run_bf16) across partitions.  Forward: the
+ * sender rounds its X (NTS_DTYPE_F32, or NTS_DTYPE_BF16 used as is when F % 8 == 0 and 16-byte aligned) once per call
+ * into BF16 rows of stride ceil(F/8)*8 and pushes them (half the bytes), every chunk gathers BF16 rows.  Backward: dY
+ * is rounded once locally; partial gradients are computed, pushed and added in FP32.  Every chunk runs through a plan
+ * tuned per (width, type); the pipelined-vs-merged choice is made per (direction, width, type). */
+int nts_exchange_forward_bf16(nts_exchange *ex, const void *x, int x_dtype, float *y, nts_vid_t feature_size,
+                              void *stream);
+int nts_exchange_backward_bf16(nts_exchange *ex, const float *g, float *dx, nts_vid_t feature_size, void *stream);
 /* per-phase device timeline of the last forward (measurement): [0] push kernel, [1] local chunk, then per ring step
  * s: [2s] wait for the rows of partition (p+s), [2s+1] aggregation of chunk (p+s); [2P] whole call.  2P+1 floats (ms);
  * nts_exchange_last_timeline synchronises the device */

@@ -60,6 +60,8 @@ SIGNATURES = {
     "nts_gather_plan_hubs": (_int, [_vp, C.POINTER(_int), C.POINTER(_int)]),
     "nts_gather_plan_bytes": (_u64, [_vp]),
     "nts_gather_plan_run": (_int, [_vp, _vp, _vp, _u32, _vp]),
+    "nts_gather_plan_run_bf16": (_int, [_vp, _vp, _int, _vp, _u32, _vp]),
+    "nts_gather_plan_create_tuned_bf16": (_vp, [_vp, _vp, _vp, _vp, _u32, _u32, _u64, _u32, _u32, _vp]),
     "nts_gather_plan_last_launch": (_int, [_vp] + [C.POINTER(_int)] * 5),
     "nts_gather_plan_set_tuning": (_int, [_int, _int, _int]),
     "nts_gather_plan_set_variant": (_int, [_int]),
@@ -144,6 +146,9 @@ SIGNATURES.update({
     "nts_exchange_open_peers": (_int, [_vp, C.c_char_p, C.c_char_p]),
     "nts_exchange_forward": (_int, [_vp, _vp, _vp, _u32, _vp]),
     "nts_exchange_backward": (_int, [_vp, _vp, _vp, _u32, _vp]),
+    "nts_exchange_forward_bf16": (_int, [_vp, _vp, _int, _vp, _u32, _vp]),
+    "nts_exchange_backward_bf16": (_int, [_vp, _vp, _vp, _u32, _vp]),
+    "nts_exchange_required_floats_bf16": (_u64, [_vp, _u32]),
     "nts_exchange_set_trace": (_int, [_vp, _int]),
     "nts_exchange_last_timeline": (_int, [_vp, C.POINTER(C.c_float), _int]),
     "nts_exchange_fetch_mirrors": (_int, [_vp, _vp, _vp, _u32, _vp]),

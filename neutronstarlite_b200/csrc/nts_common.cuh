@@ -50,9 +50,21 @@ inline bool aligned_to(const void *p, size_t a) { return (reinterpret_cast<uintp
 
 int sm_count();
 
+// BF16 gathers of nts_plan.cu for the exchange engine: rows of an explicit stride (lds elements of the input type),
+// and the conversion pass that writes BF16 rows of stride ld (ld % 8 == 0, zero past F, dst 16-byte aligned)
+int run_plan_bf16(nts_gather_plan *pl, const void *input, int dtype, uint32_t lds, float *output, uint32_t F,
+                  cudaStream_t st);
+int to_bf16_rows(const void *src, int dtype, uint32_t lds, void *dst, uint32_t n_rows, uint32_t F, uint32_t ld,
+                 cudaStream_t st);
+
 template <int VEC> struct Vec;
 template <> struct Vec<1> { using type = float; };
 template <> struct Vec<2> { using type = float2; };
 template <> struct Vec<4> { using type = float4; };
 
 } // namespace nts
+
+// nts_gather_plan_create_parts with the slab count measured on BF16 gathers when bf16 != 0 (nts_plan.cu)
+extern "C" nts_gather_plan *nts_plan_create_parts_typed(const nts_plan_part *parts, int n_parts, nts_vid_t n_rows,
+                                                        nts_vid_t gather_rows, int n_slabs, nts_vid_t feature_size,
+                                                        int bf16, void *stream);

@@ -70,6 +70,8 @@ struct nts_exchange {
   uint32_t epoch = 0;
   float *bsend = nullptr;             // backward partials [recv_total, F] (local)
   size_t bsend_cap = 0;
+  float *stage16 = nullptr;           // BF16 gathers: this rank's X (forward) or dY (backward) as BF16 rows of stride
+  size_t stage16_cap = 0;             // ld = ceil(F/8)*8, in floats (ld/2 per row)
   cudaStream_t comm = nullptr;
   std::vector<cudaStream_t> dma;      // [P] one stream per peer for copy-engine pushes: the copies to different peers
   std::vector<cudaEvent_t> ev_dma;    //     run on different copy engines at once (one engine alone does not fill NVLink)
@@ -77,11 +79,12 @@ struct nts_exchange {
   cudaEvent_t ev_main = nullptr, ev_comm = nullptr;
   std::vector<cudaEvent_t> ev_peer;   // backward: partial of chunk i finished
   // preprocessed aggregation per chunk direction (created on first use; nullptr = plain kernel)
-  std::vector<std::vector<std::pair<int, nts_gather_plan *>>> plan_fwd, plan_bwd; // [P] -> (feature width, plan)
+  std::vector<std::vector<std::pair<int, nts_gather_plan *>>> plan_fwd, plan_bwd; // [P] -> (plan_key(F, type), plan)
   // receive-side strategy per (direction, width), decided once from measured launch times (decide_mode):
   // 1 = pipeline (one launch per source partition as its rows land), 2 = merged (one launch over all remote chunks)
   struct Mode {
     int F, mode;
+    bool bf16;
     nts_gather_plan *merged;
     float pipeline_ms, merged_ms; // the two estimates the decision was taken on
   };
@@ -355,9 +358,18 @@ static int push_my_rows(nts_exchange *ex, const float *x, uint32_t F, size_t buf
   return 0;
 }
 
-// aggregation of one chunk direction: preprocessed plan for big chunks, the plain kernel otherwise
-static int aggregate_chunk(nts_exchange *ex, int i, bool forward, const float *in, float *out, uint32_t F,
-                           cudaStream_t st) {
+// How a call gathers: FP32 rows of stride F, or BF16 rows of stride ld = ceil(F/8)*8 (FP32 accumulation).
+struct GatherType {
+  bool bf16;
+  uint32_t ld; // row stride of the gathered input in elements
+};
+static int plan_key(uint32_t F, bool bf16) { return bf16 ? -(int)F : (int)F; } // plans are tuned per (width, type)
+
+// aggregation of one chunk direction: preprocessed plan for big chunks (and for every BF16 gather), the plain kernel
+// otherwise
+static int aggregate_chunk(nts_exchange *ex, int i, bool forward, const void *in_rows, float *out, uint32_t F,
+                           cudaStream_t st, GatherType gt = {false, 0}) {
+  const float *in = static_cast<const float *>(in_rows);
   // chunk p is the local one: its "slots" are the global source ids of my own partition (base = dst_start) and its
   // "compact" row offsets are the plain row_offset over all my vertices
   const nts_exchange_chunk &c = ex->chunks[i];
@@ -370,14 +382,15 @@ static int aggregate_chunk(nts_exchange *ex, int i, bool forward, const float *i
   const nts_vid_t *idx = forward ? c.slots : c.column_indices;
   const float *w = forward ? c.weight_forward : c.weight_backward;
   const uint32_t base = (forward && !local) ? 0u : ex->d.dst_start;
-  if (c.edges >= ex->plan_min_edges) {
+  if (c.edges >= ex->plan_min_edges || gt.bf16) {
     std::vector<std::pair<int, nts_gather_plan *>> &plans = (forward ? ex->plan_fwd : ex->plan_bwd)[i];
     nts_gather_plan *pl = nullptr;
     for (auto &e : plans)
-      if (e.first == (int)F)
+      if (e.first == plan_key(F, gt.bf16))
         pl = e.second;
-    if (!pl) { // first use of this width: slab count by measurement, built once and kept
-      pl = nts_gather_plan_create_tuned(off, idx, w, nullptr, base, n_rows, c.edges, gather_rows, F, st);
+    if (!pl) { // first use of this width and type: slab and hub counts by measurement, built once and kept
+      pl = gt.bf16 ? nts_gather_plan_create_tuned_bf16(off, idx, w, nullptr, base, n_rows, c.edges, gather_rows, F, st)
+                   : nts_gather_plan_create_tuned(off, idx, w, nullptr, base, n_rows, c.edges, gather_rows, F, st);
       if (!pl)
         return -1;
       int hc = 0, hr = 0, ehc = 0, ehr = 0;
@@ -389,8 +402,10 @@ static int aggregate_chunk(nts_exchange *ex, int i, bool forward, const float *i
           pl = e.second;
           break;
         }
-      plans.emplace_back((int)F, pl);
+      plans.emplace_back(plan_key(F, gt.bf16), pl);
     }
+    if (gt.bf16)
+      return run_plan_bf16(pl, in_rows, NTS_DTYPE_BF16, gt.ld, out, F, st);
     return nts_gather_plan_run(pl, in, out, F, st);
   }
   return nts_segment_gather_sum(in, out, w, idx, off, base, n_rows, c.edges, F, st);
@@ -427,14 +442,17 @@ template <class Fn> static int time_launches(Fn run, cudaStream_t st, float *ms)
 //   forward : pipeline ~ L + max(sum c_i, T - L)        merged ~ max(L, T) + M
 //   backward: pipeline ~ sum c_i + max(L, T / (P-1))    merged ~ M + max(L, T)
 // Each rank decides for itself (it only changes how a rank consumes its own window / fills its own staging).
-static int decide_mode(nts_exchange *ex, bool forward, uint32_t F, cudaStream_t st, nts_exchange::Mode **out) {
+//   (BF16 gathers: decided per (direction, width, type) on BF16 launches; T from the bytes actually pushed: BF16 rows
+//    of ld = ceil(F/8)*8 values forward, FP32 partials backward)
+static int decide_mode(nts_exchange *ex, bool forward, uint32_t F, cudaStream_t st, nts_exchange::Mode **out,
+                       GatherType gt = {false, 0}) {
   std::vector<nts_exchange::Mode> &modes = forward ? ex->mode_fwd : ex->mode_bwd;
   for (auto &m : modes)
-    if (m.F == (int)F) {
+    if (m.F == (int)F && m.bf16 == gt.bf16) {
       *out = &m;
       return 0;
     }
-  modes.push_back({(int)F, 1, nullptr, 0.f, 0.f});
+  modes.push_back({(int)F, 1, gt.bf16, nullptr, 0.f, 0.f});
   nts_exchange::Mode &m = modes.back();
   *out = &m;
   const int P = ex->P, p = ex->p;
@@ -466,7 +484,7 @@ static int decide_mode(nts_exchange *ex, bool forward, uint32_t F, cudaStream_t 
     parts.push_back(pt);
   }
   const uint32_t out_rows = forward ? Vp : ex->recv_total, in_rows = forward ? ex->recv_total : Vp;
-  m.merged = nts_gather_plan_create_parts(parts.data(), (int)parts.size(), out_rows, in_rows, 0, F, st);
+  m.merged = nts_plan_create_parts_typed(parts.data(), (int)parts.size(), out_rows, in_rows, 0, F, gt.bf16, st);
   if (!m.merged)
     return -1;
   if (ex->forced_mode == 2) {
@@ -475,23 +493,26 @@ static int decide_mode(nts_exchange *ex, bool forward, uint32_t F, cudaStream_t 
   }
   // measure: scratch inputs (zeros: the access pattern does not depend on the values)
   const size_t rows_max = std::max<size_t>(ex->recv_total, Vp);
+  const size_t a_bytes = rows_max * std::max<size_t>((size_t)F * sizeof(float), gt.bf16 ? (size_t)gt.ld * 2 : 0);
   float *a = nullptr, *b = nullptr;
-  NTS_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&a), rows_max * F * sizeof(float)));
+  NTS_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&a), a_bytes));
   if (cudaMalloc(reinterpret_cast<void **>(&b), rows_max * F * sizeof(float)) != cudaSuccess) {
     cudaFree(a);
     return fail(-1, "scratch allocation for the exchange mode measurement failed", __FILE__, __LINE__);
   }
-  cudaMemsetAsync(a, 0, rows_max * F * sizeof(float), st);
+  cudaMemsetAsync(a, 0, a_bytes, st);
   cudaMemsetAsync(b, 0, rows_max * F * sizeof(float), st);
   float L = 0.f, M = 0.f, sum_c = 0.f;
-  int rc = time_launches([&]() { return aggregate_chunk(ex, p, forward, a, b, F, st); }, st, &L);
+  int rc = time_launches([&]() { return aggregate_chunk(ex, p, forward, a, b, F, st, gt); }, st, &L);
   if (!rc)
-    rc = time_launches([&]() { return nts_gather_plan_run(m.merged, a, b, F, st); }, st, &M);
+    rc = time_launches([&]() {
+      return gt.bf16 ? run_plan_bf16(m.merged, a, NTS_DTYPE_BF16, gt.ld, b, F, st) : nts_gather_plan_run(m.merged, a, b, F, st);
+    }, st, &M);
   for (int i = 0; i < P && !rc; i++) {
     if (i == p || !ex->chunks[i].edges || !ex->need_count[i])
       continue;
     float c = 0.f;
-    rc = time_launches([&]() { return aggregate_chunk(ex, i, forward, a, b, F, st); }, st, &c);
+    rc = time_launches([&]() { return aggregate_chunk(ex, i, forward, a, b, F, st, gt); }, st, &c);
     sum_c += c;
   }
   cudaFree(a);
@@ -500,7 +521,8 @@ static int decide_mode(nts_exchange *ex, bool forward, uint32_t F, cudaStream_t 
     return rc;
   if (!ex->chunks[p].edges)
     L = 0.f;
-  const float T = (float)((double)(forward ? ex->recv_total : ex->recv_total) * F * 4.0 / 300e9 * 1e3); // ms
+  const double row_bytes = (forward && gt.bf16) ? gt.ld * 2.0 : F * 4.0;
+  const float T = (float)((double)ex->recv_total * row_bytes / 300e9 * 1e3); // ms
   if (forward) {
     m.pipeline_ms = L + std::max(sum_c, T - L);
     m.merged_ms = std::max(L, T) + M;
@@ -665,6 +687,7 @@ int nts_exchange_destroy(nts_exchange *ex) {
   cudaFree(ex->tickets);
   cudaFree(ex->d_peer_flags);
   cudaFree(ex->bsend);
+  cudaFree(ex->stage16);
   if (ex->err_host)
     cudaFreeHost(ex->err_host);
   if (ex->comm)
@@ -696,6 +719,13 @@ uint64_t nts_exchange_required_floats(const nts_exchange *ex, nts_vid_t feature_
   if (rows == 0)
     rows = 1;
   return rows * (uint64_t)feature_size;
+}
+
+// The same for BF16 gathers: forward rows arrive as BF16 at the padded stride ceil(F/8)*8 (ceil(F/8)*4 floats, more
+// than F for F < 4), backward partials as FP32 rows of F floats.
+uint64_t nts_exchange_required_floats_bf16(const nts_exchange *ex, nts_vid_t feature_size) {
+  const uint64_t row16 = ((feature_size + 7ull) / 8ull) * 4ull;
+  return std::max<uint64_t>(std::max<uint64_t>(ex->recv_total, 1) * row16, nts_exchange_required_floats(ex, feature_size));
 }
 
 uint64_t nts_exchange_capacity_floats(const nts_exchange *ex) { return ex ? ex->buf_floats : 0; }
@@ -754,24 +784,53 @@ int nts_exchange_open_peers(nts_exchange *ex, const unsigned char *window_handle
   return 0;
 }
 
-static int ready_for(nts_exchange *ex, nts_vid_t F) {
-  NTS_ARG_CHECK(ex->peers_open && ex->n_buffers >= 1 && nts_exchange_required_floats(ex, F) <= ex->buf_floats,
+static int ready_for(nts_exchange *ex, nts_vid_t F, bool bf16 = false) {
+  NTS_ARG_CHECK(ex->peers_open && ex->n_buffers >= 1 &&
+                    (bf16 ? nts_exchange_required_floats_bf16(ex, F) : nts_exchange_required_floats(ex, F)) <=
+                        ex->buf_floats,
                 "exchange window not reserved / peers not opened for this feature width");
   return 0;
 }
 
-static int forward_impl(nts_exchange *ex, const float *x, float *y, nts_vid_t F, void *stream) {
+// BF16 gathers: this rank's rows (X forward, dY backward) as BF16 at stride ld, converted once per call into the
+// staging buffer - or used as they are when they already are BF16 rows of 16-byte multiples, aligned.  Returns the
+// rows to push / gather from.
+static int stage_bf16(nts_exchange *ex, const void *src, int dtype, uint32_t F, GatherType gt, cudaStream_t st,
+                      const void **rows) {
+  const uint32_t n = ex->d.owned_vertices;
+  if (dtype == NTS_DTYPE_BF16 && gt.ld == F && aligned_to(src, 16)) {
+    *rows = src;
+    return 0;
+  }
+  NTS_TRY(grow(&ex->stage16, &ex->stage16_cap, (size_t)(n ? n : 1) * (gt.ld / 2)));
+  NTS_TRY(to_bf16_rows(src, dtype, F, ex->stage16, n, F, gt.ld, st));
+  *rows = ex->stage16;
+  return 0;
+}
+
+static int forward_impl(nts_exchange *ex, const void *x_in, int x_dtype, float *y, nts_vid_t F, void *stream,
+                        bool bf16 = false) {
   const nts_exchange_desc &d = ex->d;
+  const float *x = static_cast<const float *>(x_in);
   // a rank that owns no vertices (the 1024-aligned partitioner leaves such ranks on small graphs) has no rows to
   // push or produce, but still takes part in the flag protocol below
   NTS_ARG_CHECK(d.owned_vertices == 0 || (x && y), "null feature pointer");
   cudaStream_t st = as_stream(stream);
   const int P = ex->P, p = ex->p;
+  NTS_ARG_CHECK(!bf16 || P > 1, "BF16 gathers on one partition run through nts_gather_plan_run_bf16");
   if (P == 1)
     return nts_gather_by_dst_from_src(x, y, d.local_weight_forward, d.local_row_indices, d.local_column_offset,
                                       d.dst_start, d.dst_start + d.owned_vertices, d.dst_start,
                                       d.dst_start + d.owned_vertices, d.local_edges, d.owned_vertices, F, 1, stream);
-  NTS_TRY(ready_for(ex, F));
+  NTS_TRY(ready_for(ex, F, bf16));
+  // BF16: rows travel and are gathered as BF16 at stride ld; the push moves them as rows of Fw = ld/2 floats
+  const GatherType gt = {bf16, bf16 ? ((F + 7u) & ~7u) : F};
+  const uint32_t Fw = bf16 ? gt.ld / 2 : F;
+  if (bf16 && d.owned_vertices) {
+    const void *rows = nullptr;
+    NTS_TRY(stage_bf16(ex, x_in, x_dtype, F, gt, st, &rows));
+    x = static_cast<const float *>(rows);
+  }
   const uint32_t epoch = ++ex->epoch;
   const size_t buf = (size_t)(epoch % ex->n_buffers) * ex->buf_floats;
   const uint32_t wait_epoch = epoch > (uint32_t)ex->n_buffers ? epoch - ex->n_buffers : 0u;
@@ -783,15 +842,15 @@ static int forward_impl(nts_exchange *ex, const float *x, float *y, nts_vid_t F,
   if (tr)
     NTS_CUDA_OK(cudaEventRecord(ex->tev[1], ex->comm));
   // ---- side stream: my rows to every peer, ring order p-1, p-2, ... (the peer that needs them first)
-  NTS_TRY(push_my_rows(ex, x, F, buf, epoch, wait_epoch));
+  NTS_TRY(push_my_rows(ex, x, Fw, buf, epoch, wait_epoch));
   NTS_TRY(dma_join(ex, ex->comm));
   if (tr)
     NTS_CUDA_OK(cudaEventRecord(ex->tev[2], ex->comm));
   // ---- main stream: local chunk, then the remote chunks - one launch per partition as its rows arrive (pipeline) or
   // one launch over all of them once everything has landed (merged); measured once per width, see decide_mode
   nts_exchange::Mode *mode = nullptr;
-  NTS_TRY(decide_mode(ex, true, F, st, &mode));
-  NTS_TRY(aggregate_chunk(ex, p, true, x, y, F, st));
+  NTS_TRY(decide_mode(ex, true, F, st, &mode, gt));
+  NTS_TRY(aggregate_chunk(ex, p, true, x, y, F, st, gt));
   if (tr)
     NTS_CUDA_OK(cudaEventRecord(ex->tev[3], st));
   if (mode->mode == 2) {
@@ -803,7 +862,10 @@ static int forward_impl(nts_exchange *ex, const float *x, float *y, nts_vid_t F,
     NTS_LAUNCH_CHECK();
     if (tr)
       NTS_CUDA_OK(cudaEventRecord(ex->tev[4], st));
-    NTS_TRY(nts_gather_plan_run(mode->merged, ex->window + buf, y, F, st));
+    if (bf16)
+      NTS_TRY(run_plan_bf16(mode->merged, ex->window + buf, NTS_DTYPE_BF16, gt.ld, y, F, st));
+    else
+      NTS_TRY(nts_gather_plan_run(mode->merged, ex->window + buf, y, F, st));
     if (tr)
       for (int s = 1; s < P; s++) { // the merged launch is reported under ring step 1, the other steps read 0
         NTS_CUDA_OK(cudaEventRecord(ex->tev[5 + 2 * (s - 1)], st));
@@ -818,7 +880,7 @@ static int forward_impl(nts_exchange *ex, const float *x, float *y, nts_vid_t F,
       if (tr)
         NTS_CUDA_OK(cudaEventRecord(ex->tev[4 + 2 * (s - 1)], st));
       if (ex->need_count[i])
-        NTS_TRY(aggregate_chunk(ex, i, true, ex->window + buf + (size_t)ex->recv_offs[i] * F, y, F, st));
+        NTS_TRY(aggregate_chunk(ex, i, true, ex->window + buf + (size_t)ex->recv_offs[i] * Fw, y, F, st, gt));
       if (tr)
         NTS_CUDA_OK(cudaEventRecord(ex->tev[5 + 2 * (s - 1)], st));
     }
@@ -831,16 +893,22 @@ static int forward_impl(nts_exchange *ex, const float *x, float *y, nts_vid_t F,
   return 0;
 }
 
-static int backward_impl(nts_exchange *ex, const float *g, float *dx, nts_vid_t F, void *stream) {
+static int backward_impl(nts_exchange *ex, const float *g, float *dx, nts_vid_t F, void *stream, bool bf16 = false) {
   const nts_exchange_desc &d = ex->d;
   NTS_ARG_CHECK(d.owned_vertices == 0 || (g && dx), "null gradient pointer");
   cudaStream_t st = as_stream(stream);
   const int P = ex->P, p = ex->p;
+  NTS_ARG_CHECK(!bf16 || P > 1, "BF16 gathers on one partition run through nts_gather_plan_run_bf16");
   if (P == 1)
     return nts_gather_by_src_from_dst(g, dx, d.local_weight_backward, d.local_row_offset, d.local_column_indices,
                                       d.dst_start, d.dst_start + d.owned_vertices, d.dst_start,
                                       d.dst_start + d.owned_vertices, d.local_edges, d.owned_vertices, F, 1, stream);
-  NTS_TRY(ready_for(ex, F));
+  NTS_TRY(ready_for(ex, F, bf16));
+  // BF16: dY converted once into BF16 rows of stride ld, every chunk gathers from them; partials stay FP32
+  const GatherType gt = {bf16, bf16 ? ((F + 7u) & ~7u) : F};
+  const void *gin = g;
+  if (bf16 && d.owned_vertices)
+    NTS_TRY(stage_bf16(ex, g, NTS_DTYPE_F32, F, gt, st, &gin));
   const uint32_t epoch = ++ex->epoch;
   const size_t buf = (size_t)(epoch % ex->n_buffers) * ex->buf_floats;
   const uint32_t wait_epoch = epoch > (uint32_t)ex->n_buffers ? epoch - ex->n_buffers : 0u;
@@ -848,11 +916,14 @@ static int backward_impl(nts_exchange *ex, const float *g, float *dx, nts_vid_t 
   if (ex->recv_total)
     NTS_CUDA_OK(cudaMemsetAsync(ex->bsend, 0, (size_t)ex->recv_total * F * sizeof(float), st));
   nts_exchange::Mode *mode = nullptr;
-  NTS_TRY(decide_mode(ex, false, F, st, &mode));
+  NTS_TRY(decide_mode(ex, false, F, st, &mode, gt));
   if (mode->mode == 2) {
     // ---- merged: ONE launch computes the partial gradients of the active sources of all remote chunks, then every
     // slice goes to its owner through the copy engines
-    NTS_TRY(nts_gather_plan_run(mode->merged, g, ex->bsend, F, st));
+    if (bf16)
+      NTS_TRY(run_plan_bf16(mode->merged, gin, NTS_DTYPE_BF16, gt.ld, ex->bsend, F, st));
+    else
+      NTS_TRY(nts_gather_plan_run(mode->merged, g, ex->bsend, F, st));
     NTS_CUDA_OK(cudaEventRecord(ex->ev_peer[p], st));
     NTS_CUDA_OK(cudaStreamWaitEvent(ex->comm, ex->ev_peer[p], 0));
     for (int s = 1; s < P; s++) {
@@ -867,7 +938,7 @@ static int backward_impl(nts_exchange *ex, const float *g, float *dx, nts_vid_t 
       const int i = (p + s) % P;
       float *slice = ex->bsend + (size_t)ex->recv_offs[i] * F;
       if (ex->need_count[i])
-        NTS_TRY(aggregate_chunk(ex, i, false, g, slice, F, st));
+        NTS_TRY(aggregate_chunk(ex, i, false, gin, slice, F, st, gt));
       NTS_CUDA_OK(cudaEventRecord(ex->ev_peer[i], st));
       NTS_CUDA_OK(cudaStreamWaitEvent(ex->comm, ex->ev_peer[i], 0));
       NTS_TRY(dma_push(ex, i, ex->bsend + (size_t)ex->recv_offs[i] * F, ex->bwd_push_off[i], ex->need_count[i], F, buf,
@@ -875,7 +946,7 @@ static int backward_impl(nts_exchange *ex, const float *g, float *dx, nts_vid_t 
     }
   }
   // ---- local chunk overlaps with the pushes; then everything the peers computed for my rows
-  NTS_TRY(aggregate_chunk(ex, p, false, g, dx, F, st));
+  NTS_TRY(aggregate_chunk(ex, p, false, gin, dx, F, st, gt));
   uint32_t mask = 0;
   for (int j = 0; j < P; j++)
     if (j != p)
@@ -1022,13 +1093,25 @@ int nts_exchange_return_mirror_grads(nts_exchange *ex, const float *mirror_grad,
 // Y_p += sum_i A_{p<-i} X_i.  `y` must be zeroed by the caller (accumulate semantics, like every aggregation entry).
 int nts_exchange_forward(nts_exchange *ex, const float *x, float *y, nts_vid_t F, void *stream) {
   NTS_ARG_CHECK(ex != nullptr, "null engine");
-  return check_wait_error(ex, forward_impl(ex, x, y, F, stream));
+  return check_wait_error(ex, forward_impl(ex, x, NTS_DTYPE_F32, y, F, stream));
 }
 
 // dX_p += sum_j A_{j<-p}^T dY_j.  `dx` must be zeroed by the caller.
 int nts_exchange_backward(nts_exchange *ex, const float *g, float *dx, nts_vid_t F, void *stream) {
   NTS_ARG_CHECK(ex != nullptr, "null engine");
   return check_wait_error(ex, backward_impl(ex, g, dx, F, stream));
+}
+
+// BF16 gathers with FP32 accumulation (nts_gather_plan_run_bf16's contract) across partitions: the rows travel as BF16
+int nts_exchange_forward_bf16(nts_exchange *ex, const void *x, int x_dtype, float *y, nts_vid_t F, void *stream) {
+  NTS_ARG_CHECK(ex != nullptr, "null engine");
+  NTS_ARG_CHECK(x_dtype == NTS_DTYPE_F32 || x_dtype == NTS_DTYPE_BF16, "x_dtype must be NTS_DTYPE_F32 or NTS_DTYPE_BF16");
+  return check_wait_error(ex, forward_impl(ex, x, x_dtype, y, F, stream, true));
+}
+
+int nts_exchange_backward_bf16(nts_exchange *ex, const float *g, float *dx, nts_vid_t F, void *stream) {
+  NTS_ARG_CHECK(ex != nullptr, "null engine");
+  return check_wait_error(ex, backward_impl(ex, g, dx, F, stream, true));
 }
 
 } // extern "C"

@@ -24,9 +24,16 @@
 //
 // Plan construction (hand-written kernels + one CUB radix sort) replaces nothing in the reference: its chunks are
 // built on the host by single-threaded loops (core/PartitionedGraph.hpp:324-420) and never re-bucketed.
+//
+// BF16 gathers (nts_gather_plan_run_bf16): the gathered operand is read as BF16 rows (round-to-nearest-even of the
+// FP32 input, one conversion pass per call into the plan's workspace at a stride of ceil(F/8)*8) and widened to FP32
+// in registers; weights, accumulators and outputs stay FP32.  A 16-byte load then carries 8 values instead of 4, so
+// every gathered edge moves half the bytes through L2 and the L1 data stage.
 #include <cub/cub.cuh>
+#include <cuda_bf16.h>
 
 #include <algorithm>
+#include <type_traits>
 #include <vector>
 
 #include "nts_common.cuh"
@@ -42,6 +49,8 @@ struct nts_gather_plan {
   std::vector<uint64_t> slab_edge; // [slabs + 1] host copy of voff[s * n_rows]
   float *workspace = nullptr;  // padded copy of the input when its rows are not 16-byte multiples / aligned
   size_t workspace_floats = 0;
+  __nv_bfloat16 *workspace_bf16 = nullptr; // BF16 copy of the input for BF16 gathers (rows padded to 8 values)
+  size_t workspace_bf16_elems = 0;
   // dense hub blocks (nts_gather_plan_create_hybrid); the slab-bucketed pairs hold the remaining edges only
   int hub_cols = 0, hub_rows = 0;
   uint32_t *hub_col_ids = nullptr; // [hub_cols] gathered rows of the column block, most referenced first
@@ -219,6 +228,34 @@ __global__ void pad_rows_kernel(const float *__restrict__ src, float *__restrict
   }
 }
 
+// dst[r, 0:ld] = {bf16(src[r, 0:F]), 0...}   (ld % 8 == 0; one thread per 16-byte chunk of 8 output values)
+// S = float: round to nearest even (cvt.rn.bf16x2.f32, what torch's .to(torch.bfloat16) executes on the GPU);
+// S = __nv_bfloat16: the values are copied as they are (re-strided / realigned BF16 input).
+template <class S>
+__global__ void bf16_rows_kernel(const S *__restrict__ src, uint32_t lds, uint4 *__restrict__ dst, uint32_t n_rows,
+                                 uint32_t F, uint32_t ld) {
+  const uint32_t ld8 = ld / 8;
+  const uint64_t total = (uint64_t)n_rows * ld8;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t r = i / ld8;
+    const uint32_t c = (uint32_t)(i - r * ld8) * 8;
+    const S *s = src + r * lds;
+    uint32_t w[4];
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const uint32_t c0 = c + 2 * j, c1 = c0 + 1;
+      if constexpr (std::is_same<S, float>::value) {
+        const __nv_bfloat162 h = __floats2bfloat162_rn(c0 < F ? __ldg(s + c0) : 0.f, c1 < F ? __ldg(s + c1) : 0.f);
+        w[j] = *reinterpret_cast<const uint32_t *>(&h);
+      } else {
+        const uint16_t *u = reinterpret_cast<const uint16_t *>(s);
+        w[j] = (c0 < F ? (uint32_t)__ldg(u + c0) : 0u) | ((c1 < F ? (uint32_t)__ldg(u + c1) : 0u) << 16);
+      }
+    }
+    dst[i] = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
 // ---- the aggregation kernel ----------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t p_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void p_mbar_init(uint64_t *bar, uint32_t count) {
@@ -291,21 +328,48 @@ __device__ __forceinline__ void flush_chunk(float *__restrict__ orow, uint32_t c
   }
 }
 
-// K    : float4 chunks per lane per column tile (a tile covers K*128 floats)
+// Gathered element types.  A chunk is the 16 bytes one lane loads per column step: 4 floats, or 8 BF16 values that are
+// widened to FP32 in registers (a BF16 value is the upper half of the FP32 with the same bits: exact, one ALU op).
+template <class T> struct GatherT;
+template <> struct GatherT<float> {
+  using chunk = float4;
+  static constexpr int V = 4;
+  __device__ static __forceinline__ void widen(const float4 &c, float (&v)[4]) {
+    v[0] = c.x, v[1] = c.y, v[2] = c.z, v[3] = c.w;
+  }
+};
+template <> struct GatherT<__nv_bfloat16> {
+  using chunk = uint4;
+  static constexpr int V = 8;
+  __device__ static __forceinline__ void widen(const uint4 &c, float (&v)[8]) {
+    const uint32_t u[4] = {c.x, c.y, c.z, c.w};
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      v[2 * i] = __uint_as_float(u[i] << 16);
+      v[2 * i + 1] = __uint_as_float(u[i] & 0xffff0000u);
+    }
+  }
+};
+
+// T    : gathered element type (float | __nv_bfloat16); a chunk holds V = 4 | 8 values
+// K    : chunks per lane per column tile (a tile covers K*32*V values)
 // U    : edges whose K loads are issued before any FMA (U*K independent 16-byte loads per lane)
 // OUTV : floats per output store (4 when F % 4 == 0 and the output is 16-byte aligned, else 2 or 1)
 // MINB : __launch_bounds__ minimum CTAs per SM
-// G    : virtual warps per warp.  Rows of at most 16 / 8 float4 (F <= 64 / 32) would leave half / three quarters of
-//        the lanes idle, so a warp is split into G independent groups of 32/G lanes, each with its own edge quantum,
+// G    : virtual warps per warp.  Rows of at most 16 / 8 chunks (FP32: F <= 64 / 32) would leave half / three quarters
+//        of the lanes idle, so a warp is split into G independent groups of 32/G lanes, each with its own edge quantum,
 //        row bookkeeping and accumulators (the kernel has no warp-wide shuffles: all state is per lane already).
 // Warp g owns the edge quantum [e_begin + q*Q, ...) of column tile t (g = q*tiles + t); the (row, weight) pairs of the
 // CTA's edge span are staged in shared memory by one cp.async.bulk, completion on an mbarrier.
-template <int K, int U, int OUTV, int MINB, int G = 1>
+template <class T, int K, int U, int OUTV, int MINB, int G = 1>
 __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
-    planned_gather_sum_kernel(const float4 *__restrict__ in, uint32_t ld4, float *__restrict__ out, uint32_t F,
-                              const uint2 *__restrict__ pairs, const uint32_t *__restrict__ off, uint32_t n_rows,
-                              uint32_t e_begin, uint32_t e_end, uint32_t Q, uint32_t tiles, uint32_t tile_vecs) {
+    planned_gather_sum_kernel(const typename GatherT<T>::chunk *__restrict__ in, uint32_t ldc, float *__restrict__ out,
+                              uint32_t F, const uint2 *__restrict__ pairs, const uint32_t *__restrict__ off,
+                              uint32_t n_rows, uint32_t e_begin, uint32_t e_end, uint32_t Q, uint32_t tiles,
+                              uint32_t tile_vecs) {
   static_assert(G == 1 || K == 1, "virtual warps are for rows narrower than a warp");
+  using Chunk = typename GatherT<T>::chunk;
+  constexpr int V = GatherT<T>::V;
   constexpr uint32_t GS = 32 / G;                       // lanes per virtual warp
   const uint32_t lane = threadIdx.x & (GS - 1);         // lane within the virtual warp
   const uint32_t vwarp_in_block = threadIdx.x / GS;
@@ -348,33 +412,41 @@ __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
   const uint32_t e0 = (uint32_t)e0_64;
   const uint32_t e1 = (e0_64 + Q < e_end) ? e0 + Q : e_end;
 
-  const uint32_t c0 = tile * tile_vecs + lane; // first float4 column of this lane
+  const uint32_t c0 = tile * tile_vecs + lane; // first chunk column of this lane
   bool act[K];
 #pragma unroll
   for (int k = 0; k < K; k++)
-    act[k] = (k * GS + lane) < tile_vecs && (c0 + k * GS) < ld4;
+    act[k] = (k * GS + lane) < tile_vecs && (c0 + k * GS) < ldc;
 
   uint32_t row = plan_find_row(off, n_rows, e0);
   uint32_t row_end = __ldg(off + row + 1);
   bool row_started_inside = __ldg(off + row) >= e0;
 
-  float4 acc[K];
+  float acc[K][V];
 #pragma unroll
   for (int k = 0; k < K; k++)
-    acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int j = 0; j < V; j++)
+      acc[k][j] = 0.f;
 
   auto flush = [&](bool whole) {
     float *orow = out + (size_t)row * F;
 #pragma unroll
     for (int k = 0; k < K; k++) {
-      const uint32_t col = (c0 + k * GS) * 4;
-      if (act[k] && col < F) {
-        if (whole)
-          flush_chunk<OUTV, false>(orow, col, F, acc[k]);
-        else
-          flush_chunk<OUTV, true>(orow, col, F, acc[k]);
+#pragma unroll
+      for (int h = 0; h < V; h += 4) { // the output keeps OUTV-float stores: a BF16 chunk flushes as two float4
+        const uint32_t col = (c0 + k * GS) * V + h;
+        const float4 a = make_float4(acc[k][h], acc[k][h + 1], acc[k][h + 2], acc[k][h + 3]);
+        if (act[k] && col < F) {
+          if (whole)
+            flush_chunk<OUTV, false>(orow, col, F, a);
+          else
+            flush_chunk<OUTV, true>(orow, col, F, a);
+        }
       }
-      acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+      for (int j = 0; j < V; j++)
+        acc[k][j] = 0.f;
     }
   };
   auto advance = [&](uint32_t ee) {
@@ -391,14 +463,21 @@ __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
 
   const uint2 *sp = s_pair - cta_e_base;
   uint32_t e = e0;
+  auto fma_chunk = [&](int k, float w, const Chunk &c) {
+    float x[V];
+    GatherT<T>::widen(c, x);
+#pragma unroll
+    for (int j = 0; j < V; j++)
+      acc[k][j] = fmaf(w, x[j], acc[k][j]);
+  };
   for (; e + U <= e1; e += U) {
-    float4 v[U][K];
+    Chunk v[U][K];
     float wu[U];
 #pragma unroll
     for (int u = 0; u < U; u++) {
       const uint2 pr = sp[e + u];
       wu[u] = __uint_as_float(pr.y);
-      const float4 *p = in + (size_t)pr.x * ld4 + c0;
+      const Chunk *p = in + (size_t)pr.x * ldc + c0;
 #pragma unroll
       for (int k = 0; k < K; k++)
         if (act[k])
@@ -410,19 +489,15 @@ __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
         advance(e + u);
 #pragma unroll
       for (int k = 0; k < K; k++)
-        if (act[k]) {
-          acc[k].x = fmaf(wu[u], v[u][k].x, acc[k].x);
-          acc[k].y = fmaf(wu[u], v[u][k].y, acc[k].y);
-          acc[k].z = fmaf(wu[u], v[u][k].z, acc[k].z);
-          acc[k].w = fmaf(wu[u], v[u][k].w, acc[k].w);
-        }
+        if (act[k])
+          fma_chunk(k, wu[u], v[u][k]);
     }
   }
   for (; e < e1; e++) {
     const uint2 pr = sp[e];
     const float wj = __uint_as_float(pr.y);
-    const float4 *p = in + (size_t)pr.x * ld4 + c0;
-    float4 v1[K];
+    const Chunk *p = in + (size_t)pr.x * ldc + c0;
+    Chunk v1[K];
 #pragma unroll
     for (int k = 0; k < K; k++)
       if (act[k])
@@ -431,12 +506,8 @@ __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
       advance(e);
 #pragma unroll
     for (int k = 0; k < K; k++)
-      if (act[k]) {
-        acc[k].x = fmaf(wj, v1[k].x, acc[k].x);
-        acc[k].y = fmaf(wj, v1[k].y, acc[k].y);
-        acc[k].z = fmaf(wj, v1[k].z, acc[k].z);
-        acc[k].w = fmaf(wj, v1[k].w, acc[k].w);
-      }
+      if (act[k])
+        fma_chunk(k, wj, v1[k]);
   }
   flush(row_started_inside && row_end <= e1);
 }
@@ -592,10 +663,11 @@ struct PlanShape {
   uint32_t tiles, tile_vecs;
 };
 
-template <int K, int U, int OUTV, int MINB, int G = 1>
-static int launch_planned(nts_gather_plan *pl, const PlanShape &sh, const float4 *in, uint32_t ld4, float *out,
+template <class T, int K, int U, int OUTV, int MINB, int G = 1>
+static int launch_planned(nts_gather_plan *pl, const PlanShape &sh, const T *in_rows, uint32_t ldc, float *out,
                           uint32_t F, uint32_t Q, cudaStream_t st) {
-  auto kern = planned_gather_sum_kernel<K, U, OUTV, MINB, G>;
+  auto kern = planned_gather_sum_kernel<T, K, U, OUTV, MINB, G>;
+  const auto *in = reinterpret_cast<const typename GatherT<T>::chunk *>(in_rows);
   const size_t smem = 16 + ((size_t)kPlanWarps * G * Q + 4) * 8;
   NTS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   pl->last_launches = 0;
@@ -606,7 +678,7 @@ static int launch_planned(nts_gather_plan *pl, const PlanShape &sh, const float4
     const uint64_t quanta = (ee - eb + Q - 1) / Q;
     const uint64_t blocks = (quanta * sh.tiles + kPlanWarps * G - 1) / (kPlanWarps * G);
     NTS_ARG_CHECK(blocks <= 0x7fffffffull, "aggregation grid too large");
-    kern<<<(unsigned)blocks, kPlanWarps * 32, smem, st>>>(in, ld4, out, F, pl->pairs, pl->voff + (size_t)s * pl->n_rows,
+    kern<<<(unsigned)blocks, kPlanWarps * 32, smem, st>>>(in, ldc, out, F, pl->pairs, pl->voff + (size_t)s * pl->n_rows,
                                                           pl->n_rows, (uint32_t)eb, (uint32_t)ee, Q, sh.tiles,
                                                           sh.tile_vecs);
     NTS_LAUNCH_CHECK();
@@ -655,19 +727,19 @@ static int launch_planned_tma(nts_gather_plan *pl, const PlanShape &sh, const fl
 #define NTS_PLAN_CASE_G(U_, B_, G_)                                                                                 \
   if (sh.k == 1 && sh.u == U_ && sh.minb == B_ && sh.g == G_) {                                                     \
     if (sh.outv == 4)                                                                                               \
-      return launch_planned<1, U_, 4, B_, G_>(pl, sh, in4, ld4, out, F, Q, st);                                     \
+      return launch_planned<T, 1, U_, 4, B_, G_>(pl, sh, in, ldc, out, F, Q, st);                                   \
     if (sh.outv == 2)                                                                                               \
-      return launch_planned<1, U_, 2, B_, G_>(pl, sh, in4, ld4, out, F, Q, st);                                     \
-    return launch_planned<1, U_, 1, B_, G_>(pl, sh, in4, ld4, out, F, Q, st);                                       \
+      return launch_planned<T, 1, U_, 2, B_, G_>(pl, sh, in, ldc, out, F, Q, st);                                   \
+    return launch_planned<T, 1, U_, 1, B_, G_>(pl, sh, in, ldc, out, F, Q, st);                                     \
   }
 
 #define NTS_PLAN_CASE(K_, U_, B_)                                                                                   \
   if (sh.k == K_ && sh.u == U_ && sh.minb == B_) {                                                                  \
     if (sh.outv == 4)                                                                                               \
-      return launch_planned<K_, U_, 4, B_>(pl, sh, in4, ld4, out, F, Q, st);                                         \
+      return launch_planned<T, K_, U_, 4, B_>(pl, sh, in, ldc, out, F, Q, st);                                       \
     if (sh.outv == 2)                                                                                               \
-      return launch_planned<K_, U_, 2, B_>(pl, sh, in4, ld4, out, F, Q, st);                                         \
-    return launch_planned<K_, U_, 1, B_>(pl, sh, in4, ld4, out, F, Q, st);                                           \
+      return launch_planned<T, K_, U_, 2, B_>(pl, sh, in, ldc, out, F, Q, st);                                       \
+    return launch_planned<T, K_, U_, 1, B_>(pl, sh, in, ldc, out, F, Q, st);                                         \
   }
 
 // ---- dense hub blocks: FP32 SIMT GEMM (FFMA only, no tensor cores) ----------------------------------------------------
@@ -686,14 +758,18 @@ __device__ __forceinline__ void p_cp_async16(void *smem_dst, const void *gmem_sr
                : "memory");
 }
 
-template <int OUTV, bool SPLIT>
+// TB = __nv_bfloat16: B rows are BF16 (ldb % 8 == 0), cp.async fills half-size B tiles and the values are widened to
+// FP32 at the shared-memory read; A, the accumulators and the FFMA math are those of the FP32 instantiation.
+template <class TB, int OUTV, bool SPLIT>
 __global__ void __launch_bounds__(kHubThreads, 2)
     hub_block_gemm_kernel(const float *__restrict__ At, uint32_t lda, uint32_t M, uint32_t K, uint32_t k_split,
-                          const float *__restrict__ B, uint32_t ldb, const uint32_t *__restrict__ colmap,
+                          const TB *__restrict__ B, uint32_t ldb, const uint32_t *__restrict__ colmap,
                           float *__restrict__ out, uint32_t F, const uint32_t *__restrict__ rowmap, uint32_t m_tiles,
                           uint32_t n_tiles) {
+  constexpr bool kBf16 = std::is_same<TB, __nv_bfloat16>::value;
+  constexpr uint32_t kBV = 16 / sizeof(TB); // B values per 16-byte chunk
   __shared__ __align__(16) float As[2][kHubBK][kHubBM];
-  __shared__ __align__(16) float Bs[2][kHubBK][kHubBN];
+  __shared__ __align__(16) TB Bs[2][kHubBK][kHubBN];
   const uint32_t t = threadIdx.x;
   const uint32_t n_tile = blockIdx.x % n_tiles, rest = blockIdx.x / n_tiles;
   const uint32_t m0 = (rest % m_tiles) * kHubBM, n0 = n_tile * kHubBN;
@@ -705,17 +781,31 @@ __global__ void __launch_bounds__(kHubThreads, 2)
 
   auto load = [&](uint32_t kt, int buf) {
 #pragma unroll
-    for (int i = 0; i < 2; i++) { // 512 16-byte chunks per operand tile, 2 per thread
+    for (int i = 0; i < 2; i++) { // 512 16-byte chunks per A tile, 2 per thread
       const uint32_t c = t + i * kHubThreads, kk = c >> 5, c4 = (c & 31) * 4;
       const uint32_t k = k_begin + kt * kHubBK + kk;
-      const bool kin = k < k_end;
-      const bool a_ok = kin && m0 + c4 < lda;
+      const bool a_ok = k < k_end && m0 + c4 < lda;
       p_cp_async16(&As[buf][kk][c4], a_ok ? At + (size_t)k * lda + m0 + c4 : At, a_ok);
-      const bool b_ok = kin && n0 + c4 < ldb;
+    }
+#pragma unroll
+    for (int i = 0; i < (int)(kHubBK * kHubBN / kBV / kHubThreads); i++) { // 512 (FP32) / 256 (BF16) B chunks
+      constexpr uint32_t kRowChunks = kHubBN / kBV;
+      const uint32_t c = t + i * kHubThreads, kk = c / kRowChunks, cv = (c % kRowChunks) * kBV;
+      const uint32_t k = k_begin + kt * kHubBK + kk;
+      const bool b_ok = k < k_end && n0 + cv < ldb;
       const uint32_t brow = b_ok ? (colmap ? __ldg(colmap + k) : k) : 0;
-      p_cp_async16(&Bs[buf][kk][c4], B + (size_t)brow * ldb + (b_ok ? n0 + c4 : 0), b_ok);
+      p_cp_async16(&Bs[buf][kk][cv], B + (size_t)brow * ldb + (b_ok ? n0 + cv : 0), b_ok);
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+  auto read_b4 = [&](int buf, int kk, uint32_t n) -> float4 { // B values n .. n+3 of row kk as FP32
+    if constexpr (kBf16) {
+      const uint2 u = *reinterpret_cast<const uint2 *>(&Bs[buf][kk][n]);
+      return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
+                         __uint_as_float(u.y & 0xffff0000u));
+    } else {
+      return *reinterpret_cast<const float4 *>(&Bs[buf][kk][n]);
+    }
   };
 
   const uint32_t tx = t & 15, ty = t >> 4;
@@ -740,8 +830,8 @@ __global__ void __launch_bounds__(kHubThreads, 2)
     for (int kk = 0; kk < kHubBK; kk++) {
       const float4 a0 = *reinterpret_cast<const float4 *>(&As[buf][kk][ty * 4]);
       const float4 a1 = *reinterpret_cast<const float4 *>(&As[buf][kk][64 + ty * 4]);
-      const float4 b0 = *reinterpret_cast<const float4 *>(&Bs[buf][kk][tx * 4]);
-      const float4 b1 = *reinterpret_cast<const float4 *>(&Bs[buf][kk][64 + tx * 4]);
+      const float4 b0 = read_b4(buf, kk, tx * 4);
+      const float4 b1 = read_b4(buf, kk, 64 + tx * 4);
       const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
       const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
@@ -769,15 +859,15 @@ __global__ void __launch_bounds__(kHubThreads, 2)
   }
 }
 
-template <int OUTV>
-static int launch_hub_blocks(nts_gather_plan *pl, const float *in, uint32_t ldb, float *out, uint32_t F,
+template <class TB, int OUTV>
+static int launch_hub_blocks(nts_gather_plan *pl, const TB *in, uint32_t ldb, float *out, uint32_t F,
                              cudaStream_t st) {
   const uint32_t n_tiles = (F + kHubBN - 1) / kHubBN;
   if (pl->hub_cols) { // column block: M = n_rows, K = hub_cols
     const uint32_t m_tiles = (pl->n_rows + kHubBM - 1) / kHubBM;
     const uint64_t blocks = (uint64_t)m_tiles * n_tiles;
     NTS_ARG_CHECK(blocks <= 0x7fffffffull, "hub column block grid too large");
-    hub_block_gemm_kernel<OUTV, false><<<(unsigned)blocks, kHubThreads, 0, st>>>(
+    hub_block_gemm_kernel<TB, OUTV, false><<<(unsigned)blocks, kHubThreads, 0, st>>>(
         pl->dense, pl->lda_c, pl->n_rows, (uint32_t)pl->hub_cols, (uint32_t)pl->hub_cols, in, ldb, pl->hub_col_ids, out,
         F, nullptr, m_tiles, n_tiles);
     NTS_LAUNCH_CHECK();
@@ -790,7 +880,7 @@ static int launch_hub_blocks(nts_gather_plan *pl, const float *in, uint32_t ldb,
     uint32_t k_split = (uint32_t)((K + splits - 1) / splits);
     k_split = std::max<uint32_t>((k_split + kHubBK - 1) / kHubBK * kHubBK, 16 * kHubBK);
     splits = (K + k_split - 1) / k_split;
-    hub_block_gemm_kernel<OUTV, true><<<(unsigned)(splits * m_tiles * n_tiles), kHubThreads, 0, st>>>(
+    hub_block_gemm_kernel<TB, OUTV, true><<<(unsigned)(splits * m_tiles * n_tiles), kHubThreads, 0, st>>>(
         pl->dense + (size_t)pl->hub_cols * pl->lda_c, pl->lda_r, (uint32_t)pl->hub_rows, K, k_split, in, ldb, nullptr,
         out, F, pl->hub_row_ids, m_tiles, n_tiles);
     NTS_LAUNCH_CHECK();
@@ -798,45 +888,28 @@ static int launch_hub_blocks(nts_gather_plan *pl, const float *in, uint32_t ldb,
   return 0;
 }
 
-static int run_plan(nts_gather_plan *pl, const float *input, float *output, uint32_t F, cudaStream_t st) {
-  if (pl->n_rows == 0 || pl->n_edges == 0 || F == 0)
-    return 0;
-  NTS_ARG_CHECK(input && output, "null feature pointer");
-  // 16-byte loads need 16-byte aligned rows: otherwise gather from a zero-padded copy (ld = F rounded up to 4)
-  const uint32_t ld = (F + 3u) & ~3u;
-  const float *in = input;
-  if (ld != F || !aligned_to(input, 16)) {
-    const size_t need = (size_t)pl->gather_rows * ld;
-    if (need > pl->workspace_floats) {
-      if (pl->workspace)
-        NTS_CUDA_OK(cudaFree(pl->workspace));
-      pl->workspace = nullptr;
-      NTS_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&pl->workspace), need * sizeof(float)));
-      pl->workspace_floats = need;
-    }
-    const uint64_t total = (uint64_t)pl->gather_rows * ld;
-    const unsigned blocks = (unsigned)std::min<uint64_t>((total + 255) / 256, (uint64_t)sm_count() * 32);
-    pad_rows_kernel<<<blocks, 256, 0, st>>>(input, pl->workspace, pl->gather_rows, F, ld);
-    NTS_LAUNCH_CHECK();
-    in = pl->workspace;
-  }
+// The gather of rows already in the kernel's layout: `in` holds gather_rows rows of ld values of T, 16-byte aligned,
+// ld % V == 0, zero past F.  Dense hub blocks first, then the residual edges' slab launches (stream order).
+template <class T>
+static int run_gather(nts_gather_plan *pl, const T *in, uint32_t ld, float *output, uint32_t F, cudaStream_t st) {
+  constexpr bool kBf16 = std::is_same<T, __nv_bfloat16>::value;
   PlanShape sh;
-  const uint32_t ld4 = ld / 4;
-  const uint32_t chunks = (ld4 + 31) / 32;
+  const uint32_t ldc = ld / GatherT<T>::V; // 16-byte chunks per row
+  const uint32_t chunks = (ldc + 31) / 32;
   const uint32_t kmax = 5;
   sh.tiles = (chunks + kmax - 1) / kmax;
-  sh.tile_vecs = (ld4 + sh.tiles - 1) / sh.tiles;
+  sh.tile_vecs = (ldc + sh.tiles - 1) / sh.tiles;
   sh.k = (int)((sh.tile_vecs + 31) / 32);
-  sh.tiles = (ld4 + sh.tile_vecs - 1) / sh.tile_vecs;
+  sh.tiles = (ldc + sh.tile_vecs - 1) / sh.tile_vecs;
   sh.outv = (F % 4 == 0 && aligned_to(output, 16)) ? 4 : ((F % 2 == 0 && aligned_to(output, 8)) ? 2 : 1);
-  if (pl->hub_cols || pl->hub_rows) { // dense blocks first, then the residual edges' slab launches (stream order)
-    const int rc = sh.outv == 4   ? launch_hub_blocks<4>(pl, in, ld, output, F, st)
-                   : sh.outv == 2 ? launch_hub_blocks<2>(pl, in, ld, output, F, st)
-                                  : launch_hub_blocks<1>(pl, in, ld, output, F, st);
+  if (pl->hub_cols || pl->hub_rows) {
+    const int rc = sh.outv == 4   ? launch_hub_blocks<T, 4>(pl, in, ld, output, F, st)
+                   : sh.outv == 2 ? launch_hub_blocks<T, 2>(pl, in, ld, output, F, st)
+                                  : launch_hub_blocks<T, 1>(pl, in, ld, output, F, st);
     if (rc)
       return rc;
   }
-  sh.g = ld4 <= 8 ? 4 : (ld4 <= 16 ? 2 : 1); // rows narrower than half / a quarter of a warp: virtual warps
+  sh.g = ldc <= 8 ? 4 : (ldc <= 16 ? 2 : 1); // rows narrower than half / a quarter of a warp: virtual warps
   if (g_plan_variant == 1 || getenv("NTS_PLAN_NO_SUBWARP"))
     sh.g = 1;
   // (U, min CTAs/SM): U*K 16-byte loads in flight per lane
@@ -846,6 +919,14 @@ static int run_plan(nts_gather_plan *pl, const float *input, float *output, uint
   // k = 1, F = 128: U=4 at 4 CTAs 3.98 ms vs U=8 at 3 CTAs 4.37 / U=16 at 2 CTAs 5.5
   sh.minb = sh.k >= 3 ? 2 : (sh.k == 2 ? 3 : 4);
   sh.u = sh.k == 4 ? 2 : 4;
+  if constexpr (kBf16) {
+    // BF16 rows (8 values per chunk: F = 602 is k = 3, F = 128 is k = 1 with 2 virtual warps), measured on an H100
+    // SXM at 700 W with tools/gather_dtype_sweep.py --tune (BF16-tuned plans of config B, whole call):
+    // k = 3, F = 602: U=2 at 3 CTAs/SM 10.16 ms vs U=4 at 2 CTAs 10.56 / U=6 at 1 CTA 13.77;
+    // k = 1, F = 128 (G = 2): U=4 at 4 CTAs 1.74 ms vs U=8 at 2 CTAs 2.06 (forward and backward alike)
+    sh.minb = sh.k >= 4 ? 2 : (sh.k >= 2 ? 3 : 4);
+    sh.u = sh.k == 1 ? 4 : 2;
+  }
   {
     static int env_read = 0;
     if (!env_read) {
@@ -869,8 +950,31 @@ static int run_plan(nts_gather_plan *pl, const float *input, float *output, uint
   if (Q * sh.g > 1024)
     Q = (1024 / sh.g) & ~31u;
   pl->last_k = sh.k, pl->last_u = sh.u, pl->last_outv = sh.outv;
-  const float4 *in4 = reinterpret_cast<const float4 *>(in);
   float *out = output;
+  if constexpr (kBf16) {
+    // only points that compile without spills (a BF16 chunk holds 8 accumulators: U*K loads cost what they do in
+    // FP32, the accumulators twice as much)
+    NTS_PLAN_CASE_G(4, 4, 2)
+    NTS_PLAN_CASE_G(4, 4, 4)
+    NTS_PLAN_CASE_G(8, 2, 2)
+    NTS_PLAN_CASE_G(8, 2, 4)
+    if (sh.g != 1)
+      return fail(-1, "no BF16 virtual-warp instantiation for this (U, occupancy) point", __FILE__, __LINE__);
+    NTS_PLAN_CASE(1, 4, 4)
+    NTS_PLAN_CASE(1, 8, 2)
+    NTS_PLAN_CASE(2, 2, 3)
+    NTS_PLAN_CASE(2, 4, 2)
+    NTS_PLAN_CASE(3, 4, 2)
+    NTS_PLAN_CASE(3, 2, 3)
+    NTS_PLAN_CASE(3, 6, 1)
+    NTS_PLAN_CASE(4, 2, 2)
+    NTS_PLAN_CASE(4, 4, 2)
+    NTS_PLAN_CASE(5, 2, 2)
+    return fail(-1, "no BF16 planned-aggregation instantiation for this (chunks, U, occupancy) point", __FILE__,
+                __LINE__);
+  } else {
+  const float4 *in4 = reinterpret_cast<const float4 *>(in);
+  const uint32_t ld4 = ldc;
   if (g_plan_variant == 1) { // TMA row staging (measurement variant): U = ring depth
     const int stages = sh.u >= 8 ? 8 : (sh.u >= 4 ? 4 : 2);
     sh.minb = g_plan_minb > 0 ? g_plan_minb : (sh.k >= 4 ? 2 : 4);
@@ -910,6 +1014,79 @@ static int run_plan(nts_gather_plan *pl, const float *input, float *output, uint
   NTS_PLAN_CASE(5, 4, 1)
   NTS_PLAN_CASE(5, 4, 2)
   return fail(-1, "no planned-aggregation instantiation for this (chunks, U, occupancy) point", __FILE__, __LINE__);
+  }
+}
+
+// Workspace of at least `elems` values of E (grown, never shrunk; shared by every width that runs the plan).
+template <class E> static int ensure_workspace(E *&ws, size_t &have, size_t elems) {
+  if (elems <= have)
+    return 0;
+  if (ws)
+    NTS_CUDA_OK(cudaFree(ws));
+  ws = nullptr;
+  have = 0;
+  NTS_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&ws), elems * sizeof(E)));
+  have = elems;
+  return 0;
+}
+
+static int run_plan(nts_gather_plan *pl, const float *input, float *output, uint32_t F, cudaStream_t st) {
+  if (pl->n_rows == 0 || pl->n_edges == 0 || F == 0)
+    return 0;
+  NTS_ARG_CHECK(input && output, "null feature pointer");
+  // 16-byte loads need 16-byte aligned rows: otherwise gather from a zero-padded copy (ld = F rounded up to 4)
+  const uint32_t ld = (F + 3u) & ~3u;
+  const float *in = input;
+  if (ld != F || !aligned_to(input, 16)) {
+    if (const int rc = ensure_workspace(pl->workspace, pl->workspace_floats, (size_t)pl->gather_rows * ld))
+      return rc;
+    const uint64_t total = (uint64_t)pl->gather_rows * ld;
+    const unsigned blocks = (unsigned)std::min<uint64_t>((total + 255) / 256, (uint64_t)sm_count() * 32);
+    pad_rows_kernel<<<blocks, 256, 0, st>>>(input, pl->workspace, pl->gather_rows, F, ld);
+    NTS_LAUNCH_CHECK();
+    in = pl->workspace;
+  }
+  return run_gather<float>(pl, in, ld, output, F, st);
+}
+
+// dst[r, 0:ld] = {bf16(src[r, 0:F]), 0...} for rows of stride lds (elements of src's type); ld % 8 == 0
+int to_bf16_rows(const void *src, int dtype, uint32_t lds, void *dst, uint32_t n_rows, uint32_t F, uint32_t ld,
+                 cudaStream_t st) {
+  NTS_ARG_CHECK(dtype == NTS_DTYPE_F32 || dtype == NTS_DTYPE_BF16, "input dtype must be NTS_DTYPE_F32 or NTS_DTYPE_BF16");
+  NTS_ARG_CHECK(ld % 8 == 0 && ld >= F && lds >= F && aligned_to(dst, 16), "bad BF16 row layout");
+  if (!n_rows || !F)
+    return 0;
+  const uint64_t total = (uint64_t)n_rows * (ld / 8);
+  const unsigned blocks = (unsigned)std::min<uint64_t>((total + 255) / 256, (uint64_t)sm_count() * 32);
+  uint4 *d = static_cast<uint4 *>(dst);
+  if (dtype == NTS_DTYPE_F32)
+    bf16_rows_kernel<float><<<blocks, 256, 0, st>>>(static_cast<const float *>(src), lds, d, n_rows, F, ld);
+  else
+    bf16_rows_kernel<__nv_bfloat16><<<blocks, 256, 0, st>>>(static_cast<const __nv_bfloat16 *>(src), lds, d, n_rows,
+                                                            F, ld);
+  NTS_LAUNCH_CHECK();
+  return 0;
+}
+
+// BF16 gathers on rows of stride lds elements: an FP32 input is rounded into the BF16 workspace (stride ld = F rounded
+// up to 8); a BF16 input is gathered in place when its stride is a whole number of 16-byte chunks and it is aligned
+// (values between F and lds are never written to an output column), else re-strided into the workspace.
+int run_plan_bf16(nts_gather_plan *pl, const void *input, int dtype, uint32_t lds, float *output, uint32_t F,
+                  cudaStream_t st) {
+  NTS_ARG_CHECK(dtype == NTS_DTYPE_F32 || dtype == NTS_DTYPE_BF16, "input dtype must be NTS_DTYPE_F32 or NTS_DTYPE_BF16");
+  NTS_ARG_CHECK(g_plan_variant == 0, "the TMA row-staging variant (nts_gather_plan_set_variant(1)) gathers FP32 rows only");
+  if (pl->n_rows == 0 || pl->n_edges == 0 || F == 0)
+    return 0;
+  NTS_ARG_CHECK(input && output, "null feature pointer");
+  NTS_ARG_CHECK(lds >= F, "row stride below the feature width");
+  if (dtype == NTS_DTYPE_BF16 && lds % 8 == 0 && aligned_to(input, 16))
+    return run_gather<__nv_bfloat16>(pl, static_cast<const __nv_bfloat16 *>(input), lds, output, F, st);
+  const uint32_t ld = (F + 7u) & ~7u;
+  if (const int rc = ensure_workspace(pl->workspace_bf16, pl->workspace_bf16_elems, (size_t)pl->gather_rows * ld))
+    return rc;
+  if (const int rc = to_bf16_rows(input, dtype, lds, pl->workspace_bf16, pl->gather_rows, F, ld, st))
+    return rc;
+  return run_gather<__nv_bfloat16>(pl, pl->workspace_bf16, ld, output, F, st);
 }
 
 } // namespace nts
@@ -918,11 +1095,12 @@ using namespace nts;
 
 extern "C" {
 
-int nts_gather_plan_pick_slabs(nts_vid_t gather_rows, uint64_t n_edges, nts_vid_t n_rows, nts_vid_t feature_size,
+// Slab-count bound for gathered rows of row_bytes bytes each (FP32: F rounded up to 4 floats, BF16: to 8 values).
+static int pick_slabs_for_rows(nts_vid_t gather_rows, uint64_t n_edges, nts_vid_t n_rows, uint64_t row_bytes,
                                uint64_t l2_budget_bytes) {
   if (!l2_budget_bytes)
     l2_budget_bytes = 16ull << 20; // a third of the 50 MB L2: the slab stays resident next to the streamed outputs
-  const uint64_t bytes = (uint64_t)gather_rows * ((feature_size + 3u) & ~3u) * 4ull;
+  const uint64_t bytes = (uint64_t)gather_rows * row_bytes;
   uint64_t s = (bytes + l2_budget_bytes - 1) / l2_budget_bytes;
   // every (slab, row) segment costs one read-modify-write of the output row: keep >= 16 edges per segment on average
   const uint64_t by_degree = n_rows ? n_edges / ((uint64_t)n_rows * 16ull) : 1;
@@ -931,6 +1109,11 @@ int nts_gather_plan_pick_slabs(nts_vid_t gather_rows, uint64_t n_edges, nts_vid_
   if (s > 64)
     s = 64;
   return s < 1 ? 1 : (int)s;
+}
+
+int nts_gather_plan_pick_slabs(nts_vid_t gather_rows, uint64_t n_edges, nts_vid_t n_rows, nts_vid_t feature_size,
+                               uint64_t l2_budget_bytes) {
+  return pick_slabs_for_rows(gather_rows, n_edges, n_rows, ((feature_size + 3ull) & ~3ull) * 4ull, l2_budget_bytes);
 }
 
 // Exact reference counts of the gathered rows and segment lengths of the output rows, on the host.
@@ -1269,9 +1452,11 @@ static nts_gather_plan *build_plan_parts(const nts_plan_part *parts, int n_parts
   return pl;
 }
 
-// n_slabs >= 1: that slab count; n_slabs == 0: measured for feature_size like nts_gather_plan_create_tuned
-nts_gather_plan *nts_gather_plan_create_parts(const nts_plan_part *parts, int n_parts, nts_vid_t n_rows,
-                                              nts_vid_t gather_rows, int n_slabs, nts_vid_t feature_size, void *stream) {
+// n_slabs >= 1: that slab count; n_slabs == 0: measured for feature_size like nts_gather_plan_create_tuned (bf16:
+// timed as BF16 gathers, slab bound on 2-byte rows, like nts_gather_plan_create_tuned_bf16)
+nts_gather_plan *nts_plan_create_parts_typed(const nts_plan_part *parts, int n_parts, nts_vid_t n_rows,
+                                             nts_vid_t gather_rows, int n_slabs, nts_vid_t feature_size, int bf16,
+                                             void *stream) {
   if (!parts || n_parts < 1) {
     fail(-1, "no plan parts", __FILE__, __LINE__);
     return nullptr;
@@ -1282,13 +1467,15 @@ nts_gather_plan *nts_gather_plan_create_parts(const nts_plan_part *parts, int n_
   uint64_t total = 0;
   for (int k = 0; k < n_parts; k++)
     total += parts[k].n_edges;
-  const int s_max = nts_gather_plan_pick_slabs(gather_rows, total, n_rows, feature_size, 16ull << 20);
+  const uint64_t row_bytes = bf16 ? ((feature_size + 7ull) & ~7ull) * 2ull : ((feature_size + 3ull) & ~3ull) * 4ull;
+  const int s_max = pick_slabs_for_rows(gather_rows, total, n_rows, row_bytes, 16ull << 20);
   nts_gather_plan *best = build_plan_parts(parts, n_parts, n_rows, gather_rows, 1, st);
   if (!best || s_max <= 1 || total == 0 || feature_size == 0)
     return best;
   float *x = nullptr, *y = nullptr;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
-  const size_t xb = (size_t)gather_rows * feature_size * sizeof(float), yb = (size_t)n_rows * feature_size * sizeof(float);
+  const size_t xb = (size_t)gather_rows * feature_size * (bf16 ? 2 : sizeof(float)),
+               yb = (size_t)n_rows * feature_size * sizeof(float);
   bool ok = cudaMalloc(reinterpret_cast<void **>(&x), xb) == cudaSuccess &&
             cudaMalloc(reinterpret_cast<void **>(&y), yb) == cudaSuccess &&
             cudaMemsetAsync(x, 0, xb, st) == cudaSuccess && cudaMemsetAsync(y, 0, yb, st) == cudaSuccess &&
@@ -1297,7 +1484,9 @@ nts_gather_plan *nts_gather_plan_create_parts(const nts_plan_part *parts, int n_
     *ms = 1e30f;
     for (int it = 0; it < 3; it++) {
       float t = 0.f;
-      if (cudaEventRecord(e0, st) != cudaSuccess || run_plan(pl, x, y, feature_size, st) != 0 ||
+      if (cudaEventRecord(e0, st) != cudaSuccess ||
+          (bf16 ? run_plan_bf16(pl, x, NTS_DTYPE_BF16, feature_size, y, feature_size, st)
+                : run_plan(pl, x, y, feature_size, st)) != 0 ||
           cudaEventRecord(e1, st) != cudaSuccess || cudaEventSynchronize(e1) != cudaSuccess ||
           cudaEventElapsedTime(&t, e0, e1) != cudaSuccess)
         return false;
@@ -1337,6 +1526,11 @@ nts_gather_plan *nts_gather_plan_create_parts(const nts_plan_part *parts, int n_
   return best;
 }
 
+nts_gather_plan *nts_gather_plan_create_parts(const nts_plan_part *parts, int n_parts, nts_vid_t n_rows,
+                                              nts_vid_t gather_rows, int n_slabs, nts_vid_t feature_size, void *stream) {
+  return nts_plan_create_parts_typed(parts, n_parts, n_rows, gather_rows, n_slabs, feature_size, 0, stream);
+}
+
 float nts_gather_plan_tuned_ms(const nts_gather_plan *pl) { return pl ? pl->tuned_ms : 0.f; }
 
 // Slab count by measurement.  Whether bucketing pays depends on how skewed the gathered rows are (hub sources stay in
@@ -1357,12 +1551,14 @@ float nts_gather_plan_tuned_ms(const nts_gather_plan *pl) { return pl ? pl->tune
 static constexpr double kHubFloor = 0.05;
 static constexpr int kHubMax = 512;
 
-nts_gather_plan *nts_gather_plan_create_tuned(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
-                                              const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows,
-                                              uint64_t n_edges, nts_vid_t gather_rows, nts_vid_t feature_size,
-                                              void *stream) {
+// bf16: candidates are timed with BF16 gathers (a BF16 input of width feature_size, gathered as a BF16 run gathers
+// it) and the slab bound counts rows of ceil(F/8)*8 2-byte values.
+static nts_gather_plan *create_tuned(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
+                                     const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows, uint64_t n_edges,
+                                     nts_vid_t gather_rows, nts_vid_t feature_size, bool bf16, void *stream) {
   cudaStream_t st = as_stream(stream);
-  const int s_max = nts_gather_plan_pick_slabs(gather_rows, n_edges, n_rows, feature_size, 16ull << 20);
+  const uint64_t row_bytes = bf16 ? ((feature_size + 7ull) & ~7ull) * 2ull : ((feature_size + 3ull) & ~3ull) * 4ull;
+  const int s_max = pick_slabs_for_rows(gather_rows, n_edges, n_rows, row_bytes, 16ull << 20);
   const char *hub_env = getenv("NTS_PLAN_HUBS");
   const bool try_hubs = !(hub_env && strcmp(hub_env, "0") == 0) && n_rows > 0 && gather_rows > 0;
   nts_gather_plan *best = nts_gather_plan_create(offsets, indices, weight, slot_of, index_base, n_rows, n_edges,
@@ -1371,16 +1567,21 @@ nts_gather_plan *nts_gather_plan_create_tuned(const nts_vid_t *offsets, const nt
     return best;
   float *x = nullptr, *y = nullptr;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
-  const size_t xb = (size_t)gather_rows * feature_size * sizeof(float), yb = (size_t)n_rows * feature_size * sizeof(float);
+  const size_t xb = (size_t)gather_rows * feature_size * (bf16 ? 2 : sizeof(float)),
+               yb = (size_t)n_rows * feature_size * sizeof(float);
   bool ok = cudaMalloc(reinterpret_cast<void **>(&x), xb) == cudaSuccess &&
             cudaMalloc(reinterpret_cast<void **>(&y), yb) == cudaSuccess &&
             cudaMemsetAsync(x, 0, xb, st) == cudaSuccess && cudaMemsetAsync(y, 0, yb, st) == cudaSuccess &&
             cudaEventCreate(&e0) == cudaSuccess && cudaEventCreate(&e1) == cudaSuccess;
+  auto run_one = [&](nts_gather_plan *pl) {
+    return bf16 ? run_plan_bf16(pl, x, NTS_DTYPE_BF16, feature_size, y, feature_size, st)
+                : run_plan(pl, x, y, feature_size, st);
+  };
   auto time_plan = [&](nts_gather_plan *pl, float *ms) -> bool {
     *ms = 1e30f;
     for (int it = 0; it < 3; it++) {
       float t = 0.f;
-      if (cudaEventRecord(e0, st) != cudaSuccess || run_plan(pl, x, y, feature_size, st) != 0 ||
+      if (cudaEventRecord(e0, st) != cudaSuccess || run_one(pl) != 0 ||
           cudaEventRecord(e1, st) != cudaSuccess || cudaEventSynchronize(e1) != cudaSuccess ||
           cudaEventElapsedTime(&t, e0, e1) != cudaSuccess)
         return false;
@@ -1449,12 +1650,29 @@ nts_gather_plan *nts_gather_plan_create_tuned(const nts_vid_t *offsets, const nt
   return best;
 }
 
+nts_gather_plan *nts_gather_plan_create_tuned(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
+                                              const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows,
+                                              uint64_t n_edges, nts_vid_t gather_rows, nts_vid_t feature_size,
+                                              void *stream) {
+  return create_tuned(offsets, indices, weight, slot_of, index_base, n_rows, n_edges, gather_rows, feature_size, false,
+                      stream);
+}
+
+nts_gather_plan *nts_gather_plan_create_tuned_bf16(const nts_vid_t *offsets, const nts_vid_t *indices,
+                                                   const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
+                                                   nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows,
+                                                   nts_vid_t feature_size, void *stream) {
+  return create_tuned(offsets, indices, weight, slot_of, index_base, n_rows, n_edges, gather_rows, feature_size, true,
+                      stream);
+}
+
 int nts_gather_plan_destroy(nts_gather_plan *pl) {
   if (!pl)
     return 0;
   cudaFree(pl->pairs);
   cudaFree(pl->voff);
   cudaFree(pl->workspace);
+  cudaFree(pl->workspace_bf16);
   cudaFree(pl->dense);
   cudaFree(pl->hub_col_ids);
   cudaFree(pl->hub_row_ids);
@@ -1477,7 +1695,7 @@ uint64_t nts_gather_plan_bytes(const nts_gather_plan *pl) {
   if (!pl)
     return 0;
   return pl->n_edges * 8ull + ((uint64_t)pl->slabs * pl->n_rows + 1) * 4ull + pl->workspace_floats * 4ull +
-         pl->dense_floats * 4ull + ((uint64_t)pl->hub_cols + pl->hub_rows) * 4ull;
+         pl->workspace_bf16_elems * 2ull + pl->dense_floats * 4ull + ((uint64_t)pl->hub_cols + pl->hub_rows) * 4ull;
 }
 
 int nts_gather_plan_last_launch(const nts_gather_plan *pl, int *launches, int *grid, int *k, int *u, int *outv) {
@@ -1498,6 +1716,12 @@ int nts_gather_plan_last_launch(const nts_gather_plan *pl, int *launches, int *g
 int nts_gather_plan_run(nts_gather_plan *pl, const float *input, float *output, nts_vid_t feature_size, void *stream) {
   NTS_ARG_CHECK(pl != nullptr, "null plan");
   return run_plan(pl, input, output, feature_size, as_stream(stream));
+}
+
+int nts_gather_plan_run_bf16(nts_gather_plan *pl, const void *input, int input_dtype, float *output,
+                             nts_vid_t feature_size, void *stream) {
+  NTS_ARG_CHECK(pl != nullptr, "null plan");
+  return run_plan_bf16(pl, input, input_dtype, feature_size, output, feature_size, as_stream(stream));
 }
 
 int nts_gather_plan_set_variant(int variant) {

@@ -24,6 +24,10 @@ Transports:
           as the rows of partition (p+s) have landed - the reference's per-chunk pipeline (core/graph.hpp:3678-3719)
           with the host staging removed.  Backward: per-chunk partials pushed to the owner while the next chunk
           computes.  Big chunks run through nts_gather_plan (slab count measured per width).
+
+gather_dtype=torch.bfloat16 (both transports): the gathered operand is rounded to BF16 once per call by its owner,
+forward rows travel as BF16 (half the bytes), every chunk gathers through a plan tuned per (width, type) and
+accumulates in FP32; backward partial gradients stay FP32.
 """
 from __future__ import annotations
 
@@ -209,23 +213,45 @@ class GpuExchange:
             self._p2p = None
 
     # ---- buffers ---------------------------------------------------------------------------------------------
-    def _buf(self, key, rows, F):
+    def _buf(self, key, rows, F, dtype=torch.float32):
         t = self._staging.get((key, F))
         if t is None or t.shape[0] < rows:
-            t = torch.empty((max(rows, 1), F), dtype=torch.float32, device=self.device)
+            t = torch.empty((max(rows, 1), F), dtype=dtype, device=self.device)
             self._staging[(key, F)] = t
         return t[:rows]
 
     # ---- forward -----------------------------------------------------------------------------------------------
-    def forward(self, x):
+    def _merged_plan(self, direction, F):
+        """BF16 gathers on the NCCL transport: the merged remote CSC (forward) / compact CSR (backward) as one
+        nts_gather_plan tuned for BF16 rows of width F (BF16 gathers exist only in plans), built once per width."""
+        plans = self.__dict__.setdefault("_bf16_merged", {})
+        pl = plans.get((direction, F))
+        if pl is None:
+            plan, Vp = self.plan, self.pg.owned_vertices
+            if direction == "fwd":
+                pl = ops.GatherPlan(plan.remote_col_offset, plan.remote_slots, plan.remote_w, 0, Vp,
+                                    plan.remote_edges, plan.recv_total, 0, tune_for=F, gather_dtype=torch.bfloat16)
+            else:
+                pl = ops.GatherPlan(plan.bwd_offsets, plan.bwd_indices, plan.bwd_w,
+                                    self.pg.graph_chunks[self.p].dst_range[0], plan.recv_total, plan.remote_edges,
+                                    Vp, 0, tune_for=F, gather_dtype=torch.bfloat16)
+            plans[(direction, F)] = pl
+        return pl
+
+    def forward(self, x, gather_dtype=None):
+        """gather_dtype=torch.bfloat16: BF16 gathers with FP32 accumulation (ops.GatherPlan.run's contract); x may be
+        float32 or bfloat16, the rows travel as BF16 on both transports."""
         pg, plan, P, p = self.pg, self.plan, self.P, self.p
+        bf16 = ops._check_gather_dtype(gather_dtype) is not None
         F = x.shape[1]
         y = torch.zeros((pg.owned_vertices, F), dtype=torch.float32, device=x.device)
         cur = torch.cuda.current_stream()
         if P == 1:
-            return ops.gather_by_dst_from_src(pg.graph_chunks[0], y, x)
+            return ops.gather_by_dst_from_src(pg.graph_chunks[0], y, x, gather_dtype=gather_dtype)
         if self._p2p is not None:
-            return self._forward_p2p(x, y)
+            return self._forward_p2p(x, y, bf16)
+        if bf16:
+            return self._forward_nccl_bf16(x, y)
         # pack the rows every peer needs (one launch over the concatenated row list), exchange on the side stream
         send = self._buf("fsend", plan.send_total, F)
         recv = self._buf("frecv", plan.recv_total, F)
@@ -244,6 +270,55 @@ class GpuExchange:
         recv.record_stream(cur)
         self._aggregate_remote(y, recv)
         return y
+
+    def _forward_nccl_bf16(self, x, y):
+        """x converted to BF16 once; the packed rows travel as BF16 (half the bytes); the local chunk and the merged
+        remote chunks gather BF16 rows."""
+        pg, plan, P, p = self.pg, self.plan, self.P, self.p
+        F = x.shape[1]
+        cur = torch.cuda.current_stream()
+        xb = x if x.dtype == torch.bfloat16 else x.to(torch.bfloat16)
+        send = self._buf("fsend16", plan.send_total, F, torch.bfloat16)
+        recv = self._buf("frecv16", plan.recv_total, F, torch.bfloat16)
+        if plan.send_total:
+            torch.index_select(xb, 0, plan.send_rows_all, out=send)
+        self.comm_stream.wait_stream(cur)
+        with torch.cuda.stream(self.comm_stream):
+            in_split = [plan.send_count[j] if j != p else 0 for j in range(P)]
+            out_split = [plan.need_count[i] if i != p else 0 for i in range(P)]
+            dist.all_to_all_single(recv, send, output_split_sizes=out_split, input_split_sizes=in_split,
+                                   group=self.group)
+        ops.gather_by_dst_from_src(pg.graph_chunks[p], y, xb, gather_dtype=torch.bfloat16)
+        cur.wait_stream(self.comm_stream)
+        recv.record_stream(cur)
+        if plan.remote_edges:
+            self._merged_plan("fwd", F).run(recv, y, torch.bfloat16)
+        return y
+
+    def _backward_nccl_bf16(self, g, dx):
+        """dY converted to BF16 once locally; partial gradients are computed, sent and added in FP32."""
+        pg, plan, P, p = self.pg, self.plan, self.P, self.p
+        F = g.shape[1]
+        cur = torch.cuda.current_stream()
+        gb = g.to(torch.bfloat16)
+        send = self._buf("bsend", plan.recv_total, F)
+        recv = self._buf("brecv", plan.send_total, F)
+        send.zero_()
+        if plan.remote_edges:
+            self._merged_plan("bwd", F).run(gb, send, torch.bfloat16)
+        self.comm_stream.wait_stream(cur)
+        with torch.cuda.stream(self.comm_stream):
+            in_split = [plan.need_count[i] if i != p else 0 for i in range(P)]
+            out_split = [plan.send_count[j] if j != p else 0 for j in range(P)]
+            dist.all_to_all_single(recv, send, output_split_sizes=out_split, input_split_sizes=in_split,
+                                   group=self.group)
+        ops.gather_by_src_from_dst(pg.graph_chunks[p], dx, gb, gather_dtype=torch.bfloat16)
+        cur.wait_stream(self.comm_stream)
+        recv.record_stream(cur)
+        if plan.send_total:
+            _lib.call("nts_scatter_add_rows_atomic", _ptr(dx), _ptr(recv), _ptr(plan.send_rows_all), plan.send_total, F,
+                      cur.cuda_stream)
+        return dx
 
     def _aggregate_remote(self, y, staged):
         """All remote chunks in one launch: merged CSC whose indices are slots of the receive staging buffer."""
@@ -338,15 +413,18 @@ class GpuExchange:
         return dx
 
     # ---- backward ----------------------------------------------------------------------------------------------
-    def backward(self, g):
+    def backward(self, g, gather_dtype=None):
         pg, plan, P, p = self.pg, self.plan, self.P, self.p
+        bf16 = ops._check_gather_dtype(gather_dtype) is not None
         F = g.shape[1]
         dx = torch.zeros((pg.owned_vertices, F), dtype=torch.float32, device=g.device)
         cur = torch.cuda.current_stream()
         if P == 1:
-            return ops.gather_by_src_from_dst(pg.graph_chunks[0], dx, g)
+            return ops.gather_by_src_from_dst(pg.graph_chunks[0], dx, g, gather_dtype=gather_dtype)
         if self._p2p is not None:
-            return self._backward_p2p(g, dx)
+            return self._backward_p2p(g, dx, bf16)
+        if bf16:
+            return self._backward_nccl_bf16(g, dx)
         # partial gradients of the active sources of every remote chunk, written straight into the send staging
         send = self._buf("bsend", plan.recv_total, F)
         recv = self._buf("brecv", plan.send_total, F)
@@ -367,24 +445,28 @@ class GpuExchange:
         return dx
 
     # ---- peer-memory transport: the C++ engine (csrc/nts_exchange.cu) --------------------------------------------------
-    def _forward_p2p(self, x, y):
-        self._p2p.reserve(x.shape[1])
+    def _forward_p2p(self, x, y, bf16=False):
+        self._p2p.reserve(x.shape[1], bf16)
         ev = ops._timer.bracket("fwd", x.shape[1], self.pg.owned_edges, self.pg.owned_vertices) if ops._timer else None
         if ev:
             ev[0].record()
-        _lib.call("nts_exchange_forward", self._p2p.handle, _ptr(x), _ptr(y), x.shape[1],
-                  torch.cuda.current_stream().cuda_stream)
+        if bf16:
+            _lib.call("nts_exchange_forward_bf16", self._p2p.handle, _ptr(x), ops._DTYPE_CODE[x.dtype], _ptr(y),
+                      x.shape[1], torch.cuda.current_stream().cuda_stream)
+        else:
+            _lib.call("nts_exchange_forward", self._p2p.handle, _ptr(x), _ptr(y), x.shape[1],
+                      torch.cuda.current_stream().cuda_stream)
         if ev:
             ev[1].record()
         return y
 
-    def _backward_p2p(self, g, dx):
-        self._p2p.reserve(g.shape[1])
+    def _backward_p2p(self, g, dx, bf16=False):
+        self._p2p.reserve(g.shape[1], bf16)
         ev = ops._timer.bracket("bwd", g.shape[1], self.pg.owned_edges, self.pg.owned_vertices) if ops._timer else None
         if ev:
             ev[0].record()
-        _lib.call("nts_exchange_backward", self._p2p.handle, _ptr(g), _ptr(dx), g.shape[1],
-                  torch.cuda.current_stream().cuda_stream)
+        _lib.call("nts_exchange_backward_bf16" if bf16 else "nts_exchange_backward", self._p2p.handle, _ptr(g),
+                  _ptr(dx), g.shape[1], torch.cuda.current_stream().cuda_stream)
         if ev:
             ev[1].record()
         return dx
@@ -441,21 +523,23 @@ class _PeerWindows:
     def _cpu_collective(self):
         return dist.get_backend(self.ex.group) != "nccl"
 
-    def reserve(self, F):
-        """Make the exported receive window large enough for feature width F on EVERY rank.  Collective whenever a
-        rank needs more than it has (all ranks always hold the same capacity: it is the max over ranks):
+    def reserve(self, F, bf16=False):
+        """Make the exported receive window large enough for feature width F (BF16 calls: padded BF16 rows forward,
+        nts_exchange_required_floats_bf16) on EVERY rank.  Collective whenever a rank needs more than it has (all
+        ranks always hold the same capacity: it is the max over ranks):
         release peers -> barrier -> reallocate -> all-gather of the IPC handles -> open -> barrier
         (the contract of nts_exchange_reserve, include/nts_b200.h)."""
         import ctypes as C
         L = _lib.load()
         ex = self.ex
-        if L.nts_exchange_required_floats(self.handle, F) <= L.nts_exchange_capacity_floats(self.handle) and \
-                F <= getattr(self, "_max_F", 0):
+        required = L.nts_exchange_required_floats_bf16 if bf16 else L.nts_exchange_required_floats
+        seen = "_max_F16" if bf16 else "_max_F"       # every rank makes the same sequence of calls
+        if required(self.handle, F) <= L.nts_exchange_capacity_floats(self.handle) and F <= getattr(self, seen, 0):
             return
         cdev = torch.device("cpu") if self._cpu_collective() else ex.device
-        need = torch.tensor([L.nts_exchange_required_floats(self.handle, F)], dtype=torch.int64, device=cdev)
+        need = torch.tensor([required(self.handle, F)], dtype=torch.int64, device=cdev)
         dist.all_reduce(need, op=dist.ReduceOp.MAX, group=ex.group)
-        self._max_F = max(F, getattr(self, "_max_F", 0))
+        setattr(self, seen, max(F, getattr(self, seen, 0)))
         if int(need.item()) <= L.nts_exchange_capacity_floats(self.handle):
             return
         _lib.call("nts_exchange_release_peers", self.handle)

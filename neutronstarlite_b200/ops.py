@@ -31,6 +31,29 @@ def _check_input(t, name="input"):
     return t
 
 
+def _check_gather_dtype(gather_dtype):
+    """The gathered-operand options: None (FP32 gathers) or torch.bfloat16 (BF16 gathers, FP32 accumulation)."""
+    if gather_dtype is not None and gather_dtype != torch.bfloat16:
+        raise _lib.NtsError("gather_dtype must be None or torch.bfloat16, not %s" % (gather_dtype,))
+    return gather_dtype
+
+
+def _check_gathered(t, name, gather_dtype):
+    """_check_input for a gathered operand: with BF16 gathers a bfloat16 tensor is accepted as well (used as is)."""
+    if gather_dtype is None or (t.is_cuda and t.dtype == torch.float32):
+        return _check_input(t, name)
+    if not t.is_cuda:
+        raise _lib.NtsError("%s must be a CUDA tensor (libnts_b200 has no CPU fallback)" % name)
+    if t.dtype != torch.bfloat16 or t.dim() != 2:
+        raise _lib.NtsError("%s must be a 2-D float32 or bfloat16 tensor" % name)
+    if not t.is_contiguous():
+        raise _lib.NtsError("%s must be contiguous" % name)
+    return t
+
+
+_DTYPE_CODE = {torch.float32: 0, torch.bfloat16: 1}   # NTS_DTYPE_F32 / NTS_DTYPE_BF16 of include/nts_b200.h
+
+
 def _ptr(t):
     return 0 if t is None else t.data_ptr()
 
@@ -96,11 +119,13 @@ class GatherPlan:
     source-slab bucketing (L2 residency), interleaved (row, weight) pairs, 16-byte aligned gathers."""
 
     def __init__(self, offsets, indices, weight, index_base, n_rows, n_edges, gather_rows, slabs, slot_of=None,
-                 tune_for=0, hubs=(0, 0)):
+                 tune_for=0, hubs=(0, 0), gather_dtype=None):
         """slabs > 0: that many source slabs and hubs = (hub columns, hub rows) dense blocks
         (nts_gather_plan_create_hybrid); slabs == 0: slab and hub counts are MEASURED for feature width `tune_for`
-        (nts_gather_plan_create_tuned).  build_s is the one-time construction (and tuning) time."""
+        (nts_gather_plan_create_tuned), timed as BF16 gathers when gather_dtype is torch.bfloat16
+        (nts_gather_plan_create_tuned_bf16).  build_s is the one-time construction (and tuning) time."""
         L = _lib.load()
+        _check_gather_dtype(gather_dtype)
         t0 = _time.perf_counter()
         if slabs > 0:
             self.handle = L.nts_gather_plan_create_hybrid(_ptr(offsets), _ptr(indices), _ptr(weight), _ptr(slot_of),
@@ -108,9 +133,9 @@ class GatherPlan:
                                                           int(gather_rows), int(slabs), int(hubs[0]), int(hubs[1]),
                                                           _stream())
         else:
-            self.handle = L.nts_gather_plan_create_tuned(_ptr(offsets), _ptr(indices), _ptr(weight), _ptr(slot_of),
-                                                         int(index_base), int(n_rows), int(n_edges),
-                                                         int(gather_rows), int(tune_for), _stream())
+            create = L.nts_gather_plan_create_tuned_bf16 if gather_dtype is not None else L.nts_gather_plan_create_tuned
+            self.handle = create(_ptr(offsets), _ptr(indices), _ptr(weight), _ptr(slot_of), int(index_base),
+                                 int(n_rows), int(n_edges), int(gather_rows), int(tune_for), _stream())
         self.build_s = _time.perf_counter() - t0      # create synchronises the stream
         if not self.handle:
             raise _lib.NtsError("nts_gather_plan_create failed: " + L.nts_last_error().decode(errors="replace"))
@@ -124,7 +149,17 @@ class GatherPlan:
         """What decides the plan's arrays besides the chunk direction: plans with equal keys are interchangeable."""
         return (self.slabs,) + ((self.hub_cols, self.hub_rows) if self.hub_cols or self.hub_rows else ())
 
-    def run(self, x, out):
+    def run(self, x, out, gather_dtype=None):
+        """out += A x.  gather_dtype=torch.bfloat16: the rows of x (float32 or bfloat16) are gathered as BF16 with FP32
+        accumulation (nts_gather_plan_run_bf16); a bfloat16 x needs that option."""
+        if _check_gather_dtype(gather_dtype) is not None:
+            if x.dtype not in _DTYPE_CODE:
+                raise _lib.NtsError("BF16 gathers take a float32 or bfloat16 input, not %s" % x.dtype)
+            _lib.call("nts_gather_plan_run_bf16", self.handle, _ptr(x), _DTYPE_CODE[x.dtype], _ptr(out),
+                      int(x.shape[1]), _stream())
+            return out
+        if x.dtype == torch.bfloat16:
+            raise _lib.NtsError("a bfloat16 input needs gather_dtype=torch.bfloat16")
         _lib.call("nts_gather_plan_run", self.handle, _ptr(x), _ptr(out), int(x.shape[1]), _stream())
         return out
 
@@ -158,25 +193,31 @@ def set_plan_mode(mode, slabs=0):
     _plan_mode, _plan_slabs = mode, int(slabs)
 
 
-def _chunk_plan(chunk, direction, F):
-    """The GatherPlan of one chunk direction for feature width F, or None when the plain kernel should run."""
-    if _plan_mode == "off" or (_plan_mode == "auto" and chunk.edge_size < PLAN_MIN_EDGES):
+def _chunk_plan(chunk, direction, F, gather_dtype=None):
+    """The GatherPlan of one chunk direction for feature width F, or None when the plain kernel should run.
+    BF16 gathers exist only in nts_gather_plan: with gather_dtype=torch.bfloat16 every chunk gets a plan, whatever its
+    size or the plan mode, tuned per (width, type)."""
+    if gather_dtype is None and (_plan_mode == "off" or (_plan_mode == "auto" and chunk.edge_size < PLAN_MIN_EDGES)):
         return None
     if direction == "fwd":
         n_rows, gather_rows = chunk.batch_size_forward, chunk.batch_size_backward
     else:
         n_rows, gather_rows = chunk.batch_size_backward, chunk.batch_size_forward
     plans = chunk.__dict__.setdefault("_gather_plans", {})      # (direction, slabs[, hub cols, hub rows]) -> plan
-    tuned = chunk.__dict__.setdefault("_gather_plan_for", {})   # (direction, F) -> plan picked by measurement
+    tuned = chunk.__dict__.setdefault("_gather_plan_for", {})   # (direction, F[, "bf16"]) -> plan picked by measurement
     key = (direction, _plan_slabs) if _plan_slabs else (direction, "F", int(F))
+    if gather_dtype is not None and not _plan_slabs:
+        key += ("bf16",)
     plan = plans.get(key) if _plan_slabs else tuned.get(key)
     if plan is None:
         if direction == "fwd":
             plan = GatherPlan(chunk.column_offset_gpu, chunk.row_indices_gpu, chunk.edge_weight_forward_gpu,
-                              chunk.src_range[0], n_rows, chunk.edge_size, gather_rows, _plan_slabs, tune_for=int(F))
+                              chunk.src_range[0], n_rows, chunk.edge_size, gather_rows, _plan_slabs, tune_for=int(F),
+                              gather_dtype=gather_dtype)
         else:
             plan = GatherPlan(chunk.row_offset_gpu, chunk.column_indices_gpu, chunk.edge_weight_backward_gpu,
-                              chunk.dst_range[0], n_rows, chunk.edge_size, gather_rows, _plan_slabs, tune_for=int(F))
+                              chunk.dst_range[0], n_rows, chunk.edge_size, gather_rows, _plan_slabs, tune_for=int(F),
+                              gather_dtype=gather_dtype)
         share = (direction,) + plan.key()
         if share in plans:     # another width already settled on these slab and hub counts: share the arrays
             plan = plans[share]
@@ -186,14 +227,23 @@ def _chunk_plan(chunk, direction, F):
     return plan
 
 
-def gather_by_dst_from_src(chunk, out, x, with_weight=True):
-    """NtsScheduler::GatherByDstFromSrc (core/NtsScheduler.hpp:151-191) on one chunk."""
-    plan = _chunk_plan(chunk, "fwd", x.shape[1]) if with_weight else None
+def _bf16_plan(chunk, direction, F, with_weight, gather_dtype):
+    if _check_gather_dtype(gather_dtype) is None:
+        return _chunk_plan(chunk, direction, F) if with_weight else None
+    if not with_weight:
+        raise _lib.NtsError("BF16 gathers always apply the edge weights (with_weight=True)")
+    return _chunk_plan(chunk, direction, F, gather_dtype)
+
+
+def gather_by_dst_from_src(chunk, out, x, with_weight=True, gather_dtype=None):
+    """NtsScheduler::GatherByDstFromSrc (core/NtsScheduler.hpp:151-191) on one chunk.  gather_dtype=torch.bfloat16:
+    x (float32 or bfloat16) is gathered as BF16 rows with FP32 accumulation (GatherPlan.run)."""
+    plan = _bf16_plan(chunk, "fwd", x.shape[1], with_weight, gather_dtype)
     ev = _timer.bracket("fwd", x.shape[1], chunk.edge_size, chunk.batch_size_forward) if _timer else None
     if ev:
         ev[0].record()
     if plan is not None:
-        plan.run(x, out)
+        plan.run(x, out, gather_dtype)
     else:
         _lib.call("nts_gather_by_dst_from_src", _ptr(x), _ptr(out), _ptr(chunk.edge_weight_forward_gpu),
                   _ptr(chunk.row_indices_gpu), _ptr(chunk.column_offset_gpu), chunk.src_range[0], chunk.src_range[1],
@@ -204,14 +254,15 @@ def gather_by_dst_from_src(chunk, out, x, with_weight=True):
     return out
 
 
-def gather_by_src_from_dst(chunk, out, grad, with_weight=True):
-    """NtsScheduler::GatherBySrcFromDst (core/NtsScheduler.hpp:257-293) on one chunk."""
-    plan = _chunk_plan(chunk, "bwd", grad.shape[1]) if with_weight else None
+def gather_by_src_from_dst(chunk, out, grad, with_weight=True, gather_dtype=None):
+    """NtsScheduler::GatherBySrcFromDst (core/NtsScheduler.hpp:257-293) on one chunk (gather_dtype as in
+    gather_by_dst_from_src: the gathered output gradient is rounded to BF16, dX accumulates in FP32)."""
+    plan = _bf16_plan(chunk, "bwd", grad.shape[1], with_weight, gather_dtype)
     ev = _timer.bracket("bwd", grad.shape[1], chunk.edge_size, chunk.batch_size_backward) if _timer else None
     if ev:
         ev[0].record()
     if plan is not None:
-        plan.run(grad, out)
+        plan.run(grad, out, gather_dtype)
     else:
         _lib.call("nts_gather_by_src_from_dst", _ptr(grad), _ptr(out), _ptr(chunk.edge_weight_backward_gpu),
                   _ptr(chunk.row_offset_gpu), _ptr(chunk.column_indices_gpu), chunk.src_range[0], chunk.src_range[1],
@@ -241,19 +292,26 @@ class ntsGraphOp:
 
 class ForwardSingleGPUfuseOp(ntsGraphOp):
     """core/ntsSingleGPUFusedGraphOp.hpp:48-71 -> Graph::forward_single / backward_single
-    (core/graph.hpp:3805-3855): Y = A X on chunk 0, dX = A^T dY, no communication."""
+    (core/graph.hpp:3805-3855): Y = A X on chunk 0, dX = A^T dY, no communication.
+
+    gather_dtype=torch.bfloat16: the gathered operand (X forward, dY backward) is rounded to BF16 and accumulated in
+    FP32; forward takes a float32 or bfloat16 X, Y and dX are float32, backward takes a float32 dY."""
+
+    def __init__(self, partitioned_graph, active=None, gather_dtype=None):
+        super().__init__(partitioned_graph, active)
+        self.gather_dtype = _check_gather_dtype(gather_dtype)
 
     def forward(self, f_input, f_input1=None):
-        x = _check_input(f_input)
+        x = _check_gathered(f_input, "input", self.gather_dtype)
         c = self.partitioned_graph_.graph_chunks[0]
         y = torch.zeros((c.batch_size_forward, x.shape[1]), dtype=torch.float32, device=x.device)
-        return gather_by_dst_from_src(c, y, x)
+        return gather_by_dst_from_src(c, y, x, gather_dtype=self.gather_dtype)
 
     def backward(self, f_output_grad):
         g = _check_input(f_output_grad, "output_grad")
         c = self.partitioned_graph_.graph_chunks[0]
         dx = torch.zeros((c.batch_size_backward, g.shape[1]), dtype=torch.float32, device=g.device)
-        return gather_by_src_from_dst(c, dx, g)
+        return gather_by_src_from_dst(c, dx, g, gather_dtype=self.gather_dtype)
 
 
 class ForwardGPUfuseOp(ntsGraphOp):
@@ -261,18 +319,25 @@ class ForwardGPUfuseOp(ntsGraphOp):
     through Graph::sync_compute_decoupled / compute_sync_decoupled with host-staged MPI messages
     (core/graph.hpp:3455-3719); here the exchange is device-resident (neutronstarlite_b200.exchange)."""
 
-    def __init__(self, partitioned_graph, active=None, exchange=None):
+    def __init__(self, partitioned_graph, active=None, exchange=None, gather_dtype=None):
         super().__init__(partitioned_graph, active)
+        self.gather_dtype = _check_gather_dtype(gather_dtype)
         if exchange is None:
             from .exchange import default_exchange
             exchange = default_exchange(partitioned_graph)
         self.exchange = exchange
 
     def forward(self, f_input, f_input1=None):
-        return self.exchange.forward(_check_input(f_input))
+        x = _check_gathered(f_input, "input", self.gather_dtype)
+        if self.gather_dtype is None:
+            return self.exchange.forward(x)
+        return self.exchange.forward(x, gather_dtype=self.gather_dtype)
 
     def backward(self, f_output_grad):
-        return self.exchange.backward(_check_input(f_output_grad, "output_grad"))
+        g = _check_input(f_output_grad, "output_grad")
+        if self.gather_dtype is None:
+            return self.exchange.backward(g)
+        return self.exchange.backward(g, gather_dtype=self.gather_dtype)
 
 
 # ---- edge-granular operators (core/ntsDistGPUGraphOp.hpp) ------------------------------------------------------

@@ -91,10 +91,17 @@ class Parameter:
 
 
 class GCNImpl:
-    """toolkits/GCN.hpp:33-354.  `layers` = LAYERS of the cfg, e.g. [602, 128, 41]."""
+    """toolkits/GCN.hpp:33-354.  `layers` = LAYERS of the cfg, e.g. [602, 128, 41].
+
+    gather_dtype=torch.bfloat16: every aggregation gathers its operand as BF16 rows with FP32 accumulation (the
+    operator's option), and the input features, which the first aggregation reads directly, are stored as bfloat16
+    (half the memory of the largest tensor).  Activations, weights and gradients stay float32."""
+
+    _input_is_gathered = True   # X[0] is the first aggregation's operand (stored as bfloat16 under BF16 gathers)
 
     def __init__(self, partitioned_graph, layers, features, labels, mask, learn_rate=0.01, weight_decay=0.0001,
-                 decay_rate=0.97, decay_epoch=100, drop_rate=0.5, op_class=None, op_kwargs=None, seed=0):
+                 decay_rate=0.97, decay_epoch=100, drop_rate=0.5, op_class=None, op_kwargs=None, seed=0,
+                 gather_dtype=None):
         self.pg = partitioned_graph
         self.layers = list(layers)
         self.device = features.device
@@ -112,11 +119,16 @@ class GCNImpl:
         self.MASK = mask.to(self.device)
         self.train_rows = (self.MASK == 0).nonzero().view(-1)
         self.X = [None] * len(self.layers)
+        self.gather_dtype = ops._check_gather_dtype(gather_dtype)
+        if self.gather_dtype is not None and self._input_is_gathered:
+            features = features.detach().to(self.gather_dtype)
         self.X[0] = features.requires_grad_(True)
         if op_class is None:
             op_class = ops.ForwardSingleGPUfuseOp if partitioned_graph.partitions == 1 else ops.ForwardGPUfuseOp
         self.op_class = op_class
-        self.op_kwargs = op_kwargs or {}
+        self.op_kwargs = dict(op_kwargs or {})
+        if self.gather_dtype is not None:
+            self.op_kwargs["gather_dtype"] = self.gather_dtype
         self.loss = None
         self.epoch = 0
 
@@ -183,7 +195,10 @@ class GCNEagerImpl(GCNImpl):
     Each layer runs the weight GEMM first and aggregates the NARROW result (widths LAYERS[1:], e.g. 128 and 41
     instead of 602 and 128 - 4.7x fewer gathered bytes on config B), then `log_softmax` + `nll_loss` on the last
     aggregate.  The tape is [NNOP, GRAPHOP, NNOP, GRAPHOP, NNOP(loss)], so every aggregation has a backward
-    (L forward + L backward calls per epoch)."""
+    (L forward + L backward calls per epoch).  Under gather_dtype the input features stay float32: they feed the
+    first weight GEMM, not an aggregation."""
+
+    _input_is_gathered = False
 
     def __init__(self, *args, **kwargs):
         super().__init__(*args, **kwargs)
