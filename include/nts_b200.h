@@ -297,6 +297,38 @@ int nts_gat_fused_aggregate_backward_two_pass(float *mirror_grad, float *src_sco
                                               const nts_vid_t *slot_column_indices, nts_vid_t batch_size,
                                               nts_vid_t mirror_size, nts_vid_t feature_size, nts_vid_t heads,
                                               float negative_slope, void *stream);
+/* K7 with BF16 gathers and FP32 accumulation.  With m~ = bf16(mirror) and g~ = bf16(grad_out) (round to nearest even,
+ * as torch's x.to(torch.bfloat16)) the layer computes the FP32 layer's function and gradients at the rounded operands:
+ *   forward  : output[d, hD+c] += sum_e a[e,h] * m~[slot(e), hD+c]      (a from the FP32 scores and statistics)
+ *   backward : mirror_grad[slot] += a*g~[d];  dpre = a*(<m~[slot,h], g~[d,h]> - out_dot_grad[d,h]) * leaky_relu'(pre)
+ *              with out_dot_grad[d,h] = <output[d,h], g~[d,h]> (g~, not grad_out: the two passes rely on
+ *              sum_e a*<m~, g~> = <output, g~>).
+ * BF16 rows (mirror, dst_grad) have ld values each: ld % 8 == 0, ld >= feature_size, columns past feature_size zero;
+ * with heads > 1, D = feature_size / heads must be a multiple of 8 and ld == feature_size.  The FP32 output and
+ * mirror_grad have the same row stride ld.  Scores, statistics, dst_pack and the score gradients are FP32.  mirror,
+ * output, mirror_grad, dst_grad, dst_pack and row_indices must be 16-byte aligned.  The backward additionally needs a
+ * power-of-two number of vectors per head and rows of at most 1024 values; there is no fallback: other shapes return
+ * an error.  The gradient outputs must be zeroed by the caller. */
+int nts_gat_fused_aggregate_forward_bf16(const void *mirror, float *output, const float *src_score,
+                                         const float *dst_score, const float *seg_max, const float *seg_sum,
+                                         const nts_vid_t *row_indices, const nts_vid_t *column_offset,
+                                         const nts_vid_t *mirror_index, nts_vid_t batch_size, uint64_t n_edges,
+                                         nts_vid_t feature_size, nts_vid_t ld, nts_vid_t heads, float negative_slope,
+                                         void *stream);
+int nts_gat_fused_aggregate_backward_two_pass_bf16(float *mirror_grad, float *src_score_grad, float *dst_score_grad,
+                                                   float *dst_pack, const void *mirror, const float *src_score,
+                                                   const float *dst_score, const float *seg_max, const float *seg_sum,
+                                                   const float *out_dot_grad, const void *dst_grad,
+                                                   const nts_vid_t *row_indices, const nts_vid_t *column_offset,
+                                                   const nts_vid_t *mirror_index, const nts_vid_t *slot_row_offset,
+                                                   const nts_vid_t *slot_column_indices, nts_vid_t batch_size,
+                                                   nts_vid_t mirror_size, nts_vid_t feature_size, nts_vid_t ld,
+                                                   nts_vid_t heads, float negative_slope, void *stream);
+/* dst[r, 0:ld] = {bf16(src[r, 0:feature_size]), 0 ...} for n_rows rows of stride lds (elements of src_dtype,
+ * NTS_DTYPE_F32 rounded to nearest even, NTS_DTYPE_BF16 copied); ld % 8 == 0, ld >= feature_size, dst 16-byte aligned.
+ * The conversion pass of nts_gather_plan_run_bf16, exported for the BF16 rows of the K7 entries above. */
+int nts_rows_to_bf16(const void *src, int src_dtype, nts_vid_t lds, void *dst, nts_vid_t n_rows, nts_vid_t feature_size,
+                     nts_vid_t ld, void *stream);
 
 /* ---- (vid,row) message records: the reference's host-staged exchange format (comm/network.h:143-149) ---
  * record k = { uint32 vid; float row[feature_size]; }, read through mapped pinned host memory. */

@@ -83,6 +83,9 @@ SIGNATURES = {
     "nts_gat_fused_aggregate_forward": (_int, [_vp] * 9 + [_u32, _u64, _u32, _u32, C.c_float, _vp]),
     "nts_gat_fused_aggregate_backward": (_int, [_vp] * 13 + [_u32, _u32, _u32, C.c_float, _vp]),
     "nts_gat_fused_aggregate_backward_two_pass": (_int, [_vp] * 16 + [_u32, _u32, _u32, _u32, C.c_float, _vp]),
+    "nts_gat_fused_aggregate_forward_bf16": (_int, [_vp] * 9 + [_u32, _u64, _u32, _u32, _u32, C.c_float, _vp]),
+    "nts_gat_fused_aggregate_backward_two_pass_bf16": (_int, [_vp] * 16 + [_u32] * 5 + [C.c_float, _vp]),
+    "nts_rows_to_bf16": (_int, [_vp, _int, _u32, _vp, _u32, _u32, _u32, _vp]),
     "nts_deserialize_records": (_int, [_vp, _vp, _u32, _u32, _u32, _u32, _vp]),
     "nts_aggregate_records": (_int, [_vp, _vp, _u32, _u32, _u32, _u32, _vp]),
     "nts_gather_rows": (_int, [_vp, _vp, _vp, _u32, _u32, _vp]),

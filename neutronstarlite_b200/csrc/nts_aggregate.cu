@@ -29,6 +29,8 @@
 // per-vertex attention scores and softmax statistics (the fused GAT layer, nts_edge_ops.cu K7).
 // (U, MINB) per shape come from tools/tune_aggregate.py sweeps; NTS_AGG_TUNE / NTS_AGG_TILES are
 // measurement hooks read once at first launch, not product configuration.
+#include <type_traits>
+
 #include "nts_common.cuh"
 
 namespace nts {
@@ -38,10 +40,6 @@ static int g_edges_per_warp = 0;   // 0 = auto
 static int g_last_grid = 0, g_last_block = 0, g_last_smem = 0, g_last_variant = 0;
 
 // ---- small device helpers --------------------------------------------------------------------------------
-template <int VEC> __device__ __forceinline__ typename Vec<VEC>::type ldg_vec(const typename Vec<VEC>::type *p) {
-  return __ldg(p);
-}
-
 __device__ __forceinline__ void fma_vec(float &a, float w, float x) { a = fmaf(w, x, a); }
 __device__ __forceinline__ void fma_vec(float2 &a, float w, float2 x) {
   a.x = fmaf(w, x.x, a.x);
@@ -53,9 +51,17 @@ __device__ __forceinline__ void fma_vec(float4 &a, float w, float4 x) {
   a.z = fmaf(w, x.z, a.z);
   a.w = fmaf(w, x.w, a.w);
 }
+__device__ __forceinline__ void fma_vec(float8v &a, float w, float8v x) {
+  fma_vec(a.lo, w, x.lo);
+  fma_vec(a.hi, w, x.hi);
+}
 __device__ __forceinline__ void zero_vec(float &a) { a = 0.f; }
 __device__ __forceinline__ void zero_vec(float2 &a) { a = make_float2(0.f, 0.f); }
 __device__ __forceinline__ void zero_vec(float4 &a) { a = make_float4(0.f, 0.f, 0.f, 0.f); }
+__device__ __forceinline__ void zero_vec(float8v &a) {
+  zero_vec(a.lo);
+  zero_vec(a.hi);
+}
 
 __device__ __forceinline__ void rmw_add(float *p, float a) { *p = *p + a; }
 __device__ __forceinline__ void rmw_add(float2 *p, float2 a) {
@@ -72,6 +78,10 @@ __device__ __forceinline__ void rmw_add(float4 *p, float4 a) {
   o.w += a.w;
   *p = o;
 }
+__device__ __forceinline__ void rmw_add(float8v *p, float8v a) {
+  rmw_add(&p->lo, a.lo);
+  rmw_add(&p->hi, a.hi);
+}
 // no-return vector reductions (sm_90+): one L2 atomic transaction per 8/16 bytes
 __device__ __forceinline__ void red_add(float *p, float a) { atomicAdd(p, a); }
 __device__ __forceinline__ void red_add(float2 *p, float2 a) {
@@ -80,6 +90,10 @@ __device__ __forceinline__ void red_add(float2 *p, float2 a) {
 __device__ __forceinline__ void red_add(float4 *p, float4 a) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a.x), "f"(a.y), "f"(a.z), "f"(a.w)
                : "memory");
+}
+__device__ __forceinline__ void red_add(float8v *p, float8v a) {
+  red_add(&p->lo, a.lo);
+  red_add(&p->hi, a.hi);
 }
 
 // largest r in [0, n_rows) with off[r] <= e  (requires off[0] <= e < off[n_rows])
@@ -154,16 +168,21 @@ __device__ __forceinline__ float att_weight(float s, float d, float m, float inv
 // G    : virtual warps per warp (BULK only): rows of at most 16 vectors leave half of the lanes idle, so the warp is
 //        split into G independent groups of 32/G lanes, each with its own edge quantum and row state (the BULK
 //        variant has no warp-wide shuffles; all bookkeeping is per lane).  Used by the fused GAT layers (F = 64).
-template <int VEC, int K, int U, bool BULK, int MINB = 1, int HM = 0, int G = 1>
+// T    : gathered element type.  float, or __nv_bfloat16 for the fused GAT layer (HM == 2) with VEC = 8: one 16-byte
+//        load carries 8 BF16 values that are widened to FP32 in registers; F is then the BF16 row stride ld (a multiple
+//        of 8), which the FP32 output shares.
+template <int VEC, int K, int U, bool BULK, int MINB = 1, int HM = 0, int G = 1, class T = float>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, MINB)
-    segment_gather_sum_kernel(const float *__restrict__ in, float *__restrict__ out, const float *__restrict__ w,
+    segment_gather_sum_kernel(const T *__restrict__ in, float *__restrict__ out, const float *__restrict__ w,
                               const uint32_t *__restrict__ idx, const uint32_t *__restrict__ off,
                               const uint32_t *__restrict__ slot_of, uint32_t base, uint32_t n_rows,
                               uint64_t n_edges64, uint32_t F, uint32_t Q, uint32_t tiles, uint32_t tile_vecs,
                               uint32_t tile_major, uint32_t heads, AttParams att, uint32_t e_begin, uint32_t out_mod) {
   static_assert(!(HM == 1 && BULK), "[E, H] weight matrices are not bulk-staged (indices of HM 0 / 2 are)");
   static_assert(G == 1 || (BULK && K == 1), "virtual warps need the shuffle-free variant and one chunk per lane");
+  static_assert(std::is_same<T, float>::value || (HM == 2 && VEC == 8), "BF16 rows: fused GAT layer, 8 per chunk");
   using V = typename Vec<VEC>::type;
+  using L = typename Ld<T, VEC>::type; // what a lane loads per chunk (FP32: V itself)
   constexpr uint32_t GS = 32 / G;
   constexpr uint32_t kVW = kWarpsPerBlock * G; // (virtual) warps per CTA
   const uint32_t n_edges = (uint32_t)n_edges64;
@@ -326,7 +345,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MINB)
     uint32_t j = 0;
     // full groups of U edges: U*K independent vector loads per lane, then the FMAs
     for (; j + U <= cnt; j += U) {
-      V v[U][K];
+      L v[U][K];
       float wu[U][HM == 0 ? 1 : K];
 #pragma unroll
       for (int u = 0; u < U; u++) {
@@ -341,11 +360,11 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MINB)
           if constexpr (HM == 0)
             wu[u][0] = __shfl_sync(0xffffffffu, my_w, j + u);
         }
-        const V *p = reinterpret_cast<const V *>(in + (size_t)s * F) + c0;
+        const L *p = reinterpret_cast<const L *>(in + (size_t)s * F) + c0;
 #pragma unroll
         for (int k = 0; k < K; k++) {
           if (act[k])
-            v[u][k] = ldg_vec<VEC>(p + k * GS);
+            v[u][k] = __ldg(p + k * GS);
           if constexpr (HM == 1)
             wu[u][k] = act[k] ? __ldg(w + (size_t)(e + j + u) * heads + hk[k]) : 0.f;
           if constexpr (HM == 2)
@@ -360,7 +379,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MINB)
 #pragma unroll
         for (int k = 0; k < K; k++)
           if (act[k])
-            fma_vec(acc[k], weight_of(wu[u][HM == 0 ? 0 : k], k), v[u][k]);
+            fma_vec(acc[k], weight_of(wu[u][HM == 0 ? 0 : k], k), widen(v[u][k]));
       }
     }
     // remainder (< U edges)
@@ -377,12 +396,12 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MINB)
         if constexpr (HM == 0)
           wj[0] = __shfl_sync(0xffffffffu, my_w, j);
       }
-      const V *p = reinterpret_cast<const V *>(in + (size_t)s * F) + c0;
-      V v1[K];
+      const L *p = reinterpret_cast<const L *>(in + (size_t)s * F) + c0;
+      L v1[K];
 #pragma unroll
       for (int k = 0; k < K; k++) {
         if (act[k])
-          v1[k] = ldg_vec<VEC>(p + k * GS);
+          v1[k] = __ldg(p + k * GS);
         if constexpr (HM == 1)
           wj[k] = act[k] ? __ldg(w + (size_t)(e + j) * heads + hk[k]) : 0.f;
         if constexpr (HM == 2)
@@ -394,7 +413,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MINB)
 #pragma unroll
       for (int k = 0; k < K; k++)
         if (act[k])
-          fma_vec(acc[k], weight_of(wj[HM == 0 ? 0 : k], k), v1[k]);
+          fma_vec(acc[k], weight_of(wj[HM == 0 ? 0 : k], k), widen(v1[k]));
     }
   }
   // last row of the quantum: whole only if it started inside and also ends at/before e1
@@ -625,6 +644,91 @@ static int segment_gather_sum(const float *in, float *out, const float *w, const
   return fail(-1, "no kernel instantiation for this (vector width, chunks, U, occupancy) point", __FILE__, __LINE__);
 }
 
+// ---- K7 forward on BF16 mirror rows --------------------------------------------------------------------------------
+int check_gat_bf16_layout(uint32_t F, uint32_t ld, uint32_t heads) {
+  NTS_ARG_CHECK(heads >= 1 && F % heads == 0, "feature_size must be a multiple of heads");
+  NTS_ARG_CHECK(ld % 8 == 0 && ld >= F, "BF16 rows need a stride ld >= feature_size with ld % 8 == 0");
+  NTS_ARG_CHECK(heads == 1 || ((F / heads) % 8 == 0 && ld == F),
+                "BF16 rows with heads > 1 need a head width D % 8 == 0 (a 16-byte chunk never straddles two heads) "
+                "and ld == feature_size");
+  return 0;
+}
+
+template <int K, int U, int G>
+static int launch_gat_bf16(const LaunchShape &sh, const __nv_bfloat16 *in, float *out, const uint32_t *idx,
+                           const uint32_t *off, const uint32_t *slot_of, uint32_t n_rows, uint64_t n_edges,
+                           uint32_t ld, uint32_t Q, const AttParams &att, cudaStream_t st) {
+  constexpr uint32_t kVW = kWarpsPerBlock * G;
+  const uint64_t warps = (n_edges + Q - 1) / Q * sh.tiles;
+  const uint64_t blocks = (warps + kVW - 1) / kVW;
+  NTS_ARG_CHECK(blocks <= 0x7fffffffull, "aggregation grid too large");
+  const size_t smem = 16 + 2 * ((size_t)kVW * Q + 8) * 4;
+  auto kern = segment_gather_sum_kernel<8, K, U, true, 1, 2, G, __nv_bfloat16>;
+  NTS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  g_last_grid = (int)blocks;
+  g_last_block = kWarpsPerBlock * 32;
+  g_last_smem = (int)smem;
+  g_last_variant = 2;
+  kern<<<(unsigned)blocks, kWarpsPerBlock * 32, smem, st>>>(in, out, nullptr, idx, off, slot_of, 0, n_rows, n_edges,
+                                                            ld, Q, sh.tiles, sh.tile_vecs, 0, sh.heads, att, 0, 0);
+  NTS_LAUNCH_CHECK();
+  return 0;
+}
+
+// Chunks of 8 values: K <= 4 chunks per lane per column tile; rows of at most 16 / 8 chunks (F <= 128 / 64) split the
+// warp into G = 2 / 4 virtual warps (config D's 64-wide layers are 8 chunks: one head of 8 per lane at D = 8).
+// NTS_GAT_BF16_TUNE="U,G" is a measurement hook (tools/gat_dtype_sweep.py --tune) for the one-chunk rows.
+static int gat_forward_bf16(const __nv_bfloat16 *in, float *out, const uint32_t *idx, const uint32_t *off,
+                            const uint32_t *slot_of, uint32_t n_rows, uint64_t n_edges, uint32_t ld,
+                            uint32_t heads, const AttParams &att, cudaStream_t st) {
+  LaunchShape s;
+  s.heads = heads;
+  s.vec = 8;
+  const uint32_t nvec = ld / 8;
+  const uint32_t chunks = (nvec + 31) / 32;
+  s.tiles = (chunks + 3) / 4;
+  s.tile_vecs = (nvec + s.tiles - 1) / s.tiles;
+  s.k = (int)((s.tile_vecs + 31) / 32);
+  s.tiles = (nvec + s.tile_vecs - 1) / s.tile_vecs;
+  s.tile_major = 0;
+  s.minb = 1;
+  s.g = (s.k == 1 && s.tiles == 1) ? (nvec <= 8 ? 4 : (nvec <= 16 ? 2 : 1)) : 1;
+  // U measured on config D's one-chunk rows (H100 SXM, 700 W, tools/gat_dtype_sweep.py --tune): G = 4 at U = 2 / 4 / 8
+  // 4.63 / 4.80 / 5.47 ms per 64-wide call, 3.59 / 3.69 / 4.34 ms at 41 wide; G = 2 and G = 1 are slower at every U
+  s.u = s.k == 1 ? 2 : (s.k == 2 ? 4 : 2);
+  if (const char *tune = getenv("NTS_GAT_BF16_TUNE")) {
+    int tu = 0, tg = 0;
+    if (s.k == 1 && s.tiles == 1 && sscanf(tune, "%d,%d", &tu, &tg) == 2 && tg >= 1 && (uint32_t)(32 / tg) >= nvec) {
+      s.u = tu;
+      s.g = tg;
+    }
+  }
+  uint32_t Q = 512u / (uint32_t)s.g; // edges per (virtual) warp, shrunk for small inputs as in segment_gather_sum
+  const uint64_t want_warps = (uint64_t)sm_count() * 64;
+  while (Q > 32 && ((n_edges + Q - 1) / Q) * s.tiles < want_warps)
+    Q >>= 1;
+  Q = (Q + 31u) & ~31u;
+  if (Q * s.g > 1024)
+    Q = (1024u / s.g) & ~31u;
+#define NTS_GAT16(K_, U_, G_)                                                                                    \
+  if (s.k == K_ && s.u == U_ && s.g == G_)                                                                       \
+    return launch_gat_bf16<K_, U_, G_>(s, in, out, idx, off, slot_of, n_rows, n_edges, ld, Q, att, st);
+  NTS_GAT16(1, 2, 1)
+  NTS_GAT16(1, 4, 1)
+  NTS_GAT16(1, 8, 1)
+  NTS_GAT16(1, 2, 2)
+  NTS_GAT16(1, 4, 2)
+  NTS_GAT16(1, 8, 2)
+  NTS_GAT16(1, 2, 4)
+  NTS_GAT16(1, 4, 4)
+  NTS_GAT16(1, 8, 4)
+  NTS_GAT16(2, 4, 1)
+  NTS_GAT16(3, 2, 1)
+  NTS_GAT16(4, 2, 1)
+#undef NTS_GAT16
+  return fail(-1, "no BF16 fused-GAT instantiation for this (chunks, U, virtual warps) point", __FILE__, __LINE__);
+}
+
 } // namespace nts
 
 extern "C" {
@@ -672,6 +776,26 @@ int nts_gat_fused_aggregate_forward(const float *mirror, float *output, const fl
   nts::AttParams att = {src_score, dst_score, seg_max, seg_sum, negative_slope};
   return nts::segment_gather_sum(mirror, output, nullptr, row_indices, column_offset, mirror_index, 0, batch_size,
                                  n_edges, feature_size, nts::as_stream(stream), heads, &att);
+}
+
+int nts_gat_fused_aggregate_forward_bf16(const void *mirror, float *output, const float *src_score,
+                                         const float *dst_score, const float *seg_max, const float *seg_sum,
+                                         const nts_vid_t *row_indices, const nts_vid_t *column_offset,
+                                         const nts_vid_t *mirror_index, nts_vid_t batch_size, uint64_t n_edges,
+                                         nts_vid_t feature_size, nts_vid_t ld, nts_vid_t heads, float negative_slope,
+                                         void *stream) {
+  if (const int rc = nts::check_gat_bf16_layout(feature_size, ld, heads))
+    return rc;
+  if (batch_size == 0 || n_edges == 0 || feature_size == 0)
+    return 0;
+  NTS_ARG_CHECK(mirror && output && src_score && dst_score && seg_max && seg_sum && row_indices && column_offset,
+                "null pointer passed to fused GAT forward (BF16)");
+  NTS_ARG_CHECK(nts::aligned_to(mirror, 16) && nts::aligned_to(output, 16) && nts::aligned_to(row_indices, 16),
+                "BF16 fused GAT forward needs 16-byte aligned mirror, output and row_indices");
+  NTS_ARG_CHECK(n_edges < 0xffffffffull, "chunk edge count must fit uint32 offsets");
+  nts::AttParams att = {src_score, dst_score, seg_max, seg_sum, negative_slope};
+  return nts::gat_forward_bf16(static_cast<const __nv_bfloat16 *>(mirror), output, row_indices, column_offset,
+                               mirror_index, batch_size, n_edges, ld, heads, att, nts::as_stream(stream));
 }
 
 int nts_gather_by_dst_from_src(const float *input, float *output, const float *weight_forward,

@@ -1,5 +1,6 @@
 // Shared helpers of libnts_b200: error handling, launch accounting, vector types.
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -57,10 +58,38 @@ int run_plan_bf16(nts_gather_plan *pl, const void *input, int dtype, uint32_t ld
 int to_bf16_rows(const void *src, int dtype, uint32_t lds, void *dst, uint32_t n_rows, uint32_t F, uint32_t ld,
                  cudaStream_t st);
 
+// BF16 layout rule of the fused GAT layer (K7): rows of ld values, ld % 8 == 0 and >= F; with heads > 1 every head is a
+// whole number of 16-byte chunks (D % 8 == 0) and ld == F.  Returns 0 or the argument error.
+int check_gat_bf16_layout(uint32_t F, uint32_t ld, uint32_t heads);
+
+struct __align__(16) float8v {
+  float4 lo, hi;
+};
+
 template <int VEC> struct Vec;
 template <> struct Vec<1> { using type = float; };
 template <> struct Vec<2> { using type = float2; };
 template <> struct Vec<4> { using type = float4; };
+template <> struct Vec<8> { using type = float8v; };
+
+// What one lane loads for VEC values of a row of element type T, and widen(), which turns it into the FP32 vector
+// Vec<VEC>.  A BF16 value is the upper half of the FP32 with the same bits, so widening is exact (one shift or mask);
+// for FP32 rows both are the identity.
+template <class T, int VEC> struct Ld { using type = typename Vec<VEC>::type; };
+template <> struct Ld<__nv_bfloat16, 2> { using type = uint32_t; };
+template <> struct Ld<__nv_bfloat16, 4> { using type = uint2; };
+template <> struct Ld<__nv_bfloat16, 8> { using type = uint4; };
+__device__ __forceinline__ float widen(float v) { return v; }
+__device__ __forceinline__ float2 widen(float2 v) { return v; }
+__device__ __forceinline__ float4 widen(float4 v) { return v; }
+__device__ __forceinline__ float2 widen(uint32_t u) {
+  return make_float2(__uint_as_float(u << 16), __uint_as_float(u & 0xffff0000u));
+}
+__device__ __forceinline__ float4 widen(uint2 u) {
+  const float2 a = widen(u.x), b = widen(u.y);
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ float8v widen(uint4 u) { return {widen(make_uint2(u.x, u.y)), widen(make_uint2(u.z, u.w))}; }
 
 } // namespace nts
 

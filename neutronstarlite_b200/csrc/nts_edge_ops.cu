@@ -43,22 +43,35 @@ template <> __device__ __forceinline__ void vec_red_add<4>(float4 *p, float4 a) 
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a.x), "f"(a.y), "f"(a.z), "f"(a.w)
                : "memory");
 }
+template <> __device__ __forceinline__ void vec_red_add<8>(float8v *p, float8v a) {
+  vec_red_add<4>(&p->lo, a.lo);
+  vec_red_add<4>(&p->hi, a.hi);
+}
 __device__ __forceinline__ float vec_dot(float a, float b) { return a * b; }
 __device__ __forceinline__ float vec_dot(float2 a, float2 b) { return fmaf(a.x, b.x, a.y * b.y); }
 __device__ __forceinline__ float vec_dot(float4 a, float4 b) {
   return fmaf(a.x, b.x, fmaf(a.y, b.y, fmaf(a.z, b.z, a.w * b.w)));
 }
+__device__ __forceinline__ float vec_dot(float8v a, float8v b) {
+  return fmaf(a.lo.x, b.lo.x, fmaf(a.lo.y, b.lo.y, fmaf(a.lo.z, b.lo.z, fmaf(a.lo.w, b.lo.w, vec_dot(a.hi, b.hi)))));
+}
 __device__ __forceinline__ float vec_scale(float a, float s) { return a * s; }
 __device__ __forceinline__ float2 vec_scale(float2 a, float s) { return make_float2(a.x * s, a.y * s); }
 __device__ __forceinline__ float4 vec_scale(float4 a, float s) { return make_float4(a.x * s, a.y * s, a.z * s, a.w * s); }
+__device__ __forceinline__ float8v vec_scale(float8v a, float s) { return {vec_scale(a.lo, s), vec_scale(a.hi, s)}; }
 __device__ __forceinline__ void vec_zero(float &a) { a = 0.f; }
 __device__ __forceinline__ void vec_zero(float2 &a) { a = make_float2(0.f, 0.f); }
 __device__ __forceinline__ void vec_zero(float4 &a) { a = make_float4(0.f, 0.f, 0.f, 0.f); }
+__device__ __forceinline__ void vec_zero(float8v &a) {
+  vec_zero(a.lo);
+  vec_zero(a.hi);
+}
 __device__ __forceinline__ float vec_add(float a, float b) { return a + b; }
 __device__ __forceinline__ float2 vec_add(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ float4 vec_add(float4 a, float4 b) {
   return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
 }
+__device__ __forceinline__ float8v vec_add(float8v a, float8v b) { return {vec_add(a.lo, b.lo), vec_add(a.hi, b.hi)}; }
 
 // ---- row movers ------------------------------------------------------------------------------------------
 // mode 0: dst[r,:]        = src[map(r),:]
@@ -673,15 +686,18 @@ __global__ void __launch_bounds__(kThreads)
 // VEC floats per lane load, KB chunks of 32 vectors per row, U edges gathered before any arithmetic.
 // ONEHEAD: heads == 1, any row width (the dot product is a full-warp sum); otherwise a head is a power-of-two number
 // of vectors <= 32 and per-head dots are segmented xor-shuffle sums (lanes of one head are contiguous).
-template <int VEC, int KB, int U, bool SRC_MAJOR, bool ONEHEAD>
+// T: element type of `gathered` and `row_vals` (float, or __nv_bfloat16 with VEC in {2, 4, 8}: the rows are widened to
+// FP32 in registers; F is then the BF16 row stride ld, which the FP32 `vec_out` shares).  Everything else is FP32.
+template <int VEC, int KB, int U, bool SRC_MAJOR, bool ONEHEAD, class T = float>
 __global__ void __launch_bounds__(kThreads)
     gat_backward_pass_kernel(float *__restrict__ vec_out, float *__restrict__ score_out,
-                             const float *__restrict__ gathered, const float *__restrict__ row_vals,
+                             const T *__restrict__ gathered, const T *__restrict__ row_vals,
                              const float *__restrict__ src_score, const float4 *__restrict__ dst_pack,
                              const uint32_t *__restrict__ col, const uint32_t *__restrict__ off,
                              const uint32_t *__restrict__ col_map, uint32_t n_rows, uint32_t F, uint32_t H,
                              float slope) {
   using V = typename Vec<VEC>::type;
+  using L = typename Ld<T, VEC>::type; // what a lane loads per vector (FP32: V itself)
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t nvec = F / VEC;
   const uint32_t head_vecs = ONEHEAD ? 32u : nvec / H;
@@ -704,12 +720,12 @@ __global__ void __launch_bounds__(kThreads)
     float rs[KB], acc[KB];
     float4 rp[KB];
     auto load_row = [&]() {
-      const V *yr = reinterpret_cast<const V *>(row_vals + (size_t)row * F);
+      const L *yr = reinterpret_cast<const L *>(row_vals + (size_t)row * F);
 #pragma unroll
       for (int k = 0; k < KB; k++) {
         acc[k] = 0.f;
         if (act[k])
-          yv[k] = __ldg(yr + lane + 32 * k);
+          yv[k] = widen(__ldg(yr + lane + 32 * k));
         if constexpr (SRC_MAJOR) {
           rs[k] = __ldg(src_score + (size_t)row * H + hk[k]);
           vec_zero(mg[k]);
@@ -750,13 +766,13 @@ __global__ void __launch_bounds__(kThreads)
           my_idx = __ldg(col_map + my_idx);
       }
       for (uint32_t j = 0; j < cnt; j += U) {
-        V xv[U][KB];
+        L xv[U][KB];
         float es[U][KB];
         float4 ep[U][KB];
 #pragma unroll
         for (int u = 0; u < U; u++) {
           const uint32_t idx = __shfl_sync(0xffffffffu, my_idx, min(j + u, cnt - 1));
-          const V *xr = reinterpret_cast<const V *>(gathered + (size_t)idx * F);
+          const L *xr = reinterpret_cast<const L *>(gathered + (size_t)idx * F);
 #pragma unroll
           for (int k = 0; k < KB; k++) {
             if (act[k])
@@ -784,7 +800,7 @@ __global__ void __launch_bounds__(kThreads)
           float dotk[KB];
 #pragma unroll
           for (int k = 0; k < KB; k++)
-            dotk[k] = act[k] ? vec_dot(xv[u][k], yv[k]) : 0.f;
+            dotk[k] = act[k] ? vec_dot(widen(xv[u][k]), yv[k]) : 0.f;
           if constexpr (ONEHEAD) {
             float t = dotk[0];
 #pragma unroll
@@ -808,7 +824,7 @@ __global__ void __launch_bounds__(kThreads)
             const float a = expf(leaky(pre, slope) - pk.y);
             if constexpr (SRC_MAJOR) {
               if (act[k])
-                mg[k] = vec_add(mg[k], vec_scale(xv[u][k], a));
+                mg[k] = vec_add(mg[k], vec_scale(widen(xv[u][k]), a));
             }
             acc[k] += a * (dotk[k] - pk.z) * (pre > 0.f ? 1.f : slope);
           }
@@ -1237,6 +1253,89 @@ int nts_gat_fused_aggregate_backward_two_pass(float *mirror_grad, float *src_sco
 #undef NTS_GAT2_V
 #undef NTS_GAT2_K
 #undef NTS_GAT2
+  NTS_LAUNCH_CHECK();
+  return 0;
+}
+
+int nts_gat_fused_aggregate_backward_two_pass_bf16(float *mirror_grad, float *src_score_grad, float *dst_score_grad,
+                                                   float *dst_pack, const void *mirror, const float *src_score,
+                                                   const float *dst_score, const float *seg_max, const float *seg_sum,
+                                                   const float *out_dot_grad, const void *dst_grad,
+                                                   const nts_vid_t *row_indices, const nts_vid_t *column_offset,
+                                                   const nts_vid_t *mirror_index, const nts_vid_t *slot_row_offset,
+                                                   const nts_vid_t *slot_column_indices, nts_vid_t batch_size,
+                                                   nts_vid_t mirror_size, nts_vid_t feature_size, nts_vid_t ld,
+                                                   nts_vid_t heads, float negative_slope, void *stream) {
+  if (const int rc = check_gat_bf16_layout(feature_size, ld, heads))
+    return rc;
+  // the shape rule of the FP32 passes on rows of ld BF16 values: 2, 4 or 8 values per lane (as wide as keeps 32 lanes
+  // busy), a power-of-two number of vectors per head (<= 32) and at most 4 chunks per lane; there is no fallback
+  int vec = 8;
+  while (vec > 2 && ld / vec < 32)
+    vec >>= 1;
+  const uint32_t nvec = ld / vec, hv = nvec / heads;
+  const uint32_t kb = (nvec + 31) / 32;
+  const bool one = heads == 1;
+  NTS_ARG_CHECK(kb <= 4 && (one || (hv >= 1 && (hv & (hv - 1)) == 0 && hv <= 32)),
+                "no BF16 two-pass GAT backward for this shape (heads > 1 need a power-of-two number of vectors per "
+                "head, rows at most 1024 values)");
+  cudaStream_t st = as_stream(stream);
+  if (batch_size == 0 || feature_size == 0 || mirror_size == 0)
+    return 0;
+  NTS_ARG_CHECK(mirror_grad && src_score_grad && dst_score_grad && dst_pack && mirror && src_score && dst_score &&
+                    seg_max && seg_sum && out_dot_grad && dst_grad && row_indices && column_offset &&
+                    slot_row_offset && slot_column_indices,
+                "null pointer passed to fused GAT backward (two pass, BF16)");
+  NTS_ARG_CHECK(aligned_to(mirror_grad, 16) && aligned_to(mirror, 16) && aligned_to(dst_grad, 16) &&
+                    aligned_to(dst_pack, 16),
+                "BF16 fused GAT backward needs 16-byte aligned mirror_grad, mirror, dst_grad and dst_pack");
+  const uint64_t n_pack = (uint64_t)batch_size * heads;
+  gat_pack_dst_kernel<<<stream_grid((n_pack + kThreads - 1) / kThreads), kThreads, 0, st>>>(
+      reinterpret_cast<float4 *>(dst_pack), dst_score, seg_max, seg_sum, out_dot_grad, n_pack);
+  NTS_LAUNCH_CHECK();
+  const unsigned grid = full_grid();
+  const float4 *pk = reinterpret_cast<const float4 *>(dst_pack);
+  const __nv_bfloat16 *m16 = static_cast<const __nv_bfloat16 *>(mirror);
+  const __nv_bfloat16 *g16 = static_cast<const __nv_bfloat16 *>(dst_grad);
+#define NTS_GAT2B(V_, K_, UD_, US_, ONE_)                                                                            \
+  do {                                                                                                               \
+    gat_backward_pass_kernel<V_, K_, UD_, false, ONE_, __nv_bfloat16><<<grid, kThreads, 0, st>>>(                    \
+        nullptr, dst_score_grad, m16, g16, src_score, pk, row_indices, column_offset, mirror_index, batch_size, ld,   \
+        heads, negative_slope);                                                                                      \
+    count_launch();                                                                                                  \
+    gat_backward_pass_kernel<V_, K_, US_, true, ONE_, __nv_bfloat16><<<grid, kThreads, 0, st>>>(                     \
+        mirror_grad, src_score_grad, g16, m16, src_score, pk, slot_column_indices, slot_row_offset, nullptr,         \
+        mirror_size, ld, heads, negative_slope);                                                                     \
+  } while (0)
+  // vec = 2 / 4 only on rows of fewer than 128 / 256 values (kb <= 2); vec = 8 for the wider ones.  U per pass is the
+  // FP32 choice except where that point spills with BF16 rows (single-head passes: dst-major VEC 2 x KB 1 at U = 8,
+  // src-major 2 x 2 and 8 x 2 at U = 4, all spill-free)
+#define NTS_GAT2B_ONE(ONE_)                                                                                          \
+  do {                                                                                                               \
+    if (vec == 2) {                                                                                                  \
+      if (kb == 1)                                                                                                   \
+        NTS_GAT2B(2, 1, ONE_ ? 8 : 4, 4, ONE_);                                                                      \
+      else                                                                                                           \
+        NTS_GAT2B(2, 2, 2, ONE_ ? 4 : 2, ONE_);                                                                      \
+    } else if (vec == 4) {                                                                                           \
+      if (kb == 1)                                                                                                   \
+        NTS_GAT2B(4, 1, 4, 4, ONE_);                                                                                 \
+      else                                                                                                           \
+        NTS_GAT2B(4, 2, 2, 2, ONE_);                                                                                 \
+    } else if (kb == 1) {                                                                                            \
+      NTS_GAT2B(8, 1, 4, 4, ONE_);                                                                                   \
+    } else if (kb == 2) {                                                                                            \
+      NTS_GAT2B(8, 2, 2, ONE_ ? 4 : 2, ONE_);                                                                        \
+    } else {                                                                                                         \
+      NTS_GAT2B(8, 4, 1, 1, ONE_);                                                                                   \
+    }                                                                                                                \
+  } while (0)
+  if (one)
+    NTS_GAT2B_ONE(true);
+  else
+    NTS_GAT2B_ONE(false);
+#undef NTS_GAT2B_ONE
+#undef NTS_GAT2B
   NTS_LAUNCH_CHECK();
   return 0;
 }

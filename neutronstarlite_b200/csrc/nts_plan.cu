@@ -1724,6 +1724,12 @@ int nts_gather_plan_run_bf16(nts_gather_plan *pl, const void *input, int input_d
   return run_plan_bf16(pl, input, input_dtype, feature_size, output, feature_size, as_stream(stream));
 }
 
+int nts_rows_to_bf16(const void *src, int src_dtype, nts_vid_t lds, void *dst, nts_vid_t n_rows, nts_vid_t feature_size,
+                     nts_vid_t ld, void *stream) {
+  NTS_ARG_CHECK((src && dst) || n_rows == 0 || feature_size == 0, "null pointer passed to nts_rows_to_bf16");
+  return to_bf16_rows(src, src_dtype, lds, dst, n_rows, feature_size, ld, as_stream(stream));
+}
+
 int nts_gather_plan_set_variant(int variant) {
   NTS_ARG_CHECK(variant == 0 || variant == 1, "variant must be 0 (register staging) or 1 (TMA row staging)");
   g_plan_variant = variant;

@@ -500,12 +500,21 @@ class DistGPUFusedGATOp(_EdgeOp):
             a[e,h] = softmax over the in-edges of dst(e) of leaky_relu(src_score[slot(e),h] + dst_score[dst(e),h])
             out[d, hD:(h+1)D] = sum_e a[e,h] * mirror[slot(e), hD:(h+1)D]
         backward(grad_out) -> (d_mirror, d_src_score, d_dst_score)
+
+    gather_dtype=torch.bfloat16: the aggregation and both backward passes gather BF16 rows with FP32 accumulation.  The
+    forward rounds the FP32 mirror once into m~ = bf16(mirror), the backward rounds grad_out once into g~; the layer then
+    computes the FP32 layer's function and gradients at m~ and g~ (include/nts_b200.h).  Scores, softmax statistics,
+    out, d_mirror and the score gradients stay float32.  Needs two_pass_backward=True, and with heads > 1 a head width
+    D that is a multiple of 8; other shapes raise NtsError.
     """
 
-    def __init__(self, partitioned_graph, active=None, negative_slope=0.2, two_pass_backward=True):
+    def __init__(self, partitioned_graph, active=None, negative_slope=0.2, two_pass_backward=True, gather_dtype=None):
         super().__init__(partitioned_graph, active)
         self.slope = float(negative_slope)
         self.two_pass_backward = bool(two_pass_backward)
+        self.gather_dtype = _check_gather_dtype(gather_dtype)
+        if self.gather_dtype is not None and not self.two_pass_backward:
+            raise _lib.NtsError("BF16 gathers of the fused GAT layer need two_pass_backward=True")
         self._saved = None
 
     @staticmethod
@@ -549,6 +558,8 @@ class DistGPUFusedGATOp(_EdgeOp):
             _lib.call("nts_gat_softmax_stats", _ptr(seg_max), _ptr(seg_sum), _ptr(s), _ptr(d), _ptr(slots),
                       _ptr(pg.column_offset_gpu), 0, pg.owned_vertices, H, self.slope, _stream())
         F = int(x.shape[1])
+        if self.gather_dtype is not None:
+            return self._forward_bf16(pg, x, s, d, seg_max, seg_sum, slots, H, F)
         xk, Fk = x, F
         if H == 1 and F % 4 != 0:
             # odd single-head width (the 41-wide output layer of config D): gather from a copy padded to a multiple
@@ -566,9 +577,58 @@ class DistGPUFusedGATOp(_EdgeOp):
         self._saved = (x, s, d, seg_max, seg_sum, out)
         return out
 
+    @staticmethod
+    def _to_bf16_rows(t, ld):
+        """bf16(t) as rows of ld values, the columns past t's width zero (nts_rows_to_bf16)."""
+        n, F = t.shape
+        r = torch.empty((n, ld), dtype=torch.bfloat16, device=t.device)
+        with _timed("gat_bf16_round", F, 0, n):
+            _lib.call("nts_rows_to_bf16", _ptr(t), _DTYPE_CODE[torch.float32], F, _ptr(r), n, F, ld, _stream())
+        return r
+
+    def _forward_bf16(self, pg, x, s, d, seg_max, seg_sum, slots, H, F):
+        # rows of ld = ceil(F/8)*8 BF16 values: 16-byte chunks of 8, and for the 41-wide layer this replaces the
+        # padded FP32 copy of the FP32 path; out shares the row stride and loses its zero pad columns below
+        ld = (F + 7) // 8 * 8
+        mt = self._to_bf16_rows(x, ld)
+        out = torch.zeros((pg.owned_vertices, ld), dtype=torch.float32, device=x.device)
+        with _timed("gat_fwd", F, pg.owned_edges, pg.owned_vertices):
+            _lib.call("nts_gat_fused_aggregate_forward_bf16", _ptr(mt), _ptr(out), _ptr(s), _ptr(d), _ptr(seg_max),
+                      _ptr(seg_sum), _ptr(slots), _ptr(pg.column_offset_gpu), 0, pg.owned_vertices, pg.owned_edges,
+                      F, ld, H, self.slope, _stream())
+        if ld != F:
+            out = out[:, :F].contiguous()
+        self._saved = (mt, s, d, seg_max, seg_sum, out)   # m~ is what the backward gathers: the FP32 mirror is not kept
+        return out
+
+    def _backward_bf16(self, pg, g):
+        mt, s, d, seg_max, seg_sum, out = self._saved
+        H = int(s.shape[1])
+        M, ld = mt.shape
+        F = int(out.shape[1])
+        gt = self._to_bf16_rows(g, ld)
+        # <out, g~>, not <out, g>: the passes rely on sum_e a <m~, g~> == <out, g~>; mixing g and g~ would bias the
+        # score gradients by about 2^-8
+        out_dot_g = (out.detach() * gt[:, :F].float()).view(-1, H, F // H).sum(-1).contiguous()
+        dm = torch.zeros((M, ld), dtype=torch.float32, device=g.device)
+        ds = torch.zeros_like(s)
+        dd = torch.zeros_like(d)
+        slot_off, slot_dst = self.slot_csr(pg)
+        pack = torch.empty((pg.owned_vertices, H, 4), dtype=torch.float32, device=g.device)
+        with _timed("gat_bwd", F, 2 * pg.owned_edges, pg.owned_vertices):
+            _lib.call("nts_gat_fused_aggregate_backward_two_pass_bf16", _ptr(dm), _ptr(ds), _ptr(dd), _ptr(pack),
+                      _ptr(mt), _ptr(s), _ptr(d), _ptr(seg_max), _ptr(seg_sum), _ptr(out_dot_g), _ptr(gt),
+                      _ptr(self.slot_indices(pg)), _ptr(pg.column_offset_gpu), 0, _ptr(slot_off), _ptr(slot_dst),
+                      pg.owned_vertices, M, F, ld, H, self.slope, _stream())
+        if ld != F:
+            dm = dm[:, :F].contiguous()
+        return dm, ds, dd
+
     def backward(self, f_output_grad):
         pg = self._topo()
         g = _check_input(f_output_grad, "output_grad")
+        if self.gather_dtype is not None:
+            return self._backward_bf16(pg, g)
         x, s, d, seg_max, seg_sum, out = self._saved
         H = int(s.shape[1])
         D = x.shape[1] // H

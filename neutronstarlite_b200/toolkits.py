@@ -18,7 +18,7 @@ import torch
 import torch.distributed as dist
 
 from .context import NtsContext
-from . import ops
+from . import _lib, ops
 
 
 class Parameter:
@@ -233,14 +233,21 @@ class GATImpl:
     attention scores -> [E, H] edge logits -> edge softmax -> DistAggregateDstFuseWeight) on the GPU operators, with
     H heads (the reference has one).  `layers` are total widths, e.g. [602, 64, 64, 41] with heads=8 gives hidden
     layers of 8 heads x 8 and a single-head output layer (config D of BASELINE.json).  Never materialises an [E, F]
-    message; the only edge-sized tensors are [E, H]."""
+    message; the only edge-sized tensors are [E, H].
+
+    gather_dtype=torch.bfloat16 (needs fused_kernel=True and two_pass_backward=True): every fused layer gathers BF16
+    mirror and gradient rows with FP32 accumulation (ops.DistGPUFusedGATOp's option).  The input features stay float32
+    (they feed the first GEMM), and so do the mirror fetch, activations, weights and gradients."""
 
     def __init__(self, partitioned_graph, layers, features, labels, mask, heads=8, learn_rate=0.01,
                  weight_decay=0.0001, exchange=None, seed=0, sum_fanout_grads=True, fused_kernel=False,
-                 two_pass_backward=True):
+                 two_pass_backward=True, gather_dtype=None):
         self.pg = partitioned_graph
         self.fused_kernel = fused_kernel  # True: K7 (ops.DistGPUFusedGATOp), no edge-sized tensors at all
         self.two_pass_backward = two_pass_backward
+        self.gather_dtype = ops._check_gather_dtype(gather_dtype)
+        if self.gather_dtype is not None and not (fused_kernel and two_pass_backward):
+            raise _lib.NtsError("GATImpl gather_dtype needs fused_kernel=True and two_pass_backward=True")
         self.layers = list(layers)
         self.device = features.device
         self.heads = [heads] * (len(self.layers) - 2) + [1]
@@ -286,7 +293,7 @@ class GATImpl:
                 lambda x, _i=i: (x.view(-1, H, D) * self.ar[_i].W).sum(-1).contiguous(), X_trans)
             if self.fused_kernel:
                 nbr = ctx.runGraphOpN(ops.DistGPUFusedGATOp, pg, None, [mirror, src_att, dst_att],
-                                      two_pass_backward=self.two_pass_backward)
+                                      two_pass_backward=self.two_pass_backward, gather_dtype=self.gather_dtype)
             else:
                 e_src = ctx.runGraphOp(ops.DistGPUScatterSrc, pg, None, src_att)
                 e_dst = ctx.runGraphOp(ops.DistGPUScatterDst, pg, None, dst_att)
