@@ -151,6 +151,11 @@ float nts_gather_plan_tuned_ms(const nts_gather_plan *plan); /* time of the winn
 int nts_gather_plan_destroy(nts_gather_plan *plan);
 int nts_gather_plan_slabs(const nts_gather_plan *plan);
 int nts_gather_plan_hubs(const nts_gather_plan *plan, int *cols, int *rows); /* hub columns / rows of the plan */
+/* Schedule of the hub-row block: 0 = its own launch before the slab launches, 1 = its tiles run inside the slab
+ * launches that gather the same rows (it writes only hub rows, which have no residual edges).  Measured plans pick the
+ * faster (NTS_PLAN_OVERLAP=0 forces 0); other plans start at 0.  Plans without hub rows ignore it. */
+int nts_gather_plan_overlap(const nts_gather_plan *plan);
+int nts_gather_plan_set_overlap(nts_gather_plan *plan, int overlap);
 uint64_t nts_gather_plan_bytes(const nts_gather_plan *plan);
 /* output[r,:] += sum_e input[row(e),:] * w(e)   (accumulates; one launch per non-empty slab, in stream order) */
 int nts_gather_plan_run(nts_gather_plan *plan, const float *input, float *output, nts_vid_t feature_size,

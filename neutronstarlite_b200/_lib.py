@@ -58,6 +58,8 @@ SIGNATURES = {
     "nts_gather_plan_destroy": (_int, [_vp]),
     "nts_gather_plan_slabs": (_int, [_vp]),
     "nts_gather_plan_hubs": (_int, [_vp, C.POINTER(_int), C.POINTER(_int)]),
+    "nts_gather_plan_overlap": (_int, [_vp]),
+    "nts_gather_plan_set_overlap": (_int, [_vp, _int]),
     "nts_gather_plan_bytes": (_u64, [_vp]),
     "nts_gather_plan_run": (_int, [_vp, _vp, _vp, _u32, _vp]),
     "nts_gather_plan_run_bf16": (_int, [_vp, _vp, _int, _vp, _u32, _vp]),

@@ -58,6 +58,7 @@ struct nts_gather_plan {
   uint32_t lda_c = 0, lda_r = 0;   // n_rows / hub_rows rounded up to a multiple of 4 (16-byte operand rows)
   float *dense = nullptr;          // D_c^T [hub_cols x lda_c], then D_r^T [gather_rows x lda_r]: summed edge weights
   size_t dense_floats = 0;
+  int overlap = 0;                 // 1: the row block runs inside the slab launches (planned_slab_hub_kernel)
   int last_grid = 0, last_launches = 0, last_k = 0, last_u = 0, last_outv = 0;
   float tuned_ms = 0.f;        // nts_gather_plan_create_tuned: time of the winning candidate
 };
@@ -360,30 +361,31 @@ template <> struct GatherT<__nv_bfloat16> {
 //        of the lanes idle, so a warp is split into G independent groups of 32/G lanes, each with its own edge quantum,
 //        row bookkeeping and accumulators (the kernel has no warp-wide shuffles: all state is per lane already).
 // Warp g owns the edge quantum [e_begin + q*Q, ...) of column tile t (g = q*tiles + t); the (row, weight) pairs of the
-// CTA's edge span are staged in shared memory by one cp.async.bulk, completion on an mbarrier.
-template <class T, int K, int U, int OUTV, int MINB, int G = 1>
-__global__ void __launch_bounds__(kPlanWarps * 32, MINB)
-    planned_gather_sum_kernel(const typename GatherT<T>::chunk *__restrict__ in, uint32_t ldc, float *__restrict__ out,
-                              uint32_t F, const uint2 *__restrict__ pairs, const uint32_t *__restrict__ off,
-                              uint32_t n_rows, uint32_t e_begin, uint32_t e_end, uint32_t Q, uint32_t tiles,
-                              uint32_t tile_vecs) {
+// CTA's edge span are staged in shared memory by one cp.async.bulk, completion on an mbarrier.  `vblock` is the CTA's
+// index among the gather CTAs of the launch (blockIdx.x in planned_gather_sum_kernel).
+template <class T, int K, int U, int OUTV, int G>
+__device__ __forceinline__ void planned_gather_body(unsigned char *smem_raw, uint32_t vblock,
+                                                    const typename GatherT<T>::chunk *__restrict__ in, uint32_t ldc,
+                                                    float *__restrict__ out, uint32_t F,
+                                                    const uint2 *__restrict__ pairs, const uint32_t *__restrict__ off,
+                                                    uint32_t n_rows, uint32_t e_begin, uint32_t e_end, uint32_t Q,
+                                                    uint32_t tiles, uint32_t tile_vecs) {
   static_assert(G == 1 || K == 1, "virtual warps are for rows narrower than a warp");
   using Chunk = typename GatherT<T>::chunk;
   constexpr int V = GatherT<T>::V;
   constexpr uint32_t GS = 32 / G;                       // lanes per virtual warp
   const uint32_t lane = threadIdx.x & (GS - 1);         // lane within the virtual warp
   const uint32_t vwarp_in_block = threadIdx.x / GS;
-  const uint64_t gwarp = (uint64_t)blockIdx.x * (kPlanWarps * G) + vwarp_in_block;
+  const uint64_t gwarp = (uint64_t)vblock * (kPlanWarps * G) + vwarp_in_block;
   const uint32_t tile = (uint32_t)(gwarp % tiles);
   const uint64_t q = gwarp / tiles;
   const uint64_t e0_64 = e_begin + q * (uint64_t)Q;
 
-  extern __shared__ __align__(16) unsigned char smem_raw[];
   uint64_t *bar = reinterpret_cast<uint64_t *>(smem_raw);
   uint2 *s_pair = reinterpret_cast<uint2 *>(smem_raw + 16);
   uint32_t cta_e_base = 0, bulk_bytes = 0;
   {
-    const uint64_t cta_w0 = (uint64_t)blockIdx.x * (kPlanWarps * G);
+    const uint64_t cta_w0 = (uint64_t)vblock * (kPlanWarps * G);
     const uint64_t first_q = cta_w0 / tiles;
     const uint64_t last_q = (cta_w0 + kPlanWarps * G - 1) / tiles;
     uint64_t ce0 = e_begin + first_q * (uint64_t)Q;
@@ -510,6 +512,17 @@ __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
         fma_chunk(k, wj, v1[k]);
   }
   flush(row_started_inside && row_end <= e1);
+}
+
+template <class T, int K, int U, int OUTV, int MINB, int G = 1>
+__global__ void __launch_bounds__(kPlanWarps * 32, MINB)
+    planned_gather_sum_kernel(const typename GatherT<T>::chunk *__restrict__ in, uint32_t ldc, float *__restrict__ out,
+                              uint32_t F, const uint2 *__restrict__ pairs, const uint32_t *__restrict__ off,
+                              uint32_t n_rows, uint32_t e_begin, uint32_t e_end, uint32_t Q, uint32_t tiles,
+                              uint32_t tile_vecs) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  planned_gather_body<T, K, U, OUTV, G>(smem_raw, blockIdx.x, in, ldc, out, F, pairs, off, n_rows, e_begin, e_end, Q,
+                                        tiles, tile_vecs);
 }
 
 struct PlanShape;
@@ -760,21 +773,33 @@ __device__ __forceinline__ void p_cp_async16(void *smem_dst, const void *gmem_sr
 
 // TB = __nv_bfloat16: B rows are BF16 (ldb % 8 == 0), cp.async fills half-size B tiles and the values are widened to
 // FP32 at the shared-memory read; A, the accumulators and the FFMA math are those of the FP32 instantiation.
-template <class TB, int OUTV, bool SPLIT>
-__global__ void __launch_bounds__(kHubThreads, 2)
-    hub_block_gemm_kernel(const float *__restrict__ At, uint32_t lda, uint32_t M, uint32_t K, uint32_t k_split,
-                          const TB *__restrict__ B, uint32_t ldb, const uint32_t *__restrict__ colmap,
-                          float *__restrict__ out, uint32_t F, const uint32_t *__restrict__ rowmap, uint32_t m_tiles,
-                          uint32_t n_tiles) {
+// TN = outputs per thread along N: 8 (128 x 128 tile, 8 x 8 per thread, the stand-alone kernel's) or 4 (128 x 64 tile,
+// 8 x 4 per thread: half the accumulators, for the fused slab launches whose gather runs 3 or 4 CTAs per SM).
+// KKU = unroll of the 16-step loop over one K tile.
+// Tile `tile` = (split * m_tiles + m_tile) * n_tiles + n_tile covers K rows [k_lo + split * k_split, ...) cut at k_hi.
+template <int TN, class TB> struct HubSmem {
+  static constexpr uint32_t kBN = 16 * TN;
+  float As[2][kHubBK][kHubBM];
+  TB Bs[2][kHubBK][kBN];
+};
+
+template <class TB, int OUTV, bool SPLIT, int TN, int KKU>
+__device__ __forceinline__ void hub_gemm_tile(HubSmem<TN, TB> &sm, uint32_t tile, const float *__restrict__ At,
+                                              uint32_t lda, uint32_t M, uint32_t k_lo, uint32_t k_hi, uint32_t k_split,
+                                              const TB *__restrict__ B, uint32_t ldb,
+                                              const uint32_t *__restrict__ colmap, float *__restrict__ out, uint32_t F,
+                                              const uint32_t *__restrict__ rowmap, uint32_t m_tiles, uint32_t n_tiles) {
   constexpr bool kBf16 = std::is_same<TB, __nv_bfloat16>::value;
   constexpr uint32_t kBV = 16 / sizeof(TB); // B values per 16-byte chunk
-  __shared__ __align__(16) float As[2][kHubBK][kHubBM];
-  __shared__ __align__(16) TB Bs[2][kHubBK][kHubBN];
+  constexpr uint32_t kBN = HubSmem<TN, TB>::kBN;
+  constexpr uint32_t kBChunks = kHubBK * kBN / kBV; // 512 / 256 (FP32 / BF16, TN = 8), 256 / 128 (TN = 4)
+  auto &As = sm.As;
+  auto &Bs = sm.Bs;
   const uint32_t t = threadIdx.x;
-  const uint32_t n_tile = blockIdx.x % n_tiles, rest = blockIdx.x / n_tiles;
-  const uint32_t m0 = (rest % m_tiles) * kHubBM, n0 = n_tile * kHubBN;
-  const uint32_t k_begin = (rest / m_tiles) * k_split;
-  const uint32_t k_end = min(K, k_begin + k_split);
+  const uint32_t n_tile = tile % n_tiles, rest = tile / n_tiles;
+  const uint32_t m0 = (rest % m_tiles) * kHubBM, n0 = n_tile * kBN;
+  const uint32_t k_begin = k_lo + (rest / m_tiles) * k_split;
+  const uint32_t k_end = min(k_hi, k_begin + k_split);
   if (k_begin >= k_end)
     return;
   const uint32_t n_kt = (k_end - k_begin + kHubBK - 1) / kHubBK;
@@ -788,9 +813,11 @@ __global__ void __launch_bounds__(kHubThreads, 2)
       p_cp_async16(&As[buf][kk][c4], a_ok ? At + (size_t)k * lda + m0 + c4 : At, a_ok);
     }
 #pragma unroll
-    for (int i = 0; i < (int)(kHubBK * kHubBN / kBV / kHubThreads); i++) { // 512 (FP32) / 256 (BF16) B chunks
-      constexpr uint32_t kRowChunks = kHubBN / kBV;
+    for (int i = 0; i < (int)((kBChunks + kHubThreads - 1) / kHubThreads); i++) {
+      constexpr uint32_t kRowChunks = kBN / kBV;
       const uint32_t c = t + i * kHubThreads, kk = c / kRowChunks, cv = (c % kRowChunks) * kBV;
+      if (kBChunks % kHubThreads != 0 && c >= kBChunks)
+        break;
       const uint32_t k = k_begin + kt * kHubBK + kk;
       const bool b_ok = k < k_end && n0 + cv < ldb;
       const uint32_t brow = b_ok ? (colmap ? __ldg(colmap + k) : k) : 0;
@@ -809,11 +836,11 @@ __global__ void __launch_bounds__(kHubThreads, 2)
   };
 
   const uint32_t tx = t & 15, ty = t >> 4;
-  float acc[8][8];
+  float acc[8][TN];
 #pragma unroll
   for (int i = 0; i < 8; i++)
 #pragma unroll
-    for (int j = 0; j < 8; j++)
+    for (int j = 0; j < TN; j++)
       acc[i][j] = 0.f;
 
   load(0, 0);
@@ -826,18 +853,21 @@ __global__ void __launch_bounds__(kHubThreads, 2)
       asm volatile("cp.async.wait_group 0;" ::: "memory");
     }
     __syncthreads();
-#pragma unroll
+#pragma unroll(KKU)
     for (int kk = 0; kk < kHubBK; kk++) {
       const float4 a0 = *reinterpret_cast<const float4 *>(&As[buf][kk][ty * 4]);
       const float4 a1 = *reinterpret_cast<const float4 *>(&As[buf][kk][64 + ty * 4]);
-      const float4 b0 = read_b4(buf, kk, tx * 4);
-      const float4 b1 = read_b4(buf, kk, 64 + tx * 4);
       const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-      const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+      float b[TN];
+#pragma unroll
+      for (int h = 0; h < TN / 4; h++) {
+        const float4 bh = read_b4(buf, kk, h * 64 + tx * 4);
+        b[4 * h] = bh.x, b[4 * h + 1] = bh.y, b[4 * h + 2] = bh.z, b[4 * h + 3] = bh.w;
+      }
 #pragma unroll
       for (int i = 0; i < 8; i++)
 #pragma unroll
-        for (int j = 0; j < 8; j++)
+        for (int j = 0; j < TN; j++)
           acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
     }
     __syncthreads();
@@ -850,7 +880,7 @@ __global__ void __launch_bounds__(kHubThreads, 2)
       continue;
     float *orow = out + (size_t)(rowmap ? __ldg(rowmap + m) : m) * F;
 #pragma unroll
-    for (int j = 0; j < 2; j++) {
+    for (int j = 0; j < TN / 4; j++) {
       const uint32_t col = n0 + j * 64 + tx * 4;
       if (col < F)
         flush_chunk<OUTV, SPLIT>(orow, col, F,
@@ -859,8 +889,29 @@ __global__ void __launch_bounds__(kHubThreads, 2)
   }
 }
 
+template <class TB, int OUTV, bool SPLIT>
+__global__ void __launch_bounds__(kHubThreads, 2)
+    hub_block_gemm_kernel(const float *__restrict__ At, uint32_t lda, uint32_t M, uint32_t K, uint32_t k_split,
+                          const TB *__restrict__ B, uint32_t ldb, const uint32_t *__restrict__ colmap,
+                          float *__restrict__ out, uint32_t F, const uint32_t *__restrict__ rowmap, uint32_t m_tiles,
+                          uint32_t n_tiles) {
+  __shared__ __align__(16) HubSmem<8, TB> sm;
+  hub_gemm_tile<TB, OUTV, SPLIT, 8, kHubBK>(sm, blockIdx.x, At, lda, M, 0, K, k_split, B, ldb, colmap, out, F, rowmap, m_tiles,
+                                    n_tiles);
+}
+
+// Split-K length of the row block (M = hub_rows, K = gather_rows): about 4 waves of 2 CTAs per SM over the whole K,
+// at least 16 K tiles per CTA.
+static uint32_t hub_row_k_split(uint32_t K, uint32_t m_tiles, uint32_t n_tiles) {
+  const uint64_t want = (uint64_t)sm_count() * 2 * 4;
+  const uint64_t splits = (want + (uint64_t)m_tiles * n_tiles - 1) / ((uint64_t)m_tiles * n_tiles);
+  const uint32_t k_split = (uint32_t)((K + splits - 1) / splits);
+  return std::max<uint32_t>((k_split + kHubBK - 1) / kHubBK * kHubBK, 16 * kHubBK);
+}
+
+// rows = false: the column block only (the row block runs inside the fused slab launches).
 template <class TB, int OUTV>
-static int launch_hub_blocks(nts_gather_plan *pl, const TB *in, uint32_t ldb, float *out, uint32_t F,
+static int launch_hub_blocks(nts_gather_plan *pl, const TB *in, uint32_t ldb, float *out, uint32_t F, bool rows,
                              cudaStream_t st) {
   const uint32_t n_tiles = (F + kHubBN - 1) / kHubBN;
   if (pl->hub_cols) { // column block: M = n_rows, K = hub_cols
@@ -872,14 +923,11 @@ static int launch_hub_blocks(nts_gather_plan *pl, const TB *in, uint32_t ldb, fl
         F, nullptr, m_tiles, n_tiles);
     NTS_LAUNCH_CHECK();
   }
-  if (pl->hub_rows) { // row block: M = hub_rows, K = gather_rows, split so that about 4 waves of CTAs fill the SMs
+  if (pl->hub_rows && rows) { // row block: M = hub_rows, K = gather_rows
     const uint32_t m_tiles = (pl->hub_rows + kHubBM - 1) / kHubBM;
     const uint32_t K = pl->gather_rows;
-    const uint64_t want = (uint64_t)sm_count() * 2 * 4;
-    uint64_t splits = (want + (uint64_t)m_tiles * n_tiles - 1) / ((uint64_t)m_tiles * n_tiles);
-    uint32_t k_split = (uint32_t)((K + splits - 1) / splits);
-    k_split = std::max<uint32_t>((k_split + kHubBK - 1) / kHubBK * kHubBK, 16 * kHubBK);
-    splits = (K + k_split - 1) / k_split;
+    const uint32_t k_split = hub_row_k_split(K, m_tiles, n_tiles);
+    const uint64_t splits = (K + k_split - 1) / k_split;
     hub_block_gemm_kernel<TB, OUTV, true><<<(unsigned)(splits * m_tiles * n_tiles), kHubThreads, 0, st>>>(
         pl->dense + (size_t)pl->hub_cols * pl->lda_c, pl->lda_r, (uint32_t)pl->hub_rows, K, k_split, in, ldb, nullptr,
         out, F, pl->hub_row_ids, m_tiles, n_tiles);
@@ -888,8 +936,102 @@ static int launch_hub_blocks(nts_gather_plan *pl, const TB *in, uint32_t ldb, fl
   return 0;
 }
 
+// ---- fused slab launches (nts_gather_plan.overlap): the row block's tiles run inside the slab launches --------------
+// The row block is FFMA-bound, the residual gather bound by gathered rows moving from L2 to the SMs; run one after the
+// other, each leaves idle what the other needs.  They can share a launch because they write disjoint output rows: the
+// row block takes every non-column-block edge of its hub rows (build_hybrid), so those rows have empty residual
+// segments and no gather warp writes them, while the row block writes hub rows only.  Its split-K is cut at the slab
+// boundaries, so the tiles in slab s's launch read B rows [s * slab_rows, (s+1) * slab_rows) of the gathered matrix:
+// the rows slab s's gather is making L2-resident.  (The column block writes every output row with a plain
+// read-modify-write, so it stays a launch of its own, before the first slab.)
+struct HubRowArgs {
+  const float *At;                  // D_r^T [gather_rows x lda]
+  uint32_t lda, M;                  // M = hub rows
+  uint32_t k_lo, k_hi, k_split;     // this slab's gathered rows [k_lo, k_hi), split-K length
+  const uint32_t *rowmap;           // hub row ids
+  uint32_t m_tiles, n_tiles, n_gemm; // n_gemm = row-block tiles of this launch (splits * m_tiles * n_tiles)
+  uint32_t period;                  // grid / n_gemm (>= 1)
+};
+
+// Every period-th block (period = floor(grid / n_gemm)) of the first n_gemm * period is a row-block tile, the rest are
+// gather CTAs: the tiles are spread through the grid (CTAs start in about blockIdx order) instead of forming a head
+// or a tail.  The GEMM body has half the accumulators (TN = 4) at 3 or 4 CTAs per SM, where the 8 x 8 body would not
+// fit the gather's register budget; its K-tile loop is unrolled 4-fold, not 16-fold, for the same reason.
+template <class T, int K, int U, int OUTV, int MINB, int G>
+__global__ void __launch_bounds__(kPlanWarps * 32, MINB)
+    planned_slab_hub_kernel(const typename GatherT<T>::chunk *__restrict__ in, uint32_t ldc, float *__restrict__ out,
+                            uint32_t F, const uint2 *__restrict__ pairs, const uint32_t *__restrict__ off,
+                            uint32_t n_rows, uint32_t e_begin, uint32_t e_end, uint32_t Q, uint32_t tiles,
+                            uint32_t tile_vecs, const HubRowArgs hub) {
+  static_assert(kPlanWarps * 32 == kHubThreads, "both bodies run 256 threads");
+  constexpr int TN = MINB <= 2 ? 8 : 4;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const uint32_t b = blockIdx.x, grp = b / hub.period;
+  if (grp < hub.n_gemm && b - grp * hub.period == hub.period - 1)
+    hub_gemm_tile<T, OUTV, true, TN, TN == 8 ? kHubBK : 4>(
+        *reinterpret_cast<HubSmem<TN, T> *>(smem_raw), grp, hub.At, hub.lda, hub.M, hub.k_lo, hub.k_hi, hub.k_split,
+        reinterpret_cast<const T *>(in), ldc * GatherT<T>::V, nullptr, out, F, hub.rowmap, hub.m_tiles, hub.n_tiles);
+  else
+    planned_gather_body<T, K, U, OUTV, G>(smem_raw, b - min(grp, hub.n_gemm), in, ldc, out, F, pairs, off, n_rows,
+                                          e_begin, e_end, Q, tiles, tile_vecs);
+}
+
+template <class T, int K, int U, int OUTV, int MINB, int G = 1>
+static int launch_fused(nts_gather_plan *pl, const PlanShape &sh, const T *in_rows, uint32_t ldc, float *out,
+                        uint32_t F, uint32_t Q, cudaStream_t st) {
+  constexpr int TN = MINB <= 2 ? 8 : 4;
+  auto kern = planned_slab_hub_kernel<T, K, U, OUTV, MINB, G>;
+  const auto *in = reinterpret_cast<const typename GatherT<T>::chunk *>(in_rows);
+  const size_t smem = std::max(16 + ((size_t)kPlanWarps * G * Q + 4) * 8, sizeof(HubSmem<TN, T>));
+  NTS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  HubRowArgs hub;
+  hub.At = pl->dense + (size_t)pl->hub_cols * pl->lda_c;
+  hub.lda = pl->lda_r;
+  hub.M = (uint32_t)pl->hub_rows;
+  hub.rowmap = pl->hub_row_ids;
+  hub.m_tiles = (hub.M + kHubBM - 1) / kHubBM;
+  hub.n_tiles = (F + 16 * TN - 1) / (16 * TN);
+  hub.k_split = hub_row_k_split(pl->gather_rows, hub.m_tiles, hub.n_tiles);
+  pl->last_launches = 0;
+  for (int s = 0; s < pl->slabs; s++) {
+    // slab s gathers rows [s * slab_rows, (s+1) * slab_rows); the last one runs to gather_rows
+    // (plan_hybrid_keys_kernel clamps the slab index to slabs - 1)
+    hub.k_lo = (uint32_t)std::min<uint64_t>((uint64_t)s * pl->slab_rows, pl->gather_rows);
+    hub.k_hi = s + 1 == pl->slabs ? pl->gather_rows
+                                  : (uint32_t)std::min<uint64_t>((uint64_t)(s + 1) * pl->slab_rows, pl->gather_rows);
+    const uint64_t splits = hub.k_hi > hub.k_lo ? (hub.k_hi - hub.k_lo + hub.k_split - 1) / hub.k_split : 0;
+    const uint64_t n_gemm = splits * hub.m_tiles * hub.n_tiles;
+    const uint64_t eb = pl->slab_edge[s], ee = pl->slab_edge[s + 1];
+    const uint64_t quanta = ee > eb ? (ee - eb + Q - 1) / Q : 0;
+    const uint64_t blocks = n_gemm + (quanta * sh.tiles + kPlanWarps * G - 1) / (kPlanWarps * G);
+    if (!blocks)
+      continue;
+    NTS_ARG_CHECK(blocks <= 0x7fffffffull, "aggregation grid too large");
+    hub.n_gemm = (uint32_t)n_gemm;
+    hub.period = n_gemm ? (uint32_t)(blocks / n_gemm) : 1;
+    kern<<<(unsigned)blocks, kPlanWarps * 32, smem, st>>>(in, ldc, out, F, pl->pairs, pl->voff + (size_t)s * pl->n_rows,
+                                                          pl->n_rows, (uint32_t)eb, (uint32_t)ee, Q, sh.tiles,
+                                                          sh.tile_vecs, hub);
+    NTS_LAUNCH_CHECK();
+    pl->last_grid = (int)blocks;
+    pl->last_launches++;
+  }
+  return 0;
+}
+
+// The fused schedule exists at the (chunks, U, occupancy, virtual warps) points run_gather picks by default.
+#define NTS_PLAN_FUSED_CASE(K_, U_, B_, G_)                                                                         \
+  if (sh.k == K_ && sh.u == U_ && sh.minb == B_ && sh.g == G_) {                                                    \
+    if (sh.outv == 4)                                                                                               \
+      return launch_fused<T, K_, U_, 4, B_, G_>(pl, sh, in, ldc, out, F, Q, st);                                    \
+    if (sh.outv == 2)                                                                                               \
+      return launch_fused<T, K_, U_, 2, B_, G_>(pl, sh, in, ldc, out, F, Q, st);                                    \
+    return launch_fused<T, K_, U_, 1, B_, G_>(pl, sh, in, ldc, out, F, Q, st);                                      \
+  }
+
 // The gather of rows already in the kernel's layout: `in` holds gather_rows rows of ld values of T, 16-byte aligned,
-// ld % V == 0, zero past F.  Dense hub blocks first, then the residual edges' slab launches (stream order).
+// ld % V == 0, zero past F.  Dense hub blocks first, then the residual edges' slab launches (stream order); with
+// pl->overlap the row block runs inside the slab launches instead (planned_slab_hub_kernel).
 template <class T>
 static int run_gather(nts_gather_plan *pl, const T *in, uint32_t ld, float *output, uint32_t F, cudaStream_t st) {
   constexpr bool kBf16 = std::is_same<T, __nv_bfloat16>::value;
@@ -902,10 +1044,12 @@ static int run_gather(nts_gather_plan *pl, const T *in, uint32_t ld, float *outp
   sh.k = (int)((sh.tile_vecs + 31) / 32);
   sh.tiles = (ldc + sh.tile_vecs - 1) / sh.tile_vecs;
   sh.outv = (F % 4 == 0 && aligned_to(output, 16)) ? 4 : ((F % 2 == 0 && aligned_to(output, 8)) ? 2 : 1);
+  const bool fused = pl->overlap && pl->hub_rows;
+  NTS_ARG_CHECK(!fused || g_plan_variant == 0, "the fused slab launches use the register-staging gather (variant 0)");
   if (pl->hub_cols || pl->hub_rows) {
-    const int rc = sh.outv == 4   ? launch_hub_blocks<T, 4>(pl, in, ld, output, F, st)
-                   : sh.outv == 2 ? launch_hub_blocks<T, 2>(pl, in, ld, output, F, st)
-                                  : launch_hub_blocks<T, 1>(pl, in, ld, output, F, st);
+    const int rc = sh.outv == 4   ? launch_hub_blocks<T, 4>(pl, in, ld, output, F, !fused, st)
+                   : sh.outv == 2 ? launch_hub_blocks<T, 2>(pl, in, ld, output, F, !fused, st)
+                                  : launch_hub_blocks<T, 1>(pl, in, ld, output, F, !fused, st);
     if (rc)
       return rc;
   }
@@ -951,6 +1095,26 @@ static int run_gather(nts_gather_plan *pl, const T *in, uint32_t ld, float *outp
     Q = (1024 / sh.g) & ~31u;
   pl->last_k = sh.k, pl->last_u = sh.u, pl->last_outv = sh.outv;
   float *out = output;
+  if (fused) {
+    if constexpr (kBf16) {
+      NTS_PLAN_FUSED_CASE(1, 4, 4, 2)
+      NTS_PLAN_FUSED_CASE(1, 4, 4, 4)
+      NTS_PLAN_FUSED_CASE(1, 4, 4, 1)
+      NTS_PLAN_FUSED_CASE(2, 2, 3, 1)
+      NTS_PLAN_FUSED_CASE(3, 2, 3, 1)
+      NTS_PLAN_FUSED_CASE(4, 2, 2, 1)
+      NTS_PLAN_FUSED_CASE(5, 2, 2, 1)
+    } else {
+      NTS_PLAN_FUSED_CASE(1, 4, 4, 2)
+      NTS_PLAN_FUSED_CASE(1, 4, 4, 4)
+      NTS_PLAN_FUSED_CASE(1, 4, 4, 1)
+      NTS_PLAN_FUSED_CASE(2, 4, 3, 1)
+      NTS_PLAN_FUSED_CASE(3, 4, 2, 1)
+      NTS_PLAN_FUSED_CASE(4, 2, 2, 1)
+      NTS_PLAN_FUSED_CASE(5, 4, 2, 1)
+    }
+    return fail(-1, "no fused slab/hub-row instantiation for this (chunks, U, occupancy) point", __FILE__, __LINE__);
+  }
   if constexpr (kBf16) {
     // only points that compile without spills (a BF16 chunk holds 8 accumulators: U*K loads cost what they do in
     // FP32, the accumulators twice as much)
@@ -1593,9 +1757,11 @@ static nts_gather_plan *create_tuned(const nts_vid_t *offsets, const nts_vid_t *
   float best_ms = 0.f;
   ok = ok && time_plan(best, &best_ms);
   // build and time one candidate, keep it if it is faster: 1 = kept, 0 = not kept (*ms its time), -1 = failed
-  auto consider = [&](int s, int hc, int hr, float *ms) -> int {
+  auto consider = [&](int s, int hc, int hr, float *ms, int overlap = 0) -> int {
     nts_gather_plan *pl = nts_gather_plan_create_hybrid(offsets, indices, weight, slot_of, index_base, n_rows, n_edges,
                                                         gather_rows, s, hc, hr, stream);
+    if (pl)
+      pl->overlap = overlap;
     if (!pl || !time_plan(pl, ms)) {
       nts_gather_plan_destroy(pl);
       return -1;
@@ -1639,6 +1805,22 @@ static nts_gather_plan *create_tuned(const nts_vid_t *offsets, const nts_vid_t *
       for (int s : {plain_slabs / 2, std::min(plain_slabs * 2, s_max)})
         if (s >= 1 && s != plain_slabs && s != best->slabs)
           consider(s, hc, hr, &ms);
+    }
+    // Then the schedule: the row block inside the slab launches against before them, for the chosen counts; when the
+    // fused schedule wins, more hub rows may pay under it, so the hub-row search continues upward under it.
+    // NTS_PLAN_OVERLAP=0 (measurement override) keeps the sequential schedule.
+    const char *ov_env = getenv("NTS_PLAN_OVERLAP");
+    if (ok && best->hub_rows && !(ov_env && strcmp(ov_env, "0") == 0)) {
+      best->overlap = 1;
+      float fused_ms = 0.f;
+      if (time_plan(best, &fused_ms) && fused_ms < best_ms) {
+        best_ms = fused_ms;
+        for (int r = 2 * best->hub_rows; r <= std::min(n_r, kHubMax); r *= 2)
+          if (consider(best->slabs, best->hub_cols, r, &ms, 1) != 1)
+            break;
+      } else {
+        best->overlap = 0;
+      }
     }
   }
   cudaFree(x), cudaFree(y);
@@ -1688,6 +1870,15 @@ int nts_gather_plan_hubs(const nts_gather_plan *pl, int *cols, int *rows) {
     *cols = pl->hub_cols;
   if (rows)
     *rows = pl->hub_rows;
+  return 0;
+}
+
+int nts_gather_plan_overlap(const nts_gather_plan *pl) { return pl ? pl->overlap : 0; }
+
+int nts_gather_plan_set_overlap(nts_gather_plan *pl, int overlap) {
+  NTS_ARG_CHECK(pl != nullptr, "null plan");
+  NTS_ARG_CHECK(overlap == 0 || overlap == 1, "overlap must be 0 (sequential) or 1 (fused slab launches)");
+  pl->overlap = overlap;
   return 0;
 }
 

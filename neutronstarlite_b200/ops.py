@@ -145,9 +145,19 @@ class GatherPlan:
         self.hub_cols, self.hub_rows = hc.value, hr.value
         self.n_rows, self.n_edges = int(n_rows), int(n_edges)
 
+    @property
+    def overlap(self):
+        """True when the hub-row block runs inside the slab launches (nts_gather_plan_overlap)."""
+        return bool(_lib.load().nts_gather_plan_overlap(self.handle))
+
+    def set_overlap(self, overlap):
+        _lib.call("nts_gather_plan_set_overlap", self.handle, int(bool(overlap)))
+
     def key(self):
-        """What decides the plan's arrays besides the chunk direction: plans with equal keys are interchangeable."""
-        return (self.slabs,) + ((self.hub_cols, self.hub_rows) if self.hub_cols or self.hub_rows else ())
+        """What decides the plan's arrays and schedule besides the chunk direction: plans with equal keys are
+        interchangeable."""
+        return ((self.slabs,) + ((self.hub_cols, self.hub_rows) if self.hub_cols or self.hub_rows else ())
+                + (("overlap",) if self.overlap else ()))
 
     def run(self, x, out, gather_dtype=None):
         """out += A x.  gather_dtype=torch.bfloat16: the rows of x (float32 or bfloat16) are gathered as BF16 with FP32
