@@ -544,6 +544,45 @@ int nts_host_mirror_index(const nts_vid_t *edges_src_dst, uint64_t n_edges, nts_
                           const nts_vid_t *partition_offset, int rank, nts_vid_t *mirror_index,
                           nts_vid_t *owned);
 
+/* ---- device-side graph preparation: nts_graph_build -------------------------------------------------------------------
+ * The arrays of the host builder above, for one rank, built on the GPU.  From a packed binary edge file ({u32 src,
+ * u32 dst} records; edge count = file size / 8) read twice in blocks of block_edges records - pass 1 degrees, pass 2
+ * the owned edges - so no process holds the edge list; or from edge arrays already on the device (int32 or int64;
+ * only the edges whose destination this rank owns are required when the GLOBAL clamped degrees are given, in the
+ * same type).  partition_offset (HOST array [P+1]) may be NULL: the reference's partitioner then runs on the raw
+ * out-degree (with given degrees it is required for P > 1).  Limits: 1 <= V < 2^31, owned edges < 2^31; an id >= V is
+ * an error, never clamped.  Outputs are bit-identical to nts_host_build_chunk / nts_host_mirror_index (CSC (dst, src)
+ * ascending, CSR (src, dst) ascending, weights of nts_norm_degree).  Device scratch beyond the returned arrays stays
+ * below 40 B per owned edge + 16 B per vertex.  Both builders synchronise `stream` and return NULL on failure
+ * (nts_last_error() says why); exports are asynchronous copies on `stream` into caller-allocated device arrays, and
+ * any export pointer may be NULL (arrays of length 0 included). */
+typedef struct nts_graph_build nts_graph_build;
+enum { NTS_GRAPH_BUILD_DIST = 1 };              /* also build MirrorIndex and the whole-partition CSC */
+enum { NTS_INDEX_I32 = 0, NTS_INDEX_I64 = 1 };  /* element type of device edge and degree arrays */
+nts_graph_build *nts_graph_build_from_file(const char *path, nts_vid_t n_vertices, int partitions, int rank,
+                                           const nts_vid_t *partition_offset, uint64_t block_edges, int flags,
+                                           void *stream);
+nts_graph_build *nts_graph_build_from_device(const void *src, const void *dst, int index_dtype, uint64_t n_edges,
+                                             nts_vid_t n_vertices, int partitions, int rank,
+                                             const nts_vid_t *partition_offset, const void *out_degree,
+                                             const void *in_degree, int flags, void *stream);
+/* partition_offset[P+1], chunk_edges[P], owned_mirrors (0 without NTS_GRAPH_BUILD_DIST), the peak device scratch in
+ * bytes, and pass_seconds[4] = {degrees, owned edges, chunks, distributed artefacts}; every output may be NULL */
+int nts_graph_build_info(const nts_graph_build *build, nts_vid_t *partition_offset, uint64_t *chunk_edges,
+                         nts_vid_t *owned_mirrors, uint64_t *scratch_peak_bytes, double *pass_seconds);
+/* chunk i (sources in partition i): column_offset[Vp+1], row_indices[Ei], edge_weight_forward[Ei], row_offset[Vi+1],
+ * column_indices[Ei], edge_weight_backward[Ei], source_active[Vi] */
+int nts_graph_build_export_chunk(const nts_graph_build *build, int i, nts_vid_t *column_offset, nts_vid_t *row_indices,
+                                 float *edge_weight_forward, nts_vid_t *row_offset, nts_vid_t *column_indices,
+                                 float *edge_weight_backward, unsigned char *source_active, void *stream);
+/* MirrorIndex[V+1], whole-partition column_offset[Vp+1] and row_indices[owned edges] (needs NTS_GRAPH_BUILD_DIST) */
+int nts_graph_build_export_dist(const nts_graph_build *build, nts_vid_t *mirror_index, nts_vid_t *column_offset,
+                                nts_vid_t *row_indices, void *stream);
+/* clamped degrees with multiplicity, out_degree[V] and in_degree[V] */
+int nts_graph_build_export_degrees(const nts_graph_build *build, nts_vid_t *out_degree, nts_vid_t *in_degree,
+                                   void *stream);
+int nts_graph_build_destroy(nts_graph_build *build);
+
 /* ---- feature / label / mask tables (GNNDatum, core/ntsDataloador.hpp) ----------------------------------------------------
  * Text tables exactly as GNNDatum::readFeature_Label_Mask (:156-221) reads them - "id f0 .. fF-1", "id label",
  * "id train|val|eval|test", the k-th label / mask record belongs to the k-th feature record - parsed in parallel;

@@ -106,6 +106,13 @@ SIGNATURES = {
     "nts_host_mirror_index": (_int, [_vp, _u64, _u32, _vp, _int, _vp, _vp]),
     "nts_host_read_feature_label_mask": (_int, [C.c_char_p, C.c_char_p, C.c_char_p, _u32, _u32, _u32, _vp, _vp, _vp]),
     "nts_host_read_feature_binary": (_int, [C.c_char_p, _u32, _u32, _u32, _vp]),
+    "nts_graph_build_from_file": (_vp, [C.c_char_p, _u32, _int, _int, _vp, _u64, _int, _vp]),
+    "nts_graph_build_from_device": (_vp, [_vp, _vp, _int, _u64, _u32, _int, _int, _vp, _vp, _vp, _int, _vp]),
+    "nts_graph_build_info": (_int, [_vp] * 6),
+    "nts_graph_build_export_chunk": (_int, [_vp, _int] + [_vp] * 8),
+    "nts_graph_build_export_dist": (_int, [_vp] * 5),
+    "nts_graph_build_export_degrees": (_int, [_vp] * 4),
+    "nts_graph_build_destroy": (_int, [_vp]),
 }
 
 

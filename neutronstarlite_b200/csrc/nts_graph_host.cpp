@@ -27,6 +27,39 @@ inline float norm_degree(uint32_t out_deg_src, uint32_t in_deg_dst) {
 
 } // namespace
 
+namespace nts {
+
+// core/graph.hpp:1185-1211 over the raw (un-clamped) out-degree; shared with the device builder (nts_graph_build.cu)
+int partition_offsets_from_out_degree(const uint32_t *out_degree, uint64_t n_edges, nts_vid_t V, int P,
+                                      nts_vid_t *partition_offset) {
+  const uint64_t alpha = 12ull * (uint64_t)(P + 1);
+  uint64_t remained = n_edges + (uint64_t)V * alpha;
+  partition_offset[0] = 0;
+  for (int i = 0; i < P; i++) {
+    const uint64_t parts_left = (uint64_t)(P - i);
+    const uint64_t expected = remained / parts_left;
+    if (parts_left == 1) {
+      partition_offset[i + 1] = V;
+    } else {
+      uint64_t got = 0;
+      nts_vid_t cut = partition_offset[i]; // (the reference leaves this unset if the sum never exceeds)
+      for (nts_vid_t v = partition_offset[i]; v < V; v++) {
+        got += out_degree[v] + alpha;
+        if (got > expected) {
+          cut = v;
+          break;
+        }
+      }
+      partition_offset[i + 1] = cut / kPageSize * kPageSize;
+    }
+    for (nts_vid_t v = partition_offset[i]; v < partition_offset[i + 1]; v++)
+      remained -= out_degree[v] + alpha;
+  }
+  return partition_offset[P] == V ? 0 : -1;
+}
+
+} // namespace nts
+
 extern "C" {
 
 int nts_host_degrees(const nts_vid_t *edges, uint64_t n_edges, nts_vid_t V, nts_vid_t *out_degree,
@@ -61,30 +94,7 @@ int nts_host_partition_offsets(const nts_vid_t *edges, uint64_t n_edges, nts_vid
       return -1;
     out_degree[edges[2 * e]]++;
   }
-  const uint64_t alpha = 12ull * (uint64_t)(P + 1);
-  uint64_t remained = n_edges + (uint64_t)V * alpha;
-  partition_offset[0] = 0;
-  for (int i = 0; i < P; i++) {
-    const uint64_t parts_left = (uint64_t)(P - i);
-    const uint64_t expected = remained / parts_left;
-    if (parts_left == 1) {
-      partition_offset[i + 1] = V;
-    } else {
-      uint64_t got = 0;
-      nts_vid_t cut = partition_offset[i]; // (the reference leaves this unset if the sum never exceeds)
-      for (nts_vid_t v = partition_offset[i]; v < V; v++) {
-        got += out_degree[v] + alpha;
-        if (got > expected) {
-          cut = v;
-          break;
-        }
-      }
-      partition_offset[i + 1] = cut / kPageSize * kPageSize;
-    }
-    for (nts_vid_t v = partition_offset[i]; v < partition_offset[i + 1]; v++)
-      remained -= out_degree[v] + alpha;
-  }
-  return partition_offset[P] == V ? 0 : -1;
+  return nts::partition_offsets_from_out_degree(out_degree.data(), n_edges, V, P, partition_offset);
 }
 
 int nts_host_chunk_edge_counts(const nts_vid_t *edges, uint64_t n_edges, const nts_vid_t *po, int P, int rank,

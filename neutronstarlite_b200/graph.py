@@ -6,11 +6,15 @@
   * `PartitionedGraph` <-> `PartitionedGraph` (core/PartitionedGraph.hpp:60-143,295-420): the P chunks of a rank,
                            `MirrorIndex` / `owned_mirrors`, and the whole-partition CSC used by the edge operators.
 
-All arrays are built by the C++ host routines of libnts_b200 (`nts_host_*`, nts_graph_host.cpp) or, for big
-synthetic graphs already resident on the GPU, by `PartitionedGraph.from_device_edges` (sort-based, torch);
-both produce identical arrays (tests/test_graph_host.py, tests/test_gpu_parity.py).
+All arrays are built by the C++ host routines of libnts_b200 (`nts_host_*`, nts_graph_host.cpp, through
+`generate_all`) or on the GPU by `nts_graph_build` (nts_graph_build.cu), from a packed binary edge file
+(`PartitionedGraph.from_edge_file`) or from edge tensors already on the device (`from_device_edges`); both produce
+identical arrays (tests/test_graph_host.py, tests/test_graph_build_device.py).  The device builders fill only the
+`*_gpu` arrays; the host arrays stay None.
 """
 from __future__ import annotations
+
+import os
 
 import numpy as np
 
@@ -102,6 +106,7 @@ class CSCSegment:
         self.row_offset_gpu = None
         self.column_indices_gpu = None
         self.edge_weight_backward_gpu = None
+        self.source_active_gpu = None      # u8 [Vi], filled by the device builders only
 
     def copy_graph_to_device(self, device):
         """CSC_segment_pinned::CopyGraphToDevice (core/GraphSegment.cpp:178-220)."""
@@ -252,65 +257,122 @@ class PartitionedGraph:
             self.mirror_index_gpu = torch.from_numpy(self.MirrorIndex.view(np.int32)).to(self.device)
         return self
 
-    # -- device-side construction for big synthetic graphs -------------------------------------------------
+    # -- device-side construction (nts_graph_build, csrc/nts_graph_build.cu) -------------------------------------
     @staticmethod
-    def from_device_edges(src, dst, vertices, partitions=1, partition_id=0, partition_offset=None,
-                          out_degree=None, in_degree=None):
-        """Build the chunks of one rank from edge tensors already on the GPU (int64 src/dst of ALL edges, or at
-        least of every edge whose destination this rank owns; degrees must be global).  Sort-based: CSC order =
-        (dst, src) ascending, CSR order = (src, dst) ascending - the same canonical orders as the host builder."""
+    def from_edge_file(path, vertices, partitions=1, partition_id=0, device=None, dist=False, partition_offset=None,
+                       block_edges=1 << 26):
+        """Build the chunks of one rank on the GPU from a packed binary edge file ({u32 src, u32 dst} records,
+        dep/gemini/type.hpp:100-106).  The file is streamed twice in blocks of `block_edges` records (degrees, then
+        the edges this rank owns), so no process holds the edge list in host memory.  Fills every chunk's `*_gpu`
+        arrays (plus `source_active_gpu`), the clamped degrees `out_degree_gpu` / `in_degree_gpu`, `partition_offset`
+        (the reference's partitioner unless given), `global_vertices`, `owned_vertices` and `owned_edges`; with
+        dist=True also `mirror_index_gpu`, `owned_mirrors` and the whole-partition CSC `column_offset_gpu` /
+        `row_indices_gpu`.  The host arrays (`column_offset`, `MirrorIndex`, ...) stay None.  The arrays are
+        bit-identical to the host builder's (`generate_all`)."""
         import torch
 
+        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        po = None if partition_offset is None else np.ascontiguousarray(partition_offset, dtype=np.uint32)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            h = _lib.load().nts_graph_build_from_file(os.fsencode(path), int(vertices), int(partitions),
+                                                      int(partition_id), _ptr(po), int(block_edges),
+                                                      _lib_flags(dist), stream)
+            return PartitionedGraph._from_build(h, vertices, partitions, partition_id, dev, dist, stream)
+
+    @staticmethod
+    def from_device_edges(src, dst, vertices, partitions=1, partition_id=0, partition_offset=None,
+                          out_degree=None, in_degree=None, dist=False):
+        """Build the chunks of one rank from int32 / int64 edge tensors already on the GPU (src/dst of ALL edges, or
+        - when the global degrees are given - at least of every edge whose destination this rank owns).  Degrees,
+        given or computed from the edges, are clamped to >= 1.  Same kernels, outputs and attributes as
+        `from_edge_file`; partition_offset is required for partitions > 1."""
+        import torch
+
+        if partition_offset is None and int(partitions) != 1:
+            raise ValueError("partition_offset is required for partitions > 1")
+        if src.dtype != dst.dtype or src.dtype not in (torch.int32, torch.int64):
+            raise _lib.NtsError("src / dst must both be int32 or both int64 (got %s, %s)" % (src.dtype, dst.dtype))
+        if (out_degree is None) != (in_degree is None):
+            raise _lib.NtsError("give both degree tensors or neither")
         dev = src.device
-        V = int(vertices)
-        P, p = int(partitions), int(partition_id)
-        if out_degree is None or in_degree is None:
-            out_degree = torch.bincount(src, minlength=V).clamp_(min=1)
-            in_degree = torch.bincount(dst, minlength=V).clamp_(min=1)
-        if partition_offset is None:
-            if P != 1:
-                raise ValueError("partition_offset is required for partitions > 1")
-            partition_offset = np.array([0, V], dtype=np.uint32)
-        po = np.asarray(partition_offset, dtype=np.uint32)
-        pg = PartitionedGraph(None, P, p, po)
-        pg.global_vertices = V
-        pg.device = dev
-        v0, v1 = int(po[p]), int(po[p + 1])
-        local = (dst >= v0) & (dst < v1)
-        s_l, d_l = src[local], dst[local]
-        # edge weight, nts_norm_degree (core/ntsBaseOp.hpp:194-197): float(sqrt(double)) * float(sqrt(double))
-        sq_out = out_degree.to(torch.float64).sqrt().to(torch.float32)
-        sq_in = in_degree.to(torch.float64).sqrt().to(torch.float32)
-        for i in range(P):
-            s0, s1 = int(po[i]), int(po[i + 1])
-            sel = (s_l >= s0) & (s_l < s1)
-            s, d = s_l[sel], d_l[sel]
-            c = CSCSegment()
-            c.edge_size = int(s.numel())
-            c.batch_size_forward = v1 - v0
-            c.batch_size_backward = s1 - s0
-            c.src_range = (s0, s1)
-            c.dst_range = (v0, v1)
-            key = d * V + s
-            order = torch.argsort(key)
-            cs, cd = s[order], d[order]
-            del key, order
-            c.row_indices_gpu = cs.to(torch.int32)
-            c.column_offset_gpu = torch.zeros(v1 - v0 + 1, dtype=torch.int64, device=dev)
-            c.column_offset_gpu[1:] = torch.cumsum(torch.bincount(cd - v0, minlength=v1 - v0), 0)
-            c.column_offset_gpu = c.column_offset_gpu.to(torch.int32)
-            c.edge_weight_forward_gpu = (1.0 / (sq_out[cs] * sq_in[cd])).to(torch.float32)
-            del cs, cd
-            key = s * V + d
-            order = torch.argsort(key)
-            rs, rd = s[order], d[order]
-            del key, order
-            c.column_indices_gpu = rd.to(torch.int32)
-            c.row_offset_gpu = torch.zeros(s1 - s0 + 1, dtype=torch.int64, device=dev)
-            c.row_offset_gpu[1:] = torch.cumsum(torch.bincount(rs - s0, minlength=s1 - s0), 0)
-            c.row_offset_gpu = c.row_offset_gpu.to(torch.int32)
-            c.edge_weight_backward_gpu = (1.0 / (sq_out[rs] * sq_in[rd])).to(torch.float32)
-            del rs, rd
-            pg.graph_chunks.append(c)
-        pg.owned_edges = sum(c.edge_size for c in pg.graph_chunks)
-        return pg
+        src, dst = src.contiguous(), dst.contiguous()
+        if out_degree is not None:
+            out_degree = out_degree.to(device=dev, dtype=src.dtype).contiguous()
+            in_degree = in_degree.to(device=dev, dtype=src.dtype).contiguous()
+        po = None if partition_offset is None else np.ascontiguousarray(partition_offset, dtype=np.uint32)
+        dtype = 0 if src.dtype == torch.int32 else 1   # NTS_INDEX_I32 / NTS_INDEX_I64
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            h = _lib.load().nts_graph_build_from_device(
+                src.data_ptr() or None, dst.data_ptr() or None, dtype, int(src.numel()), int(vertices),
+                int(partitions), int(partition_id), _ptr(po),
+                None if out_degree is None else out_degree.data_ptr(),
+                None if in_degree is None else in_degree.data_ptr(), _lib_flags(dist), stream)
+            return PartitionedGraph._from_build(h, vertices, partitions, partition_id, dev, dist, stream)
+
+    @staticmethod
+    def _from_build(h, vertices, partitions, partition_id, dev, dist, stream):
+        """Copy the arrays of an nts_graph_build handle into torch tensors (the caching allocator owns them), then
+        destroy the handle.  Edge arrays get the 8-element tail slack of CSCSegment.copy_graph_to_device."""
+        import torch
+
+        L = _lib.load()
+        if not h:
+            _lib.check(-1, "nts_graph_build")
+        try:
+            V, P, p = int(vertices), int(partitions), int(partition_id)
+            po = np.zeros(P + 1, dtype=np.uint32)
+            counts = np.zeros(P, dtype=np.uint64)
+            mirrors = np.zeros(1, dtype=np.uint32)
+            scratch = np.zeros(1, dtype=np.uint64)
+            secs = np.zeros(4, dtype=np.float64)
+            _lib.call("nts_graph_build_info", h, _ptr(po), _ptr(counts), _ptr(mirrors), _ptr(scratch), _ptr(secs))
+            pg = PartitionedGraph(None, P, p, po)
+            pg.global_vertices = V
+            pg.device = dev
+            pg.build_stats = {"scratch_peak_bytes": int(scratch[0]),
+                              "seconds": dict(zip(("degrees", "owned_edges", "chunks", "dist"), secs.tolist()))}
+
+            def vec(n, dtype=torch.int32):
+                return torch.empty(n, dtype=dtype, device=dev)
+
+            def edges(n, dtype=torch.int32):
+                return torch.empty(n + 8, dtype=dtype, device=dev)[:n]   # tail slack for 16-byte bulk copies
+
+            def ptr(t):
+                return t.data_ptr() if t.numel() else None
+
+            v0, v1 = int(po[p]), int(po[p + 1])
+            for i in range(P):
+                s0, s1, Ei = int(po[i]), int(po[i + 1]), int(counts[i])
+                c = CSCSegment()
+                c.edge_size = Ei
+                c.batch_size_forward, c.batch_size_backward = v1 - v0, s1 - s0
+                c.src_range, c.dst_range = (s0, s1), (v0, v1)
+                c.column_offset_gpu, c.row_offset_gpu = vec(v1 - v0 + 1), vec(s1 - s0 + 1)
+                c.row_indices_gpu, c.column_indices_gpu = edges(Ei), edges(Ei)
+                c.edge_weight_forward_gpu = edges(Ei, torch.float32)
+                c.edge_weight_backward_gpu = edges(Ei, torch.float32)
+                c.source_active_gpu = vec(s1 - s0, torch.uint8)
+                _lib.call("nts_graph_build_export_chunk", h, i, ptr(c.column_offset_gpu), ptr(c.row_indices_gpu),
+                          ptr(c.edge_weight_forward_gpu), ptr(c.row_offset_gpu), ptr(c.column_indices_gpu),
+                          ptr(c.edge_weight_backward_gpu), ptr(c.source_active_gpu), stream)
+                pg.graph_chunks.append(c)
+            pg.owned_edges = int(counts.sum())
+            pg.out_degree_gpu, pg.in_degree_gpu = vec(V), vec(V)
+            _lib.call("nts_graph_build_export_degrees", h, ptr(pg.out_degree_gpu), ptr(pg.in_degree_gpu), stream)
+            if dist:
+                pg.owned_mirrors = int(mirrors[0])
+                pg.mirror_index_gpu = vec(V + 1)
+                pg.column_offset_gpu = vec(v1 - v0 + 1)
+                pg.row_indices_gpu = edges(pg.owned_edges)
+                _lib.call("nts_graph_build_export_dist", h, ptr(pg.mirror_index_gpu), ptr(pg.column_offset_gpu),
+                          ptr(pg.row_indices_gpu), stream)
+            return pg
+        finally:
+            L.nts_graph_build_destroy(h)   # cudaFree waits for the export copies
+
+
+def _lib_flags(dist):
+    return 1 if dist else 0   # NTS_GRAPH_BUILD_DIST
