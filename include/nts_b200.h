@@ -160,6 +160,21 @@ uint64_t nts_gather_plan_bytes(const nts_gather_plan *plan);
 /* output[r,:] += sum_e input[row(e),:] * w(e)   (accumulates; one launch per non-empty slab, in stream order) */
 int nts_gather_plan_run(nts_gather_plan *plan, const float *input, float *output, nts_vid_t feature_size,
                         void *stream);
+/* Run flags of the _ex entries.
+ * NTS_PLAN_OVERWRITE: output[r,:] = sum_e ... instead of +=; output may hold anything before the call (NaN included).
+ *   The hub column block, which covers every output element and runs first, stores instead of adding; a plan without
+ *   hub columns zeroes the output first.  Each element gets the value an accumulating run into zeros gives, up to the
+ *   sign of a zero.
+ * NTS_PLAN_COPY_INPUT: gather from a zero-padded copy of the input even where it could be gathered in place (for an
+ *   input whose storage ends before the last row's input_ld-th value). */
+enum { NTS_PLAN_ACCUMULATE = 0, NTS_PLAN_OVERWRITE = 1, NTS_PLAN_COPY_INPUT = 2 };
+/* nts_gather_plan_run on input rows of pitch input_ld floats (>= feature_size).  The input is gathered in place when
+ * input_ld % 4 == 0 and it is 16-byte aligned: the gather then reads all input_ld values of every row, the last one
+ * included, and never writes values past feature_size to an output.  Otherwise its rows are copied into the plan's
+ * zero-padded workspace first (the copy reads feature_size values per row).  The output keeps the pitch
+ * feature_size.  input_ld < feature_size and a null output are rejected. */
+int nts_gather_plan_run_ex(nts_gather_plan *plan, const float *input, nts_vid_t input_ld, float *output,
+                           nts_vid_t feature_size, int flags, void *stream);
 int nts_gather_plan_last_launch(const nts_gather_plan *plan, int *launches, int *grid, int *k, int *u, int *outv);
 /* BF16 gathers with FP32 accumulation: output[r,:] += sum_e w(e) * float(bf16(input[row(e),:])).  bf16() rounds to
  * nearest even (what torch's x.to(torch.bfloat16) computes, incl. inf, NaN and subnormals); weights, accumulation
@@ -170,12 +185,23 @@ int nts_gather_plan_last_launch(const nts_gather_plan *plan, int *launches, int 
 enum { NTS_DTYPE_F32 = 0, NTS_DTYPE_BF16 = 1 };
 int nts_gather_plan_run_bf16(nts_gather_plan *plan, const void *input, int input_dtype, float *output,
                              nts_vid_t feature_size, void *stream);
+/* nts_gather_plan_run_bf16 on input rows of pitch input_ld elements of input_dtype, with the flags of
+ * nts_gather_plan_run_ex (a BF16 input is gathered in place when input_ld % 8 == 0 and it is 16-byte aligned) */
+int nts_gather_plan_run_bf16_ex(nts_gather_plan *plan, const void *input, int input_dtype, nts_vid_t input_ld,
+                                float *output, nts_vid_t feature_size, int flags, void *stream);
 /* nts_gather_plan_create_tuned with the candidates timed as BF16 gathers (and the L2 slab bound counting 2-byte rows):
  * the slab and hub counts that suit BF16 rows of this width */
 nts_gather_plan *nts_gather_plan_create_tuned_bf16(const nts_vid_t *offsets, const nts_vid_t *indices,
                                                    const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
                                                    nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows,
                                                    nts_vid_t feature_size, void *stream);
+/* nts_gather_plan_create_tuned (gather_dtype NTS_DTYPE_F32) or _bf16 (NTS_DTYPE_BF16) with the candidates timed in
+ * the run mode the plan will be used in: run_flags 0 (accumulate) or NTS_PLAN_OVERWRITE */
+nts_gather_plan *nts_gather_plan_create_tuned_ex(const nts_vid_t *offsets, const nts_vid_t *indices,
+                                                 const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
+                                                 nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows,
+                                                 nts_vid_t feature_size, int gather_dtype, int run_flags,
+                                                 void *stream);
 int nts_gather_plan_set_tuning(int u, int min_blocks, int edges_per_warp); /* measurement hook, 0 = default */
 /* 0 = gathered rows through registers (default); 1 = rows staged in shared memory by per-row cp.async.bulk (TMA) into
  * a per-warp ring, U of set_tuning = ring depth - the north star's "feature tiles via TMA", kept for measurement */

@@ -52,9 +52,10 @@ inline bool aligned_to(const void *p, size_t a) { return (reinterpret_cast<uintp
 int sm_count();
 
 // BF16 gathers of nts_plan.cu for the exchange engine: rows of an explicit stride (lds elements of the input type),
-// and the conversion pass that writes BF16 rows of stride ld (ld % 8 == 0, zero past F, dst 16-byte aligned)
+// and the conversion pass that writes BF16 rows of stride ld (ld % 8 == 0, zero past F, dst 16-byte aligned);
+// flags as for nts_gather_plan_run_bf16_ex (0: accumulate)
 int run_plan_bf16(nts_gather_plan *pl, const void *input, int dtype, uint32_t lds, float *output, uint32_t F,
-                  cudaStream_t st);
+                  cudaStream_t st, int flags = 0);
 int to_bf16_rows(const void *src, int dtype, uint32_t lds, void *dst, uint32_t n_rows, uint32_t F, uint32_t ld,
                  cudaStream_t st);
 

@@ -18,9 +18,11 @@
 //   2. (row, weight) pairs.  The base / slot lookup is applied at plan time and row index and weight are stored
 //      interleaved, so the per-edge broadcast read from shared memory is ONE 8-byte LDS instead of two 4-byte ones,
 //      and the TMA bulk copy (cp.async.bulk -> SASS UBLKCP) stages one array per CTA instead of two.
-//   3. 16-byte feature loads for every width.  Rows whose byte length is not a multiple of 16 (F = 602: 2408 B) are
-//      copied once per call into a workspace with rows padded to a multiple of 4 floats, so the gather always uses float4 loads on 16-byte aligned rows and one warp covers up to 640
-//      columns: 19 + 1 data-stage wavefronts per edge at F = 602 instead of 21.6 + 4.
+//   3. 16-byte feature loads for every width.  An input whose row pitch is a multiple of 4 floats is gathered in
+//      place; rows whose byte length is not a multiple of 16 (a contiguous F = 602 input: 2408 B) are copied once per
+//      call into a workspace with rows padded to a multiple of 4 floats, so the gather always uses float4 loads on
+//      16-byte aligned rows and one warp covers up to 640 columns: 19 + 1 data-stage wavefronts per edge at F = 602
+//      instead of 21.6 + 4.
 //
 // Plan construction (hand-written kernels + one CUB radix sort) replaces nothing in the reference: its chunks are
 // built on the host by single-threaded loops (core/PartitionedGraph.hpp:324-420) and never re-bucketed.
@@ -218,14 +220,15 @@ __global__ void plan_cell_sum_kernel(const uint64_t *__restrict__ cell_key, cons
   }
 }
 
-// dst[r, 0:ld] = {src[r, 0:F], 0...}   (ld = F rounded up to a multiple of 4; one warp per row piece)
-__global__ void pad_rows_kernel(const float *__restrict__ src, float *__restrict__ dst, uint32_t n_rows, uint32_t F,
-                                uint32_t ld) {
+// dst[r, 0:ld] = {src[r, 0:F], 0...} for src rows of stride lds   (ld = F rounded up to a multiple of 4; one warp per
+// row piece)
+__global__ void pad_rows_kernel(const float *__restrict__ src, uint32_t lds, float *__restrict__ dst, uint32_t n_rows,
+                                uint32_t F, uint32_t ld) {
   const uint64_t total = (uint64_t)n_rows * ld;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t r = i / ld;
     const uint32_t c = (uint32_t)(i - r * ld);
-    dst[i] = c < F ? __ldg(src + r * F + c) : 0.f;
+    dst[i] = c < F ? __ldg(src + r * lds + c) : 0.f;
   }
 }
 
@@ -326,6 +329,25 @@ __device__ __forceinline__ void flush_chunk(float *__restrict__ orow, uint32_t c
         else
           orow[col + i] += v[i];
       }
+  }
+}
+
+// flush_chunk's plain store: the chunk's columns (< F) are written without reading the output.
+template <int OUTV>
+__device__ __forceinline__ void store_chunk(float *__restrict__ orow, uint32_t col, uint32_t F, float4 a) {
+  if constexpr (OUTV == 4) {
+    *reinterpret_cast<float4 *>(orow + col) = a;
+  } else if constexpr (OUTV == 2) {
+    float2 *p = reinterpret_cast<float2 *>(orow + col);
+    p[0] = make_float2(a.x, a.y);
+    if (col + 2 < F)
+      p[1] = make_float2(a.z, a.w);
+  } else {
+    const float v[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+      if (col + i < F)
+        orow[col + i] = v[i];
   }
 }
 
@@ -758,10 +780,13 @@ static int launch_planned_tma(nts_gather_plan *pl, const PlanShape &sh, const fl
 // ---- dense hub blocks: FP32 SIMT GEMM (FFMA only, no tensor cores) ----------------------------------------------------
 //   out[rowmap(m), n] += sum_{k in this CTA's K range} At[k, m] * B[colmap(k), n]      m < M, n < F
 // At is the block stored K-major ([K x lda], lda % 4 == 0, columns M..lda zero), B rows are ldb floats, 16-byte
-// aligned and zero past F (the input or the padded workspace), so both operand tiles are rows of 16-byte chunks that
+// aligned (the input or the padded workspace; values past F only reach accumulators of columns >= F, which the
+// epilogue never writes), so both operand tiles are rows of 16-byte chunks that
 // cp.async copies straight into double-buffered shared memory (zero-filled past the edges).  128 x 128 x 16 tiles,
 // 256 threads, 8 x 8 outputs per thread.  Column block: colmap = hub columns, rowmap = identity, one CTA per output
-// tile -> plain read-modify-write.  Row block: colmap = identity, rowmap = hub rows, split-K -> vector red.
+// tile -> plain read-modify-write, or with STORE a plain store of the tile (overwrite runs: M = every output row, so
+// the column block writes each output element exactly once and initialises the output for the launches after it).
+// Row block: colmap = identity, rowmap = hub rows, split-K -> vector red.
 // blockIdx.x = (split * m_tiles + m_tile) * n_tiles + n_tile: the N tiles of one A tile run back to back (A from L2).
 constexpr int kHubBM = 128, kHubBN = 128, kHubBK = 16, kHubThreads = 256;
 
@@ -783,12 +808,13 @@ template <int TN, class TB> struct HubSmem {
   TB Bs[2][kHubBK][kBN];
 };
 
-template <class TB, int OUTV, bool SPLIT, int TN, int KKU>
+template <class TB, int OUTV, bool SPLIT, bool STORE, int TN, int KKU>
 __device__ __forceinline__ void hub_gemm_tile(HubSmem<TN, TB> &sm, uint32_t tile, const float *__restrict__ At,
                                               uint32_t lda, uint32_t M, uint32_t k_lo, uint32_t k_hi, uint32_t k_split,
                                               const TB *__restrict__ B, uint32_t ldb,
                                               const uint32_t *__restrict__ colmap, float *__restrict__ out, uint32_t F,
                                               const uint32_t *__restrict__ rowmap, uint32_t m_tiles, uint32_t n_tiles) {
+  static_assert(!(SPLIT && STORE), "split-K partials must be added, not stored");
   constexpr bool kBf16 = std::is_same<TB, __nv_bfloat16>::value;
   constexpr uint32_t kBV = 16 / sizeof(TB); // B values per 16-byte chunk
   constexpr uint32_t kBN = HubSmem<TN, TB>::kBN;
@@ -882,22 +908,27 @@ __device__ __forceinline__ void hub_gemm_tile(HubSmem<TN, TB> &sm, uint32_t tile
 #pragma unroll
     for (int j = 0; j < TN / 4; j++) {
       const uint32_t col = n0 + j * 64 + tx * 4;
-      if (col < F)
-        flush_chunk<OUTV, SPLIT>(orow, col, F,
-                                 make_float4(acc[i][j * 4], acc[i][j * 4 + 1], acc[i][j * 4 + 2], acc[i][j * 4 + 3]));
+      const float4 a = make_float4(acc[i][j * 4], acc[i][j * 4 + 1], acc[i][j * 4 + 2], acc[i][j * 4 + 3]);
+      if (col < F) {
+        if constexpr (STORE)
+          store_chunk<OUTV>(orow, col, F, a);
+        else
+          flush_chunk<OUTV, SPLIT>(orow, col, F, a);
+      }
     }
   }
 }
 
-template <class TB, int OUTV, bool SPLIT>
+// STORE: every tile has a non-empty K range (the column block's K = hub_cols >= 1), so no output tile is skipped.
+template <class TB, int OUTV, bool SPLIT, bool STORE>
 __global__ void __launch_bounds__(kHubThreads, 2)
     hub_block_gemm_kernel(const float *__restrict__ At, uint32_t lda, uint32_t M, uint32_t K, uint32_t k_split,
                           const TB *__restrict__ B, uint32_t ldb, const uint32_t *__restrict__ colmap,
                           float *__restrict__ out, uint32_t F, const uint32_t *__restrict__ rowmap, uint32_t m_tiles,
                           uint32_t n_tiles) {
   __shared__ __align__(16) HubSmem<8, TB> sm;
-  hub_gemm_tile<TB, OUTV, SPLIT, 8, kHubBK>(sm, blockIdx.x, At, lda, M, 0, K, k_split, B, ldb, colmap, out, F, rowmap, m_tiles,
-                                    n_tiles);
+  hub_gemm_tile<TB, OUTV, SPLIT, STORE, 8, kHubBK>(sm, blockIdx.x, At, lda, M, 0, K, k_split, B, ldb, colmap, out, F,
+                                                   rowmap, m_tiles, n_tiles);
 }
 
 // Split-K length of the row block (M = hub_rows, K = gather_rows): about 4 waves of 2 CTAs per SM over the whole K,
@@ -909,18 +940,20 @@ static uint32_t hub_row_k_split(uint32_t K, uint32_t m_tiles, uint32_t n_tiles) 
   return std::max<uint32_t>((k_split + kHubBK - 1) / kHubBK * kHubBK, 16 * kHubBK);
 }
 
-// rows = false: the column block only (the row block runs inside the fused slab launches).
+// rows = false: the column block only (the row block runs inside the fused slab launches).  overwrite: the column
+// block stores its tiles instead of adding them (it covers every output element, and it launches first).
 template <class TB, int OUTV>
 static int launch_hub_blocks(nts_gather_plan *pl, const TB *in, uint32_t ldb, float *out, uint32_t F, bool rows,
-                             cudaStream_t st) {
+                             bool overwrite, cudaStream_t st) {
   const uint32_t n_tiles = (F + kHubBN - 1) / kHubBN;
   if (pl->hub_cols) { // column block: M = n_rows, K = hub_cols
     const uint32_t m_tiles = (pl->n_rows + kHubBM - 1) / kHubBM;
     const uint64_t blocks = (uint64_t)m_tiles * n_tiles;
     NTS_ARG_CHECK(blocks <= 0x7fffffffull, "hub column block grid too large");
-    hub_block_gemm_kernel<TB, OUTV, false><<<(unsigned)blocks, kHubThreads, 0, st>>>(
-        pl->dense, pl->lda_c, pl->n_rows, (uint32_t)pl->hub_cols, (uint32_t)pl->hub_cols, in, ldb, pl->hub_col_ids, out,
-        F, nullptr, m_tiles, n_tiles);
+    auto kern = overwrite ? hub_block_gemm_kernel<TB, OUTV, false, true> : hub_block_gemm_kernel<TB, OUTV, false, false>;
+    kern<<<(unsigned)blocks, kHubThreads, 0, st>>>(pl->dense, pl->lda_c, pl->n_rows, (uint32_t)pl->hub_cols,
+                                                   (uint32_t)pl->hub_cols, in, ldb, pl->hub_col_ids, out, F, nullptr,
+                                                   m_tiles, n_tiles);
     NTS_LAUNCH_CHECK();
   }
   if (pl->hub_rows && rows) { // row block: M = hub_rows, K = gather_rows
@@ -928,7 +961,7 @@ static int launch_hub_blocks(nts_gather_plan *pl, const TB *in, uint32_t ldb, fl
     const uint32_t K = pl->gather_rows;
     const uint32_t k_split = hub_row_k_split(K, m_tiles, n_tiles);
     const uint64_t splits = (K + k_split - 1) / k_split;
-    hub_block_gemm_kernel<TB, OUTV, true><<<(unsigned)(splits * m_tiles * n_tiles), kHubThreads, 0, st>>>(
+    hub_block_gemm_kernel<TB, OUTV, true, false><<<(unsigned)(splits * m_tiles * n_tiles), kHubThreads, 0, st>>>(
         pl->dense + (size_t)pl->hub_cols * pl->lda_c, pl->lda_r, (uint32_t)pl->hub_rows, K, k_split, in, ldb, nullptr,
         out, F, pl->hub_row_ids, m_tiles, n_tiles);
     NTS_LAUNCH_CHECK();
@@ -968,7 +1001,7 @@ __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const uint32_t b = blockIdx.x, grp = b / hub.period;
   if (grp < hub.n_gemm && b - grp * hub.period == hub.period - 1)
-    hub_gemm_tile<T, OUTV, true, TN, TN == 8 ? kHubBK : 4>(
+    hub_gemm_tile<T, OUTV, true, false, TN, TN == 8 ? kHubBK : 4>(
         *reinterpret_cast<HubSmem<TN, T> *>(smem_raw), grp, hub.At, hub.lda, hub.M, hub.k_lo, hub.k_hi, hub.k_split,
         reinterpret_cast<const T *>(in), ldc * GatherT<T>::V, nullptr, out, F, hub.rowmap, hub.m_tiles, hub.n_tiles);
   else
@@ -1030,10 +1063,13 @@ static int launch_fused(nts_gather_plan *pl, const PlanShape &sh, const T *in_ro
   }
 
 // The gather of rows already in the kernel's layout: `in` holds gather_rows rows of ld values of T, 16-byte aligned,
-// ld % V == 0, zero past F.  Dense hub blocks first, then the residual edges' slab launches (stream order); with
-// pl->overlap the row block runs inside the slab launches instead (planned_slab_hub_kernel).
+// ld % V == 0 (columns F..ld are read but never reach an output).  Dense hub blocks first, then the residual edges'
+// slab launches (stream order); with pl->overlap the row block runs inside the slab launches instead
+// (planned_slab_hub_kernel).  overwrite: output = A in instead of output += A in; the column block stores the first
+// value of every output element, or, in a plan without hub columns, the output is zeroed first.
 template <class T>
-static int run_gather(nts_gather_plan *pl, const T *in, uint32_t ld, float *output, uint32_t F, cudaStream_t st) {
+static int run_gather(nts_gather_plan *pl, const T *in, uint32_t ld, float *output, uint32_t F, bool overwrite,
+                      cudaStream_t st) {
   constexpr bool kBf16 = std::is_same<T, __nv_bfloat16>::value;
   PlanShape sh;
   const uint32_t ldc = ld / GatherT<T>::V; // 16-byte chunks per row
@@ -1046,10 +1082,12 @@ static int run_gather(nts_gather_plan *pl, const T *in, uint32_t ld, float *outp
   sh.outv = (F % 4 == 0 && aligned_to(output, 16)) ? 4 : ((F % 2 == 0 && aligned_to(output, 8)) ? 2 : 1);
   const bool fused = pl->overlap && pl->hub_rows;
   NTS_ARG_CHECK(!fused || g_plan_variant == 0, "the fused slab launches use the register-staging gather (variant 0)");
+  if (overwrite && !pl->hub_cols)
+    NTS_CUDA_OK(cudaMemsetAsync(output, 0, (size_t)pl->n_rows * F * sizeof(float), st));
   if (pl->hub_cols || pl->hub_rows) {
-    const int rc = sh.outv == 4   ? launch_hub_blocks<T, 4>(pl, in, ld, output, F, !fused, st)
-                   : sh.outv == 2 ? launch_hub_blocks<T, 2>(pl, in, ld, output, F, !fused, st)
-                                  : launch_hub_blocks<T, 1>(pl, in, ld, output, F, !fused, st);
+    const int rc = sh.outv == 4   ? launch_hub_blocks<T, 4>(pl, in, ld, output, F, !fused, overwrite, st)
+                   : sh.outv == 2 ? launch_hub_blocks<T, 2>(pl, in, ld, output, F, !fused, overwrite, st)
+                                  : launch_hub_blocks<T, 1>(pl, in, ld, output, F, !fused, overwrite, st);
     if (rc)
       return rc;
   }
@@ -1194,23 +1232,47 @@ template <class E> static int ensure_workspace(E *&ws, size_t &have, size_t elem
   return 0;
 }
 
-static int run_plan(nts_gather_plan *pl, const float *input, float *output, uint32_t F, cudaStream_t st) {
-  if (pl->n_rows == 0 || pl->n_edges == 0 || F == 0)
+// Argument checks and the runs with nothing to gather, shared by the FP32 and BF16 entries: *done = the run is
+// complete (an empty overwrite run still zeroes its output).  Returns 0 or the error.
+static int run_prologue(nts_gather_plan *pl, const void *input, uint32_t lds, float *output, uint32_t F, int flags,
+                        bool *done, cudaStream_t st) {
+  *done = true;
+  NTS_ARG_CHECK((flags & ~(NTS_PLAN_OVERWRITE | NTS_PLAN_COPY_INPUT)) == 0, "unknown plan run flags");
+  if (pl->n_rows == 0 || F == 0)
     return 0;
-  NTS_ARG_CHECK(input && output, "null feature pointer");
-  // 16-byte loads need 16-byte aligned rows: otherwise gather from a zero-padded copy (ld = F rounded up to 4)
-  const uint32_t ld = (F + 3u) & ~3u;
-  const float *in = input;
-  if (ld != F || !aligned_to(input, 16)) {
-    if (const int rc = ensure_workspace(pl->workspace, pl->workspace_floats, (size_t)pl->gather_rows * ld))
-      return rc;
-    const uint64_t total = (uint64_t)pl->gather_rows * ld;
-    const unsigned blocks = (unsigned)std::min<uint64_t>((total + 255) / 256, (uint64_t)sm_count() * 32);
-    pad_rows_kernel<<<blocks, 256, 0, st>>>(input, pl->workspace, pl->gather_rows, F, ld);
-    NTS_LAUNCH_CHECK();
-    in = pl->workspace;
+  if (pl->n_edges == 0) {
+    if (flags & NTS_PLAN_OVERWRITE) {
+      NTS_ARG_CHECK(output != nullptr, "null output pointer");
+      NTS_CUDA_OK(cudaMemsetAsync(output, 0, (size_t)pl->n_rows * F * sizeof(float), st));
+    }
+    return 0;
   }
-  return run_gather<float>(pl, in, ld, output, F, st);
+  NTS_ARG_CHECK(input && output, "null feature pointer");
+  NTS_ARG_CHECK(lds >= F, "row stride below the feature width");
+  *done = false;
+  return 0;
+}
+
+// FP32 rows of stride lds.  16-byte loads need 16-byte aligned rows: the input is gathered in place when lds % 4 == 0
+// and it is aligned (the gather then reads columns F..lds of every row, the last one included, but never writes them
+// to an output); otherwise, or with NTS_PLAN_COPY_INPUT, from a zero-padded copy (ld = F rounded up to 4).
+static int run_plan(nts_gather_plan *pl, const float *input, uint32_t lds, float *output, uint32_t F, int flags,
+                    cudaStream_t st) {
+  bool done = false;
+  if (const int rc = run_prologue(pl, input, lds, output, F, flags, &done, st))
+    return rc;
+  if (done)
+    return 0;
+  if (lds % 4 == 0 && aligned_to(input, 16) && !(flags & NTS_PLAN_COPY_INPUT))
+    return run_gather<float>(pl, input, lds, output, F, flags & NTS_PLAN_OVERWRITE, st);
+  const uint32_t ld = (F + 3u) & ~3u;
+  if (const int rc = ensure_workspace(pl->workspace, pl->workspace_floats, (size_t)pl->gather_rows * ld))
+    return rc;
+  const uint64_t total = (uint64_t)pl->gather_rows * ld;
+  const unsigned blocks = (unsigned)std::min<uint64_t>((total + 255) / 256, (uint64_t)sm_count() * 32);
+  pad_rows_kernel<<<blocks, 256, 0, st>>>(input, lds, pl->workspace, pl->gather_rows, F, ld);
+  NTS_LAUNCH_CHECK();
+  return run_gather<float>(pl, pl->workspace, ld, output, F, flags & NTS_PLAN_OVERWRITE, st);
 }
 
 // dst[r, 0:ld] = {bf16(src[r, 0:F]), 0...} for rows of stride lds (elements of src's type); ld % 8 == 0
@@ -1234,23 +1296,26 @@ int to_bf16_rows(const void *src, int dtype, uint32_t lds, void *dst, uint32_t n
 
 // BF16 gathers on rows of stride lds elements: an FP32 input is rounded into the BF16 workspace (stride ld = F rounded
 // up to 8); a BF16 input is gathered in place when its stride is a whole number of 16-byte chunks and it is aligned
-// (values between F and lds are never written to an output column), else re-strided into the workspace.
+// (values between F and lds are never written to an output column), else (or with NTS_PLAN_COPY_INPUT) re-strided
+// into the workspace.  flags: NTS_PLAN_OVERWRITE / NTS_PLAN_COPY_INPUT as for nts_gather_plan_run_ex.
 int run_plan_bf16(nts_gather_plan *pl, const void *input, int dtype, uint32_t lds, float *output, uint32_t F,
-                  cudaStream_t st) {
+                  cudaStream_t st, int flags) {
   NTS_ARG_CHECK(dtype == NTS_DTYPE_F32 || dtype == NTS_DTYPE_BF16, "input dtype must be NTS_DTYPE_F32 or NTS_DTYPE_BF16");
   NTS_ARG_CHECK(g_plan_variant == 0, "the TMA row-staging variant (nts_gather_plan_set_variant(1)) gathers FP32 rows only");
-  if (pl->n_rows == 0 || pl->n_edges == 0 || F == 0)
+  bool done = false;
+  if (const int rc = run_prologue(pl, input, lds, output, F, flags, &done, st))
+    return rc;
+  if (done)
     return 0;
-  NTS_ARG_CHECK(input && output, "null feature pointer");
-  NTS_ARG_CHECK(lds >= F, "row stride below the feature width");
-  if (dtype == NTS_DTYPE_BF16 && lds % 8 == 0 && aligned_to(input, 16))
-    return run_gather<__nv_bfloat16>(pl, static_cast<const __nv_bfloat16 *>(input), lds, output, F, st);
+  const bool overwrite = flags & NTS_PLAN_OVERWRITE;
+  if (dtype == NTS_DTYPE_BF16 && lds % 8 == 0 && aligned_to(input, 16) && !(flags & NTS_PLAN_COPY_INPUT))
+    return run_gather<__nv_bfloat16>(pl, static_cast<const __nv_bfloat16 *>(input), lds, output, F, overwrite, st);
   const uint32_t ld = (F + 7u) & ~7u;
   if (const int rc = ensure_workspace(pl->workspace_bf16, pl->workspace_bf16_elems, (size_t)pl->gather_rows * ld))
     return rc;
   if (const int rc = to_bf16_rows(input, dtype, lds, pl->workspace_bf16, pl->gather_rows, F, ld, st))
     return rc;
-  return run_gather<__nv_bfloat16>(pl, pl->workspace_bf16, ld, output, F, st);
+  return run_gather<__nv_bfloat16>(pl, pl->workspace_bf16, ld, output, F, overwrite, st);
 }
 
 } // namespace nts
@@ -1650,7 +1715,7 @@ nts_gather_plan *nts_plan_create_parts_typed(const nts_plan_part *parts, int n_p
       float t = 0.f;
       if (cudaEventRecord(e0, st) != cudaSuccess ||
           (bf16 ? run_plan_bf16(pl, x, NTS_DTYPE_BF16, feature_size, y, feature_size, st)
-                : run_plan(pl, x, y, feature_size, st)) != 0 ||
+                : run_plan(pl, x, feature_size, y, feature_size, 0, st)) != 0 ||
           cudaEventRecord(e1, st) != cudaSuccess || cudaEventSynchronize(e1) != cudaSuccess ||
           cudaEventElapsedTime(&t, e0, e1) != cudaSuccess)
         return false;
@@ -1716,10 +1781,12 @@ static constexpr double kHubFloor = 0.05;
 static constexpr int kHubMax = 512;
 
 // bf16: candidates are timed with BF16 gathers (a BF16 input of width feature_size, gathered as a BF16 run gathers
-// it) and the slab bound counts rows of ceil(F/8)*8 2-byte values.
+// it) and the slab bound counts rows of ceil(F/8)*8 2-byte values.  run_flags: the mode the candidates are timed in
+// (NTS_PLAN_OVERWRITE prices the column block at its store cost, not at a read-modify-write of the whole output).
 static nts_gather_plan *create_tuned(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
                                      const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows, uint64_t n_edges,
-                                     nts_vid_t gather_rows, nts_vid_t feature_size, bool bf16, void *stream) {
+                                     nts_vid_t gather_rows, nts_vid_t feature_size, bool bf16, int run_flags,
+                                     void *stream) {
   cudaStream_t st = as_stream(stream);
   const uint64_t row_bytes = bf16 ? ((feature_size + 7ull) & ~7ull) * 2ull : ((feature_size + 3ull) & ~3ull) * 4ull;
   const int s_max = pick_slabs_for_rows(gather_rows, n_edges, n_rows, row_bytes, 16ull << 20);
@@ -1738,8 +1805,8 @@ static nts_gather_plan *create_tuned(const nts_vid_t *offsets, const nts_vid_t *
             cudaMemsetAsync(x, 0, xb, st) == cudaSuccess && cudaMemsetAsync(y, 0, yb, st) == cudaSuccess &&
             cudaEventCreate(&e0) == cudaSuccess && cudaEventCreate(&e1) == cudaSuccess;
   auto run_one = [&](nts_gather_plan *pl) {
-    return bf16 ? run_plan_bf16(pl, x, NTS_DTYPE_BF16, feature_size, y, feature_size, st)
-                : run_plan(pl, x, y, feature_size, st);
+    return bf16 ? run_plan_bf16(pl, x, NTS_DTYPE_BF16, feature_size, y, feature_size, st, run_flags)
+                : run_plan(pl, x, feature_size, y, feature_size, run_flags, st);
   };
   auto time_plan = [&](nts_gather_plan *pl, float *ms) -> bool {
     *ms = 1e30f;
@@ -1837,7 +1904,7 @@ nts_gather_plan *nts_gather_plan_create_tuned(const nts_vid_t *offsets, const nt
                                               uint64_t n_edges, nts_vid_t gather_rows, nts_vid_t feature_size,
                                               void *stream) {
   return create_tuned(offsets, indices, weight, slot_of, index_base, n_rows, n_edges, gather_rows, feature_size, false,
-                      stream);
+                      0, stream);
 }
 
 nts_gather_plan *nts_gather_plan_create_tuned_bf16(const nts_vid_t *offsets, const nts_vid_t *indices,
@@ -1845,7 +1912,21 @@ nts_gather_plan *nts_gather_plan_create_tuned_bf16(const nts_vid_t *offsets, con
                                                    nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows,
                                                    nts_vid_t feature_size, void *stream) {
   return create_tuned(offsets, indices, weight, slot_of, index_base, n_rows, n_edges, gather_rows, feature_size, true,
-                      stream);
+                      0, stream);
+}
+
+nts_gather_plan *nts_gather_plan_create_tuned_ex(const nts_vid_t *offsets, const nts_vid_t *indices,
+                                                 const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
+                                                 nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows,
+                                                 nts_vid_t feature_size, int gather_dtype, int run_flags,
+                                                 void *stream) {
+  if ((gather_dtype != NTS_DTYPE_F32 && gather_dtype != NTS_DTYPE_BF16) || (run_flags & ~NTS_PLAN_OVERWRITE)) {
+    fail(-1, "nts_gather_plan_create_tuned_ex: gather_dtype must be NTS_DTYPE_F32 or NTS_DTYPE_BF16, run_flags 0 or "
+             "NTS_PLAN_OVERWRITE", __FILE__, __LINE__);
+    return nullptr;
+  }
+  return create_tuned(offsets, indices, weight, slot_of, index_base, n_rows, n_edges, gather_rows, feature_size,
+                      gather_dtype == NTS_DTYPE_BF16, run_flags, stream);
 }
 
 int nts_gather_plan_destroy(nts_gather_plan *pl) {
@@ -1906,13 +1987,29 @@ int nts_gather_plan_last_launch(const nts_gather_plan *pl, int *launches, int *g
 
 int nts_gather_plan_run(nts_gather_plan *pl, const float *input, float *output, nts_vid_t feature_size, void *stream) {
   NTS_ARG_CHECK(pl != nullptr, "null plan");
-  return run_plan(pl, input, output, feature_size, as_stream(stream));
+  return run_plan(pl, input, feature_size, output, feature_size, 0, as_stream(stream));
+}
+
+int nts_gather_plan_run_ex(nts_gather_plan *pl, const float *input, nts_vid_t input_ld, float *output,
+                           nts_vid_t feature_size, int flags, void *stream) {
+  NTS_ARG_CHECK(input_ld >= feature_size, "input row pitch below the feature width");
+  NTS_ARG_CHECK(output != nullptr || feature_size == 0, "null output pointer");
+  NTS_ARG_CHECK(pl != nullptr, "null plan");
+  return run_plan(pl, input, input_ld, output, feature_size, flags, as_stream(stream));
 }
 
 int nts_gather_plan_run_bf16(nts_gather_plan *pl, const void *input, int input_dtype, float *output,
                              nts_vid_t feature_size, void *stream) {
   NTS_ARG_CHECK(pl != nullptr, "null plan");
   return run_plan_bf16(pl, input, input_dtype, feature_size, output, feature_size, as_stream(stream));
+}
+
+int nts_gather_plan_run_bf16_ex(nts_gather_plan *pl, const void *input, int input_dtype, nts_vid_t input_ld,
+                                float *output, nts_vid_t feature_size, int flags, void *stream) {
+  NTS_ARG_CHECK(input_ld >= feature_size, "input row pitch below the feature width");
+  NTS_ARG_CHECK(output != nullptr || feature_size == 0, "null output pointer");
+  NTS_ARG_CHECK(pl != nullptr, "null plan");
+  return run_plan_bf16(pl, input, input_dtype, input_ld, output, feature_size, as_stream(stream), flags);
 }
 
 int nts_rows_to_bf16(const void *src, int src_dtype, nts_vid_t lds, void *dst, nts_vid_t n_rows, nts_vid_t feature_size,

@@ -1,7 +1,8 @@
 """Graph operators with the reference's `ntsGraphOp` interface (core/ntsBaseOp.hpp:24-48):
 constructed from `(PartitionedGraph, active)`, `forward(x)` / `forward(x, w)`, `backward(grad)`,
 `get_additional_grad()`; outputs are freshly allocated zero tensors the kernels accumulate into
-(NtsScheduler::NewKeyTensor / NewLeafTensor, core/NtsScheduler.hpp:378-394).
+(NtsScheduler::NewKeyTensor / NewLeafTensor, core/NtsScheduler.hpp:378-394), except ForwardSingleGPUfuseOp's, which
+its aggregation writes without a zero fill.
 
 Every operator calls the sm_90a kernels through the C ABI (`_lib.call`); tensors only provide device
 memory and the current CUDA stream.  There is no CPU path: a CPU tensor raises.
@@ -20,14 +21,21 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
-def _check_input(t, name="input"):
+def row_pitched(t):
+    """True for a 2-D tensor whose rows are contiguous and start a row pitch >= its width apart (a contiguous tensor,
+    or a column slice t[:, :F] of one)."""
+    return t.dim() == 2 and (t.is_contiguous() or (t.stride(1) == 1 and t.stride(0) >= t.shape[1]))
+
+
+def _check_input(t, name="input", pitched=False):
+    """pitched=True: also accept row-pitched tensors (row_pitched), for operators that pass the row pitch on."""
     if not t.is_cuda:
         raise _lib.NtsError("%s must be a CUDA tensor (libnts_b200 has no CPU fallback)" % name)
     if t.dtype != torch.float32 or t.dim() != 2:
         raise _lib.NtsError("%s must be a 2-D float32 tensor" % name)
-    if not t.is_contiguous():
+    if not (t.is_contiguous() or (pitched and row_pitched(t))):
         # the reference borrows packed_accessor storage (core/NtsScheduler.hpp:505-515): contiguous only
-        raise _lib.NtsError("%s must be contiguous" % name)
+        raise _lib.NtsError("%s must be contiguous" % name + (" or row-pitched" if pitched else ""))
     return t
 
 
@@ -38,20 +46,21 @@ def _check_gather_dtype(gather_dtype):
     return gather_dtype
 
 
-def _check_gathered(t, name, gather_dtype):
+def _check_gathered(t, name, gather_dtype, pitched=False):
     """_check_input for a gathered operand: with BF16 gathers a bfloat16 tensor is accepted as well (used as is)."""
     if gather_dtype is None or (t.is_cuda and t.dtype == torch.float32):
-        return _check_input(t, name)
+        return _check_input(t, name, pitched)
     if not t.is_cuda:
         raise _lib.NtsError("%s must be a CUDA tensor (libnts_b200 has no CPU fallback)" % name)
     if t.dtype != torch.bfloat16 or t.dim() != 2:
         raise _lib.NtsError("%s must be a 2-D float32 or bfloat16 tensor" % name)
-    if not t.is_contiguous():
-        raise _lib.NtsError("%s must be contiguous" % name)
+    if not (t.is_contiguous() or (pitched and row_pitched(t))):
+        raise _lib.NtsError("%s must be contiguous" % name + (" or row-pitched" if pitched else ""))
     return t
 
 
 _DTYPE_CODE = {torch.float32: 0, torch.bfloat16: 1}   # NTS_DTYPE_F32 / NTS_DTYPE_BF16 of include/nts_b200.h
+PLAN_OVERWRITE, PLAN_COPY_INPUT = 1, 2                # NTS_PLAN_OVERWRITE / NTS_PLAN_COPY_INPUT
 
 
 def _ptr(t):
@@ -119,11 +128,12 @@ class GatherPlan:
     source-slab bucketing (L2 residency), interleaved (row, weight) pairs, 16-byte aligned gathers."""
 
     def __init__(self, offsets, indices, weight, index_base, n_rows, n_edges, gather_rows, slabs, slot_of=None,
-                 tune_for=0, hubs=(0, 0), gather_dtype=None):
+                 tune_for=0, hubs=(0, 0), gather_dtype=None, tune_accumulate=True):
         """slabs > 0: that many source slabs and hubs = (hub columns, hub rows) dense blocks
         (nts_gather_plan_create_hybrid); slabs == 0: slab and hub counts are MEASURED for feature width `tune_for`
-        (nts_gather_plan_create_tuned), timed as BF16 gathers when gather_dtype is torch.bfloat16
-        (nts_gather_plan_create_tuned_bf16).  build_s is the one-time construction (and tuning) time."""
+        (nts_gather_plan_create_tuned_ex), timed as BF16 gathers when gather_dtype is torch.bfloat16, and as
+        overwriting runs (`run(..., accumulate=False)`) when tune_accumulate is False.  build_s is the one-time
+        construction (and tuning) time."""
         L = _lib.load()
         _check_gather_dtype(gather_dtype)
         t0 = _time.perf_counter()
@@ -133,9 +143,10 @@ class GatherPlan:
                                                           int(gather_rows), int(slabs), int(hubs[0]), int(hubs[1]),
                                                           _stream())
         else:
-            create = L.nts_gather_plan_create_tuned_bf16 if gather_dtype is not None else L.nts_gather_plan_create_tuned
-            self.handle = create(_ptr(offsets), _ptr(indices), _ptr(weight), _ptr(slot_of), int(index_base),
-                                 int(n_rows), int(n_edges), int(gather_rows), int(tune_for), _stream())
+            self.handle = L.nts_gather_plan_create_tuned_ex(
+                _ptr(offsets), _ptr(indices), _ptr(weight), _ptr(slot_of), int(index_base), int(n_rows), int(n_edges),
+                int(gather_rows), int(tune_for), _DTYPE_CODE[gather_dtype or torch.float32],
+                0 if tune_accumulate else PLAN_OVERWRITE, _stream())
         self.build_s = _time.perf_counter() - t0      # create synchronises the stream
         if not self.handle:
             raise _lib.NtsError("nts_gather_plan_create failed: " + L.nts_last_error().decode(errors="replace"))
@@ -159,18 +170,28 @@ class GatherPlan:
         return ((self.slabs,) + ((self.hub_cols, self.hub_rows) if self.hub_cols or self.hub_rows else ())
                 + (("overlap",) if self.overlap else ()))
 
-    def run(self, x, out, gather_dtype=None):
-        """out += A x.  gather_dtype=torch.bfloat16: the rows of x (float32 or bfloat16) are gathered as BF16 with FP32
-        accumulation (nts_gather_plan_run_bf16); a bfloat16 x needs that option."""
+    def run(self, x, out, gather_dtype=None, accumulate=True):
+        """out += A x, or out = A x with accumulate=False (out may then hold anything, NaN included).  x may be
+        row-pitched (a column slice x[:, :F] of a wider tensor): its row pitch is passed on, and where the pitch allows
+        it the rows are gathered in place.  gather_dtype=torch.bfloat16: the rows of x (float32 or bfloat16) are
+        gathered as BF16 with FP32 accumulation (nts_gather_plan_run_bf16_ex); a bfloat16 x needs that option."""
+        if not row_pitched(x):
+            raise _lib.NtsError("the gathered input must have contiguous rows (unit column stride)")
+        F = int(x.shape[1])
+        ld = F if x.is_contiguous() else int(x.stride(0))
+        flags = 0 if accumulate else PLAN_OVERWRITE
+        # an in-place gather reads all ld values of the last row too: without storage behind them, gather a copy
+        if ld != F and (x.storage_offset() + x.shape[0] * ld) * x.element_size() > x.untyped_storage().nbytes():
+            flags |= PLAN_COPY_INPUT
         if _check_gather_dtype(gather_dtype) is not None:
             if x.dtype not in _DTYPE_CODE:
                 raise _lib.NtsError("BF16 gathers take a float32 or bfloat16 input, not %s" % x.dtype)
-            _lib.call("nts_gather_plan_run_bf16", self.handle, _ptr(x), _DTYPE_CODE[x.dtype], _ptr(out),
-                      int(x.shape[1]), _stream())
+            _lib.call("nts_gather_plan_run_bf16_ex", self.handle, _ptr(x), _DTYPE_CODE[x.dtype], ld, _ptr(out), F,
+                      flags, _stream())
             return out
         if x.dtype == torch.bfloat16:
             raise _lib.NtsError("a bfloat16 input needs gather_dtype=torch.bfloat16")
-        _lib.call("nts_gather_plan_run", self.handle, _ptr(x), _ptr(out), int(x.shape[1]), _stream())
+        _lib.call("nts_gather_plan_run_ex", self.handle, _ptr(x), ld, _ptr(out), F, flags, _stream())
         return out
 
     def bytes(self):
@@ -206,7 +227,8 @@ def set_plan_mode(mode, slabs=0):
 def _chunk_plan(chunk, direction, F, gather_dtype=None):
     """The GatherPlan of one chunk direction for feature width F, or None when the plain kernel should run.
     BF16 gathers exist only in nts_gather_plan: with gather_dtype=torch.bfloat16 every chunk gets a plan, whatever its
-    size or the plan mode, tuned per (width, type)."""
+    size or the plan mode, tuned per (width, type).  Measured plans are timed as overwriting runs, the mode
+    ForwardSingleGPUfuseOp runs them in."""
     if gather_dtype is None and (_plan_mode == "off" or (_plan_mode == "auto" and chunk.edge_size < PLAN_MIN_EDGES)):
         return None
     if direction == "fwd":
@@ -223,11 +245,11 @@ def _chunk_plan(chunk, direction, F, gather_dtype=None):
         if direction == "fwd":
             plan = GatherPlan(chunk.column_offset_gpu, chunk.row_indices_gpu, chunk.edge_weight_forward_gpu,
                               chunk.src_range[0], n_rows, chunk.edge_size, gather_rows, _plan_slabs, tune_for=int(F),
-                              gather_dtype=gather_dtype)
+                              gather_dtype=gather_dtype, tune_accumulate=False)
         else:
             plan = GatherPlan(chunk.row_offset_gpu, chunk.column_indices_gpu, chunk.edge_weight_backward_gpu,
                               chunk.dst_range[0], n_rows, chunk.edge_size, gather_rows, _plan_slabs, tune_for=int(F),
-                              gather_dtype=gather_dtype)
+                              gather_dtype=gather_dtype, tune_accumulate=False)
         share = (direction,) + plan.key()
         if share in plans:     # another width already settled on these slab and hub counts: share the arrays
             plan = plans[share]
@@ -245,16 +267,25 @@ def _bf16_plan(chunk, direction, F, with_weight, gather_dtype):
     return _chunk_plan(chunk, direction, F, gather_dtype)
 
 
-def gather_by_dst_from_src(chunk, out, x, with_weight=True, gather_dtype=None):
-    """NtsScheduler::GatherByDstFromSrc (core/NtsScheduler.hpp:151-191) on one chunk.  gather_dtype=torch.bfloat16:
-    x (float32 or bfloat16) is gathered as BF16 rows with FP32 accumulation (GatherPlan.run)."""
+def _plain_operands(out, x, accumulate):
+    """The plain kernels accumulate into out and read contiguous rows."""
+    if not accumulate:
+        out.zero_()
+    return x.contiguous()
+
+
+def gather_by_dst_from_src(chunk, out, x, with_weight=True, gather_dtype=None, accumulate=True):
+    """NtsScheduler::GatherByDstFromSrc (core/NtsScheduler.hpp:151-191) on one chunk: out += A x, or out = A x with
+    accumulate=False.  x may be row-pitched (GatherPlan.run).  gather_dtype=torch.bfloat16: x (float32 or bfloat16)
+    is gathered as BF16 rows with FP32 accumulation (GatherPlan.run)."""
     plan = _bf16_plan(chunk, "fwd", x.shape[1], with_weight, gather_dtype)
     ev = _timer.bracket("fwd", x.shape[1], chunk.edge_size, chunk.batch_size_forward) if _timer else None
     if ev:
         ev[0].record()
     if plan is not None:
-        plan.run(x, out, gather_dtype)
+        plan.run(x, out, gather_dtype, accumulate)
     else:
+        x = _plain_operands(out, x, accumulate)
         _lib.call("nts_gather_by_dst_from_src", _ptr(x), _ptr(out), _ptr(chunk.edge_weight_forward_gpu),
                   _ptr(chunk.row_indices_gpu), _ptr(chunk.column_offset_gpu), chunk.src_range[0], chunk.src_range[1],
                   chunk.dst_range[0], chunk.dst_range[1], chunk.edge_size, chunk.batch_size_forward,
@@ -264,16 +295,17 @@ def gather_by_dst_from_src(chunk, out, x, with_weight=True, gather_dtype=None):
     return out
 
 
-def gather_by_src_from_dst(chunk, out, grad, with_weight=True, gather_dtype=None):
-    """NtsScheduler::GatherBySrcFromDst (core/NtsScheduler.hpp:257-293) on one chunk (gather_dtype as in
-    gather_by_dst_from_src: the gathered output gradient is rounded to BF16, dX accumulates in FP32)."""
+def gather_by_src_from_dst(chunk, out, grad, with_weight=True, gather_dtype=None, accumulate=True):
+    """NtsScheduler::GatherBySrcFromDst (core/NtsScheduler.hpp:257-293) on one chunk (accumulate and gather_dtype as
+    in gather_by_dst_from_src: the gathered output gradient is rounded to BF16, dX accumulates in FP32)."""
     plan = _bf16_plan(chunk, "bwd", grad.shape[1], with_weight, gather_dtype)
     ev = _timer.bracket("bwd", grad.shape[1], chunk.edge_size, chunk.batch_size_backward) if _timer else None
     if ev:
         ev[0].record()
     if plan is not None:
-        plan.run(grad, out, gather_dtype)
+        plan.run(grad, out, gather_dtype, accumulate)
     else:
+        grad = _plain_operands(out, grad, accumulate)
         _lib.call("nts_gather_by_src_from_dst", _ptr(grad), _ptr(out), _ptr(chunk.edge_weight_backward_gpu),
                   _ptr(chunk.row_offset_gpu), _ptr(chunk.column_indices_gpu), chunk.src_range[0], chunk.src_range[1],
                   chunk.dst_range[0], chunk.dst_range[1], chunk.edge_size, chunk.batch_size_backward,
@@ -305,23 +337,27 @@ class ForwardSingleGPUfuseOp(ntsGraphOp):
     (core/graph.hpp:3805-3855): Y = A X on chunk 0, dX = A^T dY, no communication.
 
     gather_dtype=torch.bfloat16: the gathered operand (X forward, dY backward) is rounded to BF16 and accumulated in
-    FP32; forward takes a float32 or bfloat16 X, Y and dX are float32, backward takes a float32 dY."""
+    FP32; forward takes a float32 or bfloat16 X, Y and dX are float32, backward takes a float32 dY.
+
+    X and dY may be row-pitched (a column slice of a wider tensor, ops.row_pitched): a planned run passes the pitch on
+    and gathers the rows in place when it is a multiple of 16 bytes.  Y and dX are freshly allocated and written by
+    overwriting runs (GatherPlan.run(..., accumulate=False)), never zero-filled first."""
 
     def __init__(self, partitioned_graph, active=None, gather_dtype=None):
         super().__init__(partitioned_graph, active)
         self.gather_dtype = _check_gather_dtype(gather_dtype)
 
     def forward(self, f_input, f_input1=None):
-        x = _check_gathered(f_input, "input", self.gather_dtype)
+        x = _check_gathered(f_input, "input", self.gather_dtype, pitched=True)
         c = self.partitioned_graph_.graph_chunks[0]
-        y = torch.zeros((c.batch_size_forward, x.shape[1]), dtype=torch.float32, device=x.device)
-        return gather_by_dst_from_src(c, y, x, gather_dtype=self.gather_dtype)
+        y = torch.empty((c.batch_size_forward, x.shape[1]), dtype=torch.float32, device=x.device)
+        return gather_by_dst_from_src(c, y, x, gather_dtype=self.gather_dtype, accumulate=False)
 
     def backward(self, f_output_grad):
-        g = _check_input(f_output_grad, "output_grad")
+        g = _check_input(f_output_grad, "output_grad", pitched=True)
         c = self.partitioned_graph_.graph_chunks[0]
-        dx = torch.zeros((c.batch_size_backward, g.shape[1]), dtype=torch.float32, device=g.device)
-        return gather_by_src_from_dst(c, dx, g, gather_dtype=self.gather_dtype)
+        dx = torch.empty((c.batch_size_backward, g.shape[1]), dtype=torch.float32, device=g.device)
+        return gather_by_src_from_dst(c, dx, g, gather_dtype=self.gather_dtype, accumulate=False)
 
 
 class ForwardGPUfuseOp(ntsGraphOp):

@@ -95,7 +95,10 @@ class GCNImpl:
 
     gather_dtype=torch.bfloat16: every aggregation gathers its operand as BF16 rows with FP32 accumulation (the
     operator's option), and the input features, which the first aggregation reads directly, are stored as bfloat16
-    (half the memory of the largest tensor).  Activations, weights and gradients stay float32."""
+    (half the memory of the largest tensor).  Activations, weights and gradients stay float32.
+
+    With FP32 gathers on the single-GPU op, input features on the GPU whose width is not a multiple of 4 are stored
+    once as a [V, 4*ceil(F/4)] tensor viewed as X[0] = [:, :F] (a copy: the caller's tensor is left as it is)."""
 
     _input_is_gathered = True   # X[0] is the first aggregation's operand (stored as bfloat16 under BF16 gathers)
 
@@ -120,12 +123,21 @@ class GCNImpl:
         self.train_rows = (self.MASK == 0).nonzero().view(-1)
         self.X = [None] * len(self.layers)
         self.gather_dtype = ops._check_gather_dtype(gather_dtype)
-        if self.gather_dtype is not None and self._input_is_gathered:
-            features = features.detach().to(self.gather_dtype)
-        self.X[0] = features.requires_grad_(True)
         if op_class is None:
             op_class = ops.ForwardSingleGPUfuseOp if partitioned_graph.partitions == 1 else ops.ForwardGPUfuseOp
         self.op_class = op_class
+        # the single-GPU op takes row-pitched inputs: X[0] is stored once with its rows padded to 16 bytes, so that
+        # the first aggregation gathers it in place every epoch instead of copying it into padded rows
+        self._pitched_input = (self._input_is_gathered and self.gather_dtype is None and
+                               isinstance(op_class, type) and issubclass(op_class, ops.ForwardSingleGPUfuseOp))
+        if self.gather_dtype is not None and self._input_is_gathered:
+            features = features.detach().to(self.gather_dtype)
+        elif self._pitched_input and features.is_cuda and features.dim() == 2 and features.shape[1] % 4:
+            F = features.shape[1]
+            padded = torch.zeros((features.shape[0], (F + 3) // 4 * 4), dtype=features.dtype, device=features.device)
+            padded[:, :F].copy_(features.detach())
+            features = padded[:, :F]
+        self.X[0] = features.requires_grad_(True)
         self.op_kwargs = dict(op_kwargs or {})
         if self.gather_dtype is not None:
             self.op_kwargs["gather_dtype"] = self.gather_dtype
@@ -148,7 +160,8 @@ class GCNImpl:
                 dropped = torch.nn.functional.dropout(x_i, self.drop_rate, training=True)
                 self.ctx.appendNNOp(x_i, dropped)
                 x_i = dropped
-            x_i = x_i.contiguous()
+            if not (self._pitched_input and ops.row_pitched(x_i)):
+                x_i = x_i.contiguous()
             y_i = self.ctx.runGraphOp(self.op_class, self.pg, None, x_i, **self.op_kwargs)
             self.X[i + 1] = self.ctx.runVertexForward(lambda n, v, _l=i: self.vertexForward(n, v, _l), y_i, x_i)
 
