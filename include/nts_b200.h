@@ -609,6 +609,48 @@ int nts_graph_build_export_degrees(const nts_graph_build *build, nts_vid_t *out_
                                    void *stream);
 int nts_graph_build_destroy(nts_graph_build *build);
 
+/* ---- neighbour sampling for mini-batch training: nts_sampler ---------------------------------------------------------
+ * The blocks of the reference's SampledSubgraph (core/ntsSampler.hpp, core/FullyRepGraph.hpp), built on the GPU from the
+ * CSC of a single-partition graph: column_offset[V+1], row_indices[E] (global source ids, ascending inside a
+ * destination) and edge_weight[E] (nts_norm_degree).  Hop 0's destinations are the seeds; each hop's destinations are
+ * the previous hop's distinct sources.  Destination d keeps min(indeg(d), fanout[h]) of its edge slots (multi-edges
+ * are distinct slots): all of them, or a uniform subset chosen by Floyd's algorithm with the draw
+ * t = (hash(seed, step, h, d, j) * (j + 1)) >> 32 for j = deg-k .. deg-1, where hash is the upper half of a splitmix64
+ * chain (DESIGN.md §3 K8 states it exactly).  Kept slots are written in ascending slot order, so a sample is a pure
+ * function of (graph, seed, step, h, d).  A hop's sources are its distinct source ids ascending; local source ids
+ * index them.  Scratch is allocated once, at create, for max_seeds seeds; 1 <= fanout[h] <= 64, 1 <= hops <= 8.
+ * nts_sampler_sample synchronises `stream` once per hop (to read the hop's edge and source counts) and reports a seed
+ * >= V as an error after hop 0.  Hop views point into the sampler's memory and stay valid until the next sample. */
+typedef struct nts_sampler nts_sampler;
+typedef struct nts_sample_hop_view {
+  nts_vid_t n_dst, n_src;
+  uint64_t n_edges;
+  const nts_vid_t *dst;            /* [n_dst]  global destination ids */
+  const nts_vid_t *column_offset;  /* [n_dst+1] */
+  const nts_vid_t *row_indices;    /* [n_edges] local source ids (into src) */
+  const nts_vid_t *row_global;     /* [n_edges] global source ids */
+  const float *weight;             /* [n_edges] edge_weight at the kept slots, bit for bit */
+  const nts_vid_t *src;            /* [n_src]  distinct global source ids, ascending */
+  const nts_vid_t *row_offset;     /* [n_src+1] transposed block, edges of a source in edge order */
+  const nts_vid_t *column_indices; /* [n_edges] local destination of each transposed edge */
+  const float *weight_backward;    /* [n_edges] */
+} nts_sample_hop_view;
+nts_sampler *nts_sampler_create(const nts_vid_t *column_offset, const nts_vid_t *row_indices, const float *edge_weight,
+                                nts_vid_t n_vertices, uint64_t n_edges, nts_vid_t max_seeds, int hops,
+                                const int *fanout, void *stream);
+int nts_sampler_sample(nts_sampler *sampler, const nts_vid_t *seeds, nts_vid_t n_seeds, uint64_t seed, uint64_t step,
+                       void *stream);
+int nts_sampler_hop_view(const nts_sampler *sampler, int hop, nts_sample_hop_view *view);
+/* peak device bytes the sampler holds (scratch and hop storage) */
+uint64_t nts_sampler_bytes(const nts_sampler *sampler);
+int nts_sampler_destroy(nts_sampler *sampler);
+/* The transposed block of any block whose local sources are in [0, n_src), in any order: row_offset[n_src+1],
+ * column_indices[n_edges] (local destinations) and weight_backward[n_edges], edges of a source in edge order (one
+ * stable radix sort; sources without edges get empty segments).  Temporary memory is stream-ordered. */
+int nts_sample_transpose(const nts_vid_t *column_offset, const nts_vid_t *row_indices, const float *weight,
+                         nts_vid_t n_dst, nts_vid_t n_src, uint64_t n_edges, nts_vid_t *row_offset,
+                         nts_vid_t *column_indices, float *weight_backward, void *stream);
+
 /* ---- feature / label / mask tables (GNNDatum, core/ntsDataloador.hpp) ----------------------------------------------------
  * Text tables exactly as GNNDatum::readFeature_Label_Mask (:156-221) reads them - "id f0 .. fF-1", "id label",
  * "id train|val|eval|test", the k-th label / mask record belongs to the k-th feature record - parsed in parallel;

@@ -210,6 +210,25 @@ SIGNATURES.update({
     "nts_exchange_create_from_plan": (_vp, [_vp, C.POINTER(DeviceChunk)]),
 })
 
+
+class SampleHopView(C.Structure):
+    """nts_sample_hop_view of include/nts_b200.h (device arrays of one sampled hop)."""
+    _fields_ = [
+        ("n_dst", _u32), ("n_src", _u32), ("n_edges", _u64),
+        ("dst", _vp), ("column_offset", _vp), ("row_indices", _vp), ("row_global", _vp), ("weight", _vp),
+        ("src", _vp), ("row_offset", _vp), ("column_indices", _vp), ("weight_backward", _vp),
+    ]
+
+
+SIGNATURES.update({
+    "nts_sampler_create": (_vp, [_vp, _vp, _vp, _u32, _u64, _u32, _int, C.POINTER(_int), _vp]),
+    "nts_sampler_sample": (_int, [_vp, _vp, _u32, _u64, _u64, _vp]),
+    "nts_sampler_hop_view": (_int, [_vp, _int, C.POINTER(SampleHopView)]),
+    "nts_sampler_bytes": (_u64, [_vp]),
+    "nts_sampler_destroy": (_int, [_vp]),
+    "nts_sample_transpose": (_int, [_vp, _vp, _vp, _u32, _u32, _u64, _vp, _vp, _vp, _vp]),
+})
+
 _lib = None
 
 

@@ -1,0 +1,442 @@
+// K8: neighbour sampling for mini-batch training (nts_sampler) - the blocks of the reference's SampledSubgraph
+// (core/ntsSampler.hpp, core/FullyRepGraph.hpp) built on the GPU, deterministically.
+//
+// Per hop, with n_dst destinations and fanout k:
+//   count    one thread per destination: min(indeg, k); a CUB exclusive scan gives the block's column_offset
+//   select   one warp per destination: every slot when indeg <= k, else Floyd's k-subset of the slots drawn from a
+//            counter hash of (seed, step, hop, global dst, j), written in ascending slot order; every kept edge's global
+//            source id and weight go to the block, and (source id, edge position) to a padded n_dst * k pair array
+//            whose unused pairs carry the key V
+//   sort     one stable CUB radix sort of the pairs by source id
+//   finish   head flags + an inclusive scan number the distinct sources in ascending id order: the next hop's
+//            destinations, each edge's local source id, and the transposed block (the sorted order is the transposed
+//            edge order, stable by edge position), in one pass
+// then one 12-byte device-to-host copy (edge count, source count, bad-seed flag) sizes the next hop.  No atomics on
+// floats anywhere; the only atomic is the bad-seed flag.
+#include <cub/cub.cuh>
+
+#include <vector>
+
+#include "nts_common.cuh"
+
+namespace {
+
+using u32 = uint32_t;
+using u64 = uint64_t;
+
+constexpr int kMaxFanout = 64;
+constexpr int kMaxHops = 8;
+constexpr int kSelectWarps = 8;
+constexpr int kThreads = 256;
+
+__host__ __device__ __forceinline__ u64 splitmix64(u64 z) {
+  z += 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+__global__ void count_kernel(const u32 *__restrict__ dst, u32 n_dst, const u32 *__restrict__ g_col, u32 V, u32 k,
+                             u32 *__restrict__ cnt, u32 *__restrict__ bad) {
+  const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i > n_dst) return;
+  u32 c = 0;
+  if (i < n_dst) {
+    const u32 v = dst[i];
+    if (v < V) {
+      c = min(g_col[v + 1] - g_col[v], k);
+    } else {
+      atomicOr(bad, 1u);
+    }
+  }
+  cnt[i] = c;   // cnt[n_dst] = 0: the exclusive scan's last element is the edge count
+}
+
+__global__ void __launch_bounds__(kSelectWarps * 32)
+select_kernel(const u32 *__restrict__ dst, u32 n_dst, const u32 *__restrict__ g_col, const u32 *__restrict__ g_row,
+              const float *__restrict__ g_w, u32 V, u32 k, u64 step_key, u32 hop, const u32 *__restrict__ col,
+              u32 *__restrict__ row_global, float *__restrict__ weight, u32 *__restrict__ edge_dst,
+              u32 *__restrict__ keys, u32 *__restrict__ vals) {
+  __shared__ u32 chosen[kSelectWarps][kMaxFanout];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const u32 d = blockIdx.x * kSelectWarps + warp;
+  if (d >= n_dst) return;   // warp-uniform
+  const u32 v = dst[d];
+  u32 base = 0, deg = 0;
+  if (v < V) {
+    base = g_col[v];
+    deg = g_col[v + 1] - base;
+  }
+  const u32 e0 = col[d];
+  const u64 p0 = (u64)d * k;
+  auto emit = [&](u32 i, u32 slot) {
+    const u32 e = e0 + i;
+    const u32 s = g_row[base + slot];
+    row_global[e] = s;
+    weight[e] = g_w[base + slot];
+    edge_dst[e] = d;
+    keys[p0 + i] = s;
+    vals[p0 + i] = e;
+  };
+  const u32 kept = min(deg, k);
+  if (deg <= k) {
+    for (u32 i = lane; i < deg; i += 32) emit(i, i);
+  } else {
+    // Floyd: for j = deg-k .. deg-1, t = draw(j+1); add j if t is already chosen, else t.  Every lane computes the
+    // same draw; the membership test is spread over the lanes.
+    u32 *S = chosen[warp];
+    const u64 dst_key = splitmix64(step_key ^ (((u64)hop << 32) | v));
+    for (u32 i = 0; i < k; ++i) {
+      const u32 j = deg - k + i;
+      const u32 h = (u32)(splitmix64(dst_key ^ (u64)j) >> 32);
+      const u32 t = (u32)(((u64)h * (u64)(j + 1)) >> 32);
+      bool hit = false;
+      for (u32 q = lane; q < i; q += 32) hit |= S[q] == t;
+      hit = __any_sync(0xffffffffu, hit);
+      if (lane == 0) S[i] = hit ? j : t;
+      __syncwarp();
+    }
+    // ascending slot order: the chosen slots are distinct, so a slot's rank is the number of smaller ones
+    for (u32 a = lane; a < k; a += 32) {
+      const u32 x = S[a];
+      u32 r = 0;
+      for (u32 b = 0; b < k; ++b) r += S[b] < x;
+      emit(r, x);
+    }
+  }
+  for (u32 i = kept + lane; i < k; i += 32) keys[p0 + i] = V;   // unused pairs sort past every source id
+}
+
+__global__ void head_kernel(const u32 *__restrict__ skeys, u64 n_pad, const u32 *__restrict__ col, u32 n_dst,
+                            u32 *__restrict__ flag) {
+  const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_pad) return;
+  flag[i] = i < col[n_dst] && (i == 0 || skeys[i] != skeys[i - 1]);
+}
+
+__global__ void finish_kernel(const u32 *__restrict__ skeys, const u32 *__restrict__ svals,
+                              const u32 *__restrict__ pos, u64 n_pad, const u32 *__restrict__ col, u32 n_dst,
+                              const u32 *__restrict__ edge_dst, const float *__restrict__ weight,
+                              u32 *__restrict__ row_local, u32 *__restrict__ src, u32 *__restrict__ row_offset,
+                              u32 *__restrict__ col_t, float *__restrict__ w_t, u32 *__restrict__ counts) {
+  const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  const u32 n_edges = col[n_dst];
+  if (i == 0 && n_edges == 0) {
+    row_offset[0] = 0;
+    counts[0] = 0;
+    counts[1] = 0;
+  }
+  if (i >= n_edges || i >= n_pad) return;
+  const u32 l = pos[i] - 1, e = svals[i];
+  row_local[e] = l;
+  col_t[i] = edge_dst[e];
+  w_t[i] = weight[e];
+  if (i == 0 || skeys[i] != skeys[i - 1]) {
+    src[l] = skeys[i];
+    row_offset[l] = (u32)i;
+  }
+  if (i + 1 == n_edges) {
+    row_offset[l + 1] = n_edges;
+    counts[0] = n_edges;
+    counts[1] = l + 1;
+  }
+}
+
+// nts_sample_transpose: the destination of every edge, and lower bounds of each source in the sorted keys
+__global__ void edge_dst_kernel(const u32 *__restrict__ col, u32 n_dst, u32 *__restrict__ edge_dst,
+                                u32 *__restrict__ iota) {
+  const u32 d = blockIdx.x * (blockDim.x / 32) + (threadIdx.x >> 5);
+  if (d >= n_dst) return;
+  for (u32 e = col[d] + (threadIdx.x & 31); e < col[d + 1]; e += 32) {
+    edge_dst[e] = d;
+    iota[e] = e;
+  }
+}
+
+__global__ void lower_bound_kernel(const u32 *__restrict__ skeys, u64 n, u32 n_src, u32 *__restrict__ row_offset) {
+  const u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s > n_src) return;
+  u64 lo = 0, hi = n;
+  while (lo < hi) {
+    const u64 mid = (lo + hi) >> 1;
+    if (skeys[mid] < s) lo = mid + 1; else hi = mid;
+  }
+  row_offset[s] = (u32)lo;
+}
+
+__global__ void permute_kernel(const u32 *__restrict__ svals, u64 n, const u32 *__restrict__ edge_dst,
+                               const float *__restrict__ weight, u32 *__restrict__ col_t, float *__restrict__ w_t) {
+  const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const u32 e = svals[i];
+  col_t[i] = edge_dst[e];
+  w_t[i] = weight[e];
+}
+
+inline unsigned blocks_for(u64 n, int threads = kThreads) { return (unsigned)((n + threads - 1) / threads); }
+
+inline int bits_for(u32 v) {
+  int b = 1;
+  while (b < 32 && (v >> b) != 0) ++b;
+  return b;
+}
+
+} // namespace
+
+struct nts_sampler {
+  const u32 *g_col = nullptr, *g_row = nullptr;
+  const float *g_w = nullptr;
+  u32 V = 0;
+  u32 max_seeds = 0;
+  int hops = 0;
+  u32 fanout[kMaxHops] = {};
+  u64 cap_dst[kMaxHops] = {}, cap_pad[kMaxHops] = {}, cap_src[kMaxHops] = {};
+  struct Hop {
+    u32 *dst = nullptr, *col = nullptr, *row_local = nullptr, *row_global = nullptr, *edge_dst = nullptr;
+    float *weight = nullptr, *w_t = nullptr;
+    u32 *src = nullptr, *row_offset = nullptr, *col_t = nullptr;
+    u32 n_dst = 0, n_src = 0;
+    u64 n_edges = 0;
+  } hop[kMaxHops];
+  bool sampled = false;
+  // scratch shared by the hops
+  u32 *cnt = nullptr, *keys = nullptr, *keys_alt = nullptr, *vals = nullptr, *vals_alt = nullptr, *flag = nullptr,
+      *pos = nullptr, *counts = nullptr;
+  void *tmp = nullptr;
+  size_t tmp_bytes = 0;
+  u32 *counts_host = nullptr;
+  std::vector<void *> allocs;
+  u64 bytes = 0;
+
+  template <class T> int alloc(T **p, u64 n) {
+    const size_t b = (size_t)std::max<u64>(n, 1) * sizeof(T);
+    NTS_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(p), b));
+    allocs.push_back(*p);
+    bytes += b;
+    return 0;
+  }
+  ~nts_sampler() {
+    for (void *p : allocs) cudaFree(p);
+    if (counts_host) cudaFreeHost(counts_host);
+  }
+};
+
+namespace {
+
+int sampler_setup(nts_sampler *s, cudaStream_t st) {
+  u64 max_dst = 0, max_pad = 0;
+  for (int h = 0; h < s->hops; ++h) {
+    s->cap_dst[h] = h == 0 ? s->max_seeds : s->cap_src[h - 1];
+    s->cap_pad[h] = s->cap_dst[h] * s->fanout[h];
+    s->cap_src[h] = std::min<u64>(s->V, s->cap_pad[h]);
+    NTS_ARG_CHECK(s->cap_pad[h] < (1ull << 31), "sampler worst case n_dst * fanout reaches 2^31 edges in one hop");
+    max_dst = std::max(max_dst, s->cap_dst[h]);
+    max_pad = std::max(max_pad, s->cap_pad[h]);
+  }
+  for (int h = 0; h < s->hops; ++h) {
+    nts_sampler::Hop &H = s->hop[h];
+    if (h == 0) {
+      if (int rc = s->alloc(&H.dst, s->cap_dst[0])) return rc;
+    } else {
+      H.dst = s->hop[h - 1].src;
+    }
+    const u64 E = s->cap_pad[h], S = s->cap_src[h];
+    int rc = 0;
+    if ((rc = s->alloc(&H.col, s->cap_dst[h] + 1)) || (rc = s->alloc(&H.row_local, E)) ||
+        (rc = s->alloc(&H.row_global, E)) || (rc = s->alloc(&H.edge_dst, E)) || (rc = s->alloc(&H.weight, E)) ||
+        (rc = s->alloc(&H.w_t, E)) || (rc = s->alloc(&H.col_t, E)) || (rc = s->alloc(&H.src, S)) ||
+        (rc = s->alloc(&H.row_offset, S + 1)))
+      return rc;
+  }
+  int rc = 0;
+  if ((rc = s->alloc(&s->cnt, max_dst + 1)) || (rc = s->alloc(&s->keys, max_pad)) ||
+      (rc = s->alloc(&s->keys_alt, max_pad)) || (rc = s->alloc(&s->vals, max_pad)) ||
+      (rc = s->alloc(&s->vals_alt, max_pad)) || (rc = s->alloc(&s->flag, max_pad)) ||
+      (rc = s->alloc(&s->pos, max_pad)) || (rc = s->alloc(&s->counts, 4)))
+    return rc;
+  // CUB scratch for the largest scan and sort (queried again, and checked, at every call)
+  size_t b0 = 0, b1 = 0, b2 = 0;
+  cub::DoubleBuffer<u32> kd(s->keys, s->keys_alt), vd(s->vals, s->vals_alt);
+  NTS_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, b0, s->cnt, s->cnt, (int64_t)(max_dst + 1), st));
+  NTS_CUDA_OK(cub::DeviceScan::InclusiveSum(nullptr, b1, s->flag, s->pos, (int64_t)std::max<u64>(max_pad, 1), st));
+  NTS_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, b2, kd, vd, (int64_t)std::max<u64>(max_pad, 1), 0, 32, st));
+  s->tmp_bytes = std::max(b0, std::max(b1, b2));
+  if ((rc = s->alloc(reinterpret_cast<char **>(&s->tmp), s->tmp_bytes))) return rc;
+  NTS_CUDA_OK(cudaMallocHost(reinterpret_cast<void **>(&s->counts_host), 4 * sizeof(u32)));
+  return 0;
+}
+
+int check_tmp(const nts_sampler *s, size_t need) {
+  NTS_ARG_CHECK(need <= s->tmp_bytes, "sampler CUB scratch smaller than a call needs");
+  return 0;
+}
+
+int sample_hop(nts_sampler *s, int h, u64 step_key, cudaStream_t st) {
+  nts_sampler::Hop &H = s->hop[h];
+  const u32 n_dst = H.n_dst, k = s->fanout[h];
+  const u64 n_pad = (u64)n_dst * k;
+  count_kernel<<<blocks_for((u64)n_dst + 1), kThreads, 0, st>>>(H.dst, n_dst, s->g_col, s->V, k, s->cnt,
+                                                                  s->counts + 2);
+  NTS_LAUNCH_CHECK();
+  size_t need = 0;
+  NTS_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, need, s->cnt, H.col, (int64_t)n_dst + 1, st));
+  if (int rc = check_tmp(s, need)) return rc;
+  NTS_CUDA_OK(cub::DeviceScan::ExclusiveSum(s->tmp, need, s->cnt, H.col, (int64_t)n_dst + 1, st));
+  const u32 *skeys = s->keys, *svals = s->vals;
+  if (n_dst > 0) {
+    select_kernel<<<(n_dst + kSelectWarps - 1) / kSelectWarps, kSelectWarps * 32, 0, st>>>(
+        H.dst, n_dst, s->g_col, s->g_row, s->g_w, s->V, k, step_key, (u32)h, H.col, H.row_global, H.weight,
+        H.edge_dst, s->keys, s->vals);
+    NTS_LAUNCH_CHECK();
+    cub::DoubleBuffer<u32> kd(s->keys, s->keys_alt), vd(s->vals, s->vals_alt);
+    const int end_bit = bits_for(s->V);
+    NTS_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, need, kd, vd, (int64_t)n_pad, 0, end_bit, st));
+    if (int rc = check_tmp(s, need)) return rc;
+    NTS_CUDA_OK(cub::DeviceRadixSort::SortPairs(s->tmp, need, kd, vd, (int64_t)n_pad, 0, end_bit, st));
+    skeys = kd.Current();
+    svals = vd.Current();
+    head_kernel<<<blocks_for(n_pad), kThreads, 0, st>>>(skeys, n_pad, H.col, n_dst, s->flag);
+    NTS_LAUNCH_CHECK();
+    NTS_CUDA_OK(cub::DeviceScan::InclusiveSum(nullptr, need, s->flag, s->pos, (int64_t)n_pad, st));
+    if (int rc = check_tmp(s, need)) return rc;
+    NTS_CUDA_OK(cub::DeviceScan::InclusiveSum(s->tmp, need, s->flag, s->pos, (int64_t)n_pad, st));
+  }
+  finish_kernel<<<blocks_for(std::max<u64>(n_pad, 1)), kThreads, 0, st>>>(
+      skeys, svals, s->pos, n_pad, H.col, n_dst, H.edge_dst, H.weight, H.row_local, H.src, H.row_offset, H.col_t,
+      H.w_t, s->counts);
+  NTS_LAUNCH_CHECK();
+  NTS_CUDA_OK(cudaMemcpyAsync(s->counts_host, s->counts, 3 * sizeof(u32), cudaMemcpyDeviceToHost, st));
+  NTS_CUDA_OK(cudaStreamSynchronize(st));
+  NTS_ARG_CHECK(s->counts_host[2] == 0, "a seed vertex id is >= the graph's vertex count");
+  H.n_edges = s->counts_host[0];
+  H.n_src = s->counts_host[1];
+  return 0;
+}
+
+} // namespace
+
+extern "C" {
+
+nts_sampler *nts_sampler_create(const nts_vid_t *column_offset, const nts_vid_t *row_indices, const float *edge_weight,
+                                nts_vid_t n_vertices, uint64_t n_edges, nts_vid_t max_seeds, int hops,
+                                const int *fanout, void *stream) {
+  auto bad = [](const char *msg) -> nts_sampler * {
+    nts::fail(-1, msg, __FILE__, __LINE__);
+    return nullptr;
+  };
+  if (hops < 1 || hops > kMaxHops) return bad("sampler hops must be in 1..8");
+  if (!fanout) return bad("sampler fanout is null");
+  for (int h = 0; h < hops; ++h)
+    if (fanout[h] < 1 || fanout[h] > kMaxFanout) return bad("sampler fanout must be in 1..64");
+  if (n_vertices == 0 || n_vertices >= (1u << 31)) return bad("sampler needs 1 <= V < 2^31");
+  if (n_edges >= (1ull << 32)) return bad("sampler needs fewer than 2^32 edges");
+  if (!column_offset || (n_edges && (!row_indices || !edge_weight))) return bad("null graph array passed to sampler");
+  nts_sampler *s = new nts_sampler;
+  s->g_col = column_offset;
+  s->g_row = row_indices;
+  s->g_w = edge_weight;
+  s->V = n_vertices;
+  s->max_seeds = max_seeds;
+  s->hops = hops;
+  for (int h = 0; h < hops; ++h) s->fanout[h] = (u32)fanout[h];
+  if (sampler_setup(s, nts::as_stream(stream)) != 0) {
+    delete s;
+    return nullptr;
+  }
+  return s;
+}
+
+int nts_sampler_sample(nts_sampler *s, const nts_vid_t *seeds, nts_vid_t n_seeds, uint64_t seed, uint64_t step,
+                       void *stream) {
+  NTS_ARG_CHECK(s != nullptr, "sampler is null");
+  NTS_ARG_CHECK(n_seeds <= s->max_seeds, "more seeds than the sampler was created for");
+  NTS_ARG_CHECK(n_seeds == 0 || seeds != nullptr, "seeds is null");
+  cudaStream_t st = nts::as_stream(stream);
+  s->sampled = false;
+  NTS_CUDA_OK(cudaMemsetAsync(s->counts, 0, 4 * sizeof(u32), st));
+  if (n_seeds) NTS_CUDA_OK(cudaMemcpyAsync(s->hop[0].dst, seeds, n_seeds * sizeof(u32), cudaMemcpyDeviceToDevice, st));
+  const u64 step_key = splitmix64(splitmix64(seed) ^ step);
+  for (int h = 0; h < s->hops; ++h) {
+    s->hop[h].n_dst = h == 0 ? n_seeds : s->hop[h - 1].n_src;
+    if (int rc = sample_hop(s, h, step_key, st)) return rc;
+  }
+  s->sampled = true;
+  return 0;
+}
+
+int nts_sampler_hop_view(const nts_sampler *s, int hop, nts_sample_hop_view *v) {
+  NTS_ARG_CHECK(s != nullptr && v != nullptr, "null sampler or view");
+  NTS_ARG_CHECK(hop >= 0 && hop < s->hops, "hop out of range");
+  NTS_ARG_CHECK(s->sampled, "the sampler holds no complete sample");
+  const nts_sampler::Hop &H = s->hop[hop];
+  v->n_dst = H.n_dst;
+  v->n_src = H.n_src;
+  v->n_edges = H.n_edges;
+  v->dst = H.dst;
+  v->column_offset = H.col;
+  v->row_indices = H.row_local;
+  v->row_global = H.row_global;
+  v->weight = H.weight;
+  v->src = H.src;
+  v->row_offset = H.row_offset;
+  v->column_indices = H.col_t;
+  v->weight_backward = H.w_t;
+  return 0;
+}
+
+uint64_t nts_sampler_bytes(const nts_sampler *s) { return s ? s->bytes : 0; }
+
+int nts_sampler_destroy(nts_sampler *s) {
+  delete s;
+  return 0;
+}
+
+int nts_sample_transpose(const nts_vid_t *column_offset, const nts_vid_t *row_indices, const float *weight,
+                         nts_vid_t n_dst, nts_vid_t n_src, uint64_t n_edges, nts_vid_t *row_offset,
+                         nts_vid_t *column_indices, float *weight_backward, void *stream) {
+  NTS_ARG_CHECK(n_edges < (1ull << 31), "transpose needs fewer than 2^31 edges");
+  NTS_ARG_CHECK(row_offset != nullptr, "row_offset is null");
+  NTS_ARG_CHECK(n_edges == 0 || (column_offset && row_indices && weight && column_indices && weight_backward),
+                "null block array passed to nts_sample_transpose");
+  cudaStream_t st = nts::as_stream(stream);
+  if (n_edges == 0) {
+    NTS_CUDA_OK(cudaMemsetAsync(row_offset, 0, ((size_t)n_src + 1) * sizeof(u32), st));
+    return 0;
+  }
+  // edge_dst, iota, sorted keys, sorted values, CUB scratch: stream-ordered temporaries
+  size_t sort_bytes = 0;
+  cub::DoubleBuffer<u32> kd(nullptr, nullptr), vd(nullptr, nullptr);
+  const int end_bit = bits_for(n_src);
+  NTS_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, kd, vd, (int64_t)n_edges, 0, end_bit, st));
+  const size_t E4 = ((n_edges * sizeof(u32) + 255) / 256) * 256;
+  char *t = nullptr;
+  NTS_CUDA_OK(cudaMallocAsync(reinterpret_cast<void **>(&t), 5 * E4 + sort_bytes, st));
+  u32 *edge_dst = reinterpret_cast<u32 *>(t), *iota = reinterpret_cast<u32 *>(t + E4),
+      *kalt = reinterpret_cast<u32 *>(t + 2 * E4), *valt = reinterpret_cast<u32 *>(t + 3 * E4),
+      *kin = reinterpret_cast<u32 *>(t + 4 * E4);
+  int rc = 0;
+  do {
+    if (n_dst) {
+      edge_dst_kernel<<<(n_dst + 7) / 8, 256, 0, st>>>(column_offset, n_dst, edge_dst, iota);
+      ::nts::count_launch();
+      if (cudaGetLastError() != cudaSuccess) { rc = nts::fail(-1, "edge_dst_kernel launch failed", __FILE__, __LINE__); break; }
+    }
+    cudaError_t e = cudaMemcpyAsync(kin, row_indices, n_edges * sizeof(u32), cudaMemcpyDeviceToDevice, st);
+    if (e != cudaSuccess) { rc = nts::fail((int)e, cudaGetErrorString(e), __FILE__, __LINE__); break; }
+    cub::DoubleBuffer<u32> k2(kin, kalt), v2(iota, valt);
+    e = cub::DeviceRadixSort::SortPairs(t + 5 * E4, sort_bytes, k2, v2, (int64_t)n_edges, 0, end_bit, st);
+    if (e != cudaSuccess) { rc = nts::fail((int)e, cudaGetErrorString(e), __FILE__, __LINE__); break; }
+    lower_bound_kernel<<<blocks_for((u64)n_src + 1), kThreads, 0, st>>>(k2.Current(), n_edges, n_src, row_offset);
+    ::nts::count_launch();
+    permute_kernel<<<blocks_for(n_edges), kThreads, 0, st>>>(v2.Current(), n_edges, edge_dst, weight, column_indices,
+                                                              weight_backward);
+    ::nts::count_launch();
+    e = cudaGetLastError();
+    if (e != cudaSuccess) { rc = nts::fail((int)e, cudaGetErrorString(e), __FILE__, __LINE__); break; }
+  } while (0);
+  cudaError_t e = cudaFreeAsync(t, st);
+  if (rc == 0 && e != cudaSuccess) rc = nts::fail((int)e, cudaGetErrorString(e), __FILE__, __LINE__);
+  return rc;
+}
+
+} // extern "C"

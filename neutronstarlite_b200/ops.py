@@ -360,6 +360,50 @@ class ForwardSingleGPUfuseOp(ntsGraphOp):
         return gather_by_src_from_dst(c, dx, g, gather_dtype=self.gather_dtype, accumulate=False)
 
 
+class MiniBatchFuseOp(ntsGraphOp):
+    """core/ntsMiniBatchGraphOp.hpp:61-131 on one block of a sample (sample.SampledSubgraph): forward
+    Y[n_dst, F] = sum_e w_e X[src_local(e)], backward dX[n_src, F] over the transposed block, both through K1
+    (nts_segment_gather_sum) on the block's own arrays - a block changes every step, so nothing is planned.
+
+    table=True: X is the whole [V, F] feature table and the forward gathers by the block's global source ids
+    (row_global), so the table rows of the block's sources are never copied out first; the table must have at least
+    the graph's V rows (sampled_subgraph.vertices).  Such an op has no backward: it is the first graph op of the
+    model, which the tape never back-propagates."""
+
+    def __init__(self, sampled_subgraph, hop, table=False):
+        super().__init__(sampled_subgraph, None)
+        self.block = sampled_subgraph.blocks[hop]
+        self.hop, self.table = int(hop), bool(table)
+        self.vertices = getattr(sampled_subgraph, "vertices", None)
+        if self.table and (self.block.row_global is None or self.vertices is None):
+            raise _lib.NtsError("table=True needs the block's global source ids (row_global) and the graph's vertex "
+                                "count (SampledSubgraph.vertices)")
+
+    def forward(self, f_input, f_input1=None):
+        x = _check_input(f_input, "input")
+        b = self.block
+        if self.table and x.shape[0] < self.vertices:
+            raise _lib.NtsError("the feature table has %d rows, the sampled graph has %d vertices"
+                                % (x.shape[0], self.vertices))
+        if not self.table and x.shape[0] != b.n_src:
+            raise _lib.NtsError("input has %d rows, hop %d has %d sources" % (x.shape[0], self.hop, b.n_src))
+        y = torch.zeros((b.n_dst, x.shape[1]), dtype=torch.float32, device=x.device)
+        with _timed("minibatch_fwd", x.shape[1], b.n_edges, b.n_dst):
+            return segment_gather_sum(y, x, b.weight, b.row_global if self.table else b.row_indices,
+                                      b.column_offset, 0, b.n_dst, b.n_edges)
+
+    def backward(self, f_output_grad):
+        if self.table:
+            raise _lib.NtsError("a table gather (table=True) has no backward")
+        g = _check_input(f_output_grad, "output_grad")
+        b = self.block
+        if g.shape[0] != b.n_dst:
+            raise _lib.NtsError("output_grad has %d rows, hop %d has %d destinations" % (g.shape[0], self.hop, b.n_dst))
+        dx = torch.zeros((b.n_src, g.shape[1]), dtype=torch.float32, device=g.device)
+        with _timed("minibatch_bwd", g.shape[1], b.n_edges, b.n_src):
+            return segment_gather_sum(dx, g, b.weight_backward, b.column_indices, b.row_offset, 0, b.n_src, b.n_edges)
+
+
 class ForwardGPUfuseOp(ntsGraphOp):
     """core/ntsDistGPUFusedGraphOp.hpp:48-90: the distributed fused GCN aggregation.  The reference drives it
     through Graph::sync_compute_decoupled / compute_sync_decoupled with host-staged MPI messages

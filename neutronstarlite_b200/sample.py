@@ -1,0 +1,203 @@
+"""Neighbour sampling for mini-batch training: the reference's `Sampler` / `SampledSubgraph` (core/ntsSampler.hpp,
+core/FullyRepGraph.hpp) on the GPU (K8, `nts_sampler` of include/nts_b200.h).
+
+`NeighborSampler(pg, fanout, max_seeds)` samples the single-partition graph `pg` hop by hop from a list of seed
+vertices: hop 0's destinations are the seeds, hop h keeps min(indeg, fanout[h]) edge slots of every destination (a
+uniform subset by Floyd's algorithm on a counter hash of (seed, step, hop, destination, j)), and hop h+1's
+destinations are hop h's distinct sources, ascending by global id.  A sample is a pure function of (graph, seed, step)
+and the seeds: it does not depend on launch configuration, batch composition or the position of a vertex in the batch.
+
+`SampledSubgraph` holds the blocks of one sample as `SampledBlock`s (device tensors); `ops.MiniBatchFuseOp`
+aggregates over them."""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+import torch
+
+from . import _lib
+
+MAX_FANOUT = 64
+MAX_HOPS = 8
+
+
+def _stream():
+    return torch.cuda.current_stream().cuda_stream
+
+
+class _DeviceArray:
+    """A borrowed 1-D device array for torch.as_tensor (the CUDA array interface; no copy, no stream sync)."""
+
+    def __init__(self, ptr, n, typestr):
+        self.__cuda_array_interface__ = {"shape": (int(n),), "typestr": typestr, "data": (int(ptr), False),
+                                         "version": 2, "strides": None}
+
+
+class SampledBlock:
+    """One hop of a sample (the reference's sampled_sgs[hop]).
+
+    dst [n_dst] global destination ids; column_offset [n_dst+1]; row_indices [n_edges] local source ids (into src);
+    weight [n_edges]; src [n_src] global source ids; row_offset [n_src+1], column_indices [n_edges] (local destinations)
+    and weight_backward [n_edges]: the transposed block.  row_global [n_edges] (global source ids) may be None.
+    Index arrays are int32 tensors holding uint32 values."""
+
+    def __init__(self, dst, column_offset, row_indices, weight, src, row_offset=None, column_indices=None,
+                 weight_backward=None, row_global=None):
+        self.dst, self.column_offset, self.row_indices, self.weight = dst, column_offset, row_indices, weight
+        self.src, self.row_global = src, row_global
+        self.n_dst, self.n_src, self.n_edges = int(dst.numel()), int(src.numel()), int(row_indices.numel())
+        if row_offset is None:
+            row_offset, column_indices, weight_backward = transpose(column_offset, row_indices, weight, self.n_dst,
+                                                                    self.n_src)
+        self.row_offset, self.column_indices, self.weight_backward = row_offset, column_indices, weight_backward
+
+    def to_numpy(self):
+        """Host copies of every array (uint32 index arrays, float32 weights)."""
+        out = {}
+        for name in ("dst", "column_offset", "row_indices", "row_global", "weight", "src", "row_offset",
+                     "column_indices", "weight_backward"):
+            t = getattr(self, name)
+            if t is not None:
+                a = t.cpu().numpy()
+                out[name] = a.view(np.uint32) if a.dtype == np.int32 else a
+        return out
+
+    def clone(self):
+        c = object.__new__(SampledBlock)
+        c.__dict__.update({k: (v.clone() if torch.is_tensor(v) else v) for k, v in self.__dict__.items()})
+        return c
+
+
+class SampledSubgraph:
+    """The blocks of one sample, hop 0 (the seeds' block) first.  `blocks[-1]` is the deepest hop: its row_global
+    lets the first layer gather straight from the whole feature table (MiniBatchFuseOp(..., table=True))."""
+
+    def __init__(self, blocks, owner=None, vertices=None):
+        self.blocks = list(blocks)
+        self.vertices = None if vertices is None else int(vertices)   # V of the sampled graph (table gathers)
+        self._owner = owner           # keeps a sampler's memory alive while its views are in use
+
+    @property
+    def hops(self):
+        return len(self.blocks)
+
+    def seeds(self):
+        return self.blocks[0].dst
+
+    def clone(self):
+        """A copy that the next sample of the same sampler does not overwrite."""
+        return SampledSubgraph([b.clone() for b in self.blocks], vertices=self.vertices)
+
+    @staticmethod
+    def from_blocks(blocks, vertices=None):
+        """From dicts of device tensors with keys dst, column_offset, row_indices (local), weight, src (sources in any
+        order) and optionally row_global; the transposed blocks are built on the device (nts_sample_transpose).
+        `vertices` (the graph's V) is needed for table gathers."""
+        return SampledSubgraph([SampledBlock(b["dst"], b["column_offset"], b["row_indices"], b["weight"], b["src"],
+                                             row_global=b.get("row_global")) for b in blocks], vertices=vertices)
+
+
+def transpose(column_offset, row_indices, weight, n_dst, n_src):
+    """(row_offset [n_src+1], column_indices, weight_backward) of a block with local sources in [0, n_src)."""
+    dev = row_indices.device
+    n_edges = int(row_indices.numel())
+    row_offset = torch.empty(n_src + 1, dtype=torch.int32, device=dev)
+    column_indices = torch.empty(n_edges, dtype=torch.int32, device=dev)
+    weight_backward = torch.empty(n_edges, dtype=torch.float32, device=dev)
+    for t in (column_offset, row_indices, weight):
+        if not t.is_cuda or not t.is_contiguous():
+            raise _lib.NtsError("block arrays must be contiguous CUDA tensors")
+    _lib.call("nts_sample_transpose", column_offset.data_ptr(), row_indices.data_ptr(), weight.data_ptr(),
+              int(n_dst), int(n_src), n_edges, row_offset.data_ptr(), column_indices.data_ptr(),
+              weight_backward.data_ptr(), _stream())
+    return row_offset, column_indices, weight_backward
+
+
+def check_fanout(fanout):
+    fanout = [int(k) for k in fanout]
+    if not 1 <= len(fanout) <= MAX_HOPS:
+        raise _lib.NtsError("fanout needs 1..%d hops, got %d" % (MAX_HOPS, len(fanout)))
+    for k in fanout:
+        if not 1 <= k <= MAX_FANOUT:
+            raise _lib.NtsError("fanout %d is outside 1..%d" % (k, MAX_FANOUT))
+    return fanout
+
+
+class NeighborSampler:
+    """K8 on the CSC of a single-partition graph (chunk 0's column_offset_gpu / row_indices_gpu /
+    edge_weight_forward_gpu).  Device scratch for max_seeds seeds is allocated once, here.  `sample()` synchronises
+    the stream once per hop; the blocks it returns are views that the next `sample()` overwrites (clone() them to keep
+    them)."""
+
+    def __init__(self, partitioned_graph, fanout, max_seeds):
+        pg = partitioned_graph
+        if pg.partitions != 1:
+            raise _lib.NtsError("NeighborSampler needs a single-partition graph (partitions == 1), got %d"
+                                % pg.partitions)
+        self.fanout = check_fanout(fanout)
+        c = pg.graph_chunks[0]
+        if c.column_offset_gpu is None:
+            raise _lib.NtsError("the graph has no device arrays (generate_all(device=...))")
+        self.V = int(pg.global_vertices)
+        self.max_seeds = int(max_seeds)
+        self.device = c.column_offset_gpu.device
+        self._graph = (c.column_offset_gpu, c.row_indices_gpu, c.edge_weight_forward_gpu)
+        L = _lib.load()
+        ks = (C.c_int * len(self.fanout))(*self.fanout)
+        self.handle = L.nts_sampler_create(c.column_offset_gpu.data_ptr(), c.row_indices_gpu.data_ptr(),
+                                           c.edge_weight_forward_gpu.data_ptr(), self.V, int(c.edge_size),
+                                           self.max_seeds, len(self.fanout), ks, _stream())
+        if not self.handle:
+            raise _lib.NtsError("nts_sampler_create failed: " + L.nts_last_error().decode(errors="replace"))
+
+    def bytes(self):
+        return int(_lib.load().nts_sampler_bytes(self.handle))
+
+    def _seeds(self, seeds):
+        """Seeds as a contiguous int32 device tensor; ids are checked against V before any device work when they
+        are given on the host (numpy, list, CPU tensor)."""
+        if torch.is_tensor(seeds) and seeds.is_cuda:
+            if seeds.dtype.is_floating_point or seeds.dtype.is_complex or seeds.dtype == torch.bool:
+                raise _lib.NtsError("seeds must be an integer tensor, not %s" % seeds.dtype)
+            # range check in the caller's dtype: a cast first could wrap an int64 id >= 2^32 into [0, V)
+            if seeds.numel() and (int(seeds.min()) < 0 or int(seeds.max()) >= self.V):
+                raise _lib.NtsError("seed vertex ids must be in [0, %d)" % self.V)
+            t = seeds.reshape(-1).to(torch.int32).contiguous()
+        else:
+            a = np.asarray(seeds.numpy() if torch.is_tensor(seeds) else seeds).reshape(-1).astype(np.int64)
+            if a.size and (a.min() < 0 or a.max() >= self.V):
+                raise _lib.NtsError("seed vertex ids must be in [0, %d)" % self.V)
+            t = torch.from_numpy(a.astype(np.int32)).to(self.device)
+        if t.numel() > self.max_seeds:
+            raise _lib.NtsError("%d seeds, the sampler was created for at most %d" % (t.numel(), self.max_seeds))
+        return t
+
+    def sample(self, seeds, seed, step):
+        """The SampledSubgraph of `seeds` for (seed, step)."""
+        s = self._seeds(seeds)
+        _lib.call("nts_sampler_sample", self.handle, s.data_ptr() if s.numel() else None, int(s.numel()),
+                  int(seed) & 0xFFFFFFFFFFFFFFFF, int(step) & 0xFFFFFFFFFFFFFFFF, _stream())
+        return SampledSubgraph([self._view(h) for h in range(len(self.fanout))], owner=self, vertices=self.V)
+
+    def _view(self, hop):
+        v = _lib.SampleHopView()
+        _lib.call("nts_sampler_hop_view", self.handle, int(hop), C.byref(v))
+
+        def arr(ptr, n, typestr="<i4"):
+            if n == 0:
+                return torch.empty(0, dtype=torch.int32 if typestr == "<i4" else torch.float32, device=self.device)
+            return torch.as_tensor(_DeviceArray(ptr, n, typestr), device=self.device)
+
+        nd, ns, ne = int(v.n_dst), int(v.n_src), int(v.n_edges)
+        return SampledBlock(arr(v.dst, nd), arr(v.column_offset, nd + 1), arr(v.row_indices, ne),
+                            arr(v.weight, ne, "<f4"), arr(v.src, ns), arr(v.row_offset, ns + 1),
+                            arr(v.column_indices, ne), arr(v.weight_backward, ne, "<f4"), arr(v.row_global, ne))
+
+    def __del__(self):
+        try:
+            if getattr(self, "handle", None):
+                _lib.load().nts_sampler_destroy(self.handle)
+                self.handle = None
+        except Exception:
+            pass

@@ -6,6 +6,8 @@
                      mask, tape backward, Adam); the single-GPU op of toolkits/GCN_EAGER_single.hpp when P = 1.
   * `GCNEagerImpl` <-> toolkits/GCN_EAGER_single.hpp / GCN_EAGER.hpp order (X.W first, aggregate the narrow result).
   * `GATImpl`    <-> the flow of toolkits/GAT_CPU_DIST_OPTM.hpp on the fused multi-head aggregation (K7).
+  * `GCNSampleImpl` <-> toolkits/GCN_CPU_SAMPLE.hpp (neighbour-sampled mini-batch GCN) on the K8 sampler and
+                     ops.MiniBatchFuseOp, one GPU.
 
 Dense NN work (mm, relu, log_softmax, nll_loss, Adam element-wise) stays on torch/cuBLAS exactly as in the
 reference (libtorch); the aggregation goes through libnts_b200."""
@@ -239,6 +241,128 @@ class GCNEagerImpl(GCNImpl):
         self.loss = torch.nn.functional.nll_loss(a.index_select(0, self.train_rows),
                                                  self.L_GT.index_select(0, self.train_rows))
         self.ctx.appendNNOp(self.X[-1], self.loss)
+
+
+def _minibatch_op(sampled_subgraph, active, hop, table=False):
+    return ops.MiniBatchFuseOp(sampled_subgraph, hop, table=table)
+
+
+class GCNSampleImpl:
+    """Neighbour-sampled mini-batch GCN: toolkits/GCN_CPU_SAMPLE.hpp:150-289 (ALGORITHM:GCNSAMPLESINGLE) on the GPU.
+    The train vertices (mask == 0), in id order, are cut into batches of `batch_size` seeds; each batch is sampled
+    (sample.NeighborSampler, hop h with fanout[h]) and runs an L-layer GCN over hops L-1 .. 0 (layer l aggregates hop
+    L-1-l with ops.MiniBatchFuseOp, then X.W, relu on hidden layers), log_softmax + nll_loss on the seeds, tape
+    backward and one Adam step.  The first layer gathers straight from the [V, F] feature table.
+
+    Deliberate differences from the reference (DESIGN.md §8): gradients are zeroed per batch (the reference zeroes once
+    per epoch); validation and test forwards never step Adam; dropout applies only while training; the sampler is
+    Floyd's algorithm on a counter hash, with sources ascending by global id.  Step t of a run samples with
+    (seed, t): two runs with the same seeds sample the same blocks, bit for bit.  Losses and weights agree bit for bit
+    only while no aggregation row is cut into three or more pieces by K1's edge quanta (rows longer than the quantum,
+    at least 32 edges on small blocks); such rows sum in scheduling order and may differ in the last bits between
+    runs (DESIGN.md §3 K8)."""
+
+    def __init__(self, partitioned_graph, layers, features, labels, mask, fanout, batch_size, learn_rate=0.01,
+                 weight_decay=0.0001, decay_rate=0.97, decay_epoch=100, drop_rate=0.5, seed=0, sample_seed=0):
+        self.layers = list(layers)
+        if len(fanout) != len(self.layers) - 1:
+            raise _lib.NtsError("fanout needs one entry per layer (%d), got %d" % (len(self.layers) - 1, len(fanout)))
+        self.batch_size = int(batch_size)
+        if self.batch_size < 1:
+            raise _lib.NtsError("batch_size must be >= 1")
+        from .sample import NeighborSampler
+        self.sampler = NeighborSampler(partitioned_graph, fanout, self.batch_size)
+        self.device = features.device
+        self.drop_rate = drop_rate
+        self.sample_seed = int(sample_seed)
+        self.step = 0
+        self.ctx = NtsContext()
+        gen = torch.Generator().manual_seed(seed)
+        self.P = []
+        for i in range(len(self.layers) - 1):
+            p = Parameter(self.layers[i], self.layers[i + 1], learn_rate, 0.9, 0.999, 1e-9, weight_decay,
+                          device=self.device, generator=gen)
+            p.init_parameter()
+            p.set_decay(decay_rate, decay_epoch)
+            self.P.append(p)
+        self.features = ops._check_input(features.detach(), "features")
+        self.L_GT = labels.to(self.device)
+        mask = torch.as_tensor(mask).cpu()
+        self.nids = [(mask == s).nonzero().view(-1) for s in (0, 1, 2)]    # train / val / test ids, ascending
+        self.subgraph = None
+        self.loss = None
+        self.epoch = 0
+
+    def Forward(self, seeds, training):
+        """Sample the batch and run the layers; returns the last layer's [n_seeds, classes] output."""
+        self.subgraph = sg = self.sampler.sample(seeds, self.sample_seed, self.step)
+        self.step += 1
+        L = len(self.layers) - 1
+        x = self.features
+        for l in range(L):
+            hop = L - 1 - l
+            if l != 0 and training and self.drop_rate > 0:
+                dropped = torch.nn.functional.dropout(x, self.drop_rate, training=True)
+                self.ctx.appendNNOp(x, dropped)
+                x = dropped
+            y = self.ctx.runGraphOp(_minibatch_op, sg, None, x.contiguous(), hop=hop, table=l == 0)
+            if l == L - 1:
+                x = self.ctx.runVertexForward(lambda n, _l=l: self.P[_l].forward(n), y)
+            else:
+                x = self.ctx.runVertexForward(lambda n, _l=l: torch.relu(self.P[_l].forward(n)), y)
+        return x
+
+    def Loss(self, out, seeds_dev):
+        """GCN_CPU_SAMPLE.hpp:187-195: log_softmax + nll_loss over the batch's seeds."""
+        self.loss = torch.nn.functional.nll_loss(out.log_softmax(1), self.L_GT.index_select(0, seeds_dev))
+        self.ctx.appendNNOp(out, self.loss)
+        return self.loss
+
+    def Update(self):
+        for p in self.P:
+            p.all_reduce_to_gradient(p.W.grad)
+            p.learn_with_decay_Adam()
+            p.next()
+
+    def train_step(self, seeds):
+        """One batch: zero the gradients, sample, forward, loss, tape backward, Adam.  Returns (loss, correct)."""
+        for p in self.P:
+            p.zero_grad()
+        self.ctx.train()
+        out = self.Forward(seeds, True)
+        seeds_dev = self.subgraph.seeds().long()
+        loss = self.Loss(out, seeds_dev)
+        correct = (out.argmax(1) == self.L_GT.index_select(0, seeds_dev)).sum()
+        self.ctx.self_backward(False)
+        self.Update()
+        return loss.detach(), correct
+
+    def evaluate(self, s):
+        """Accuracy over mask == s from sampled forwards (no dropout, no update)."""
+        self.ctx.eval()
+        correct = torch.zeros((), dtype=torch.int64, device=self.device)
+        ids = self.nids[s]
+        with torch.no_grad():
+            for b in range(0, ids.numel(), self.batch_size):
+                out = self.Forward(ids[b:b + self.batch_size], False)
+                correct += (out.argmax(1) == self.L_GT.index_select(0, self.subgraph.seeds().long())).sum()
+        self.ctx.train()
+        return float(correct) / max(ids.numel(), 1)
+
+    def run_epoch(self, test=True):
+        """One pass over the train batches (one Adam step each) and, with test=True, sampled validation and test
+        forwards.  Returns (mean train loss, [train, val, test] accuracy) - val / test are None with test=False."""
+        ids = self.nids[0]
+        losses, correct = [], torch.zeros((), dtype=torch.int64, device=self.device)
+        for b in range(0, ids.numel(), self.batch_size):
+            loss, c = self.train_step(ids[b:b + self.batch_size])
+            losses.append(loss)
+            correct += c
+        mean_loss = float(torch.stack(losses).mean()) if losses else float("nan")
+        acc = [float(correct) / max(ids.numel(), 1)]
+        acc += [self.evaluate(1), self.evaluate(2)] if test else [None, None]
+        self.epoch += 1
+        return mean_loss, acc
 
 
 class GATImpl:

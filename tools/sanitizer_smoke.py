@@ -71,5 +71,16 @@ for H, D in ((1, 16), (4, 8)):
     single = ops.DistGPUFusedGATOp(pg, two_pass_backward=False)   # the single-pass (atomic) backward as well
     single.forward(mirror, mirror[:, :H].contiguous(), x[:, :H].contiguous())
     single.backward(out)
+# neighbour sampling (K8): Floyd and keep-all destinations, a hub, an empty sample, the device transpose
+from neutronstarlite_b200.sample import NeighborSampler, SampledSubgraph
+sampler = NeighborSampler(pg, [5, 64, 3], 128)
+sg = sampler.sample(np.arange(0, V, 6)[:128], 1, 0)
+sampler.sample(np.zeros(0, dtype=np.int64), 1, 1)
+sg = sampler.sample(np.array([3, 0, 1]), 1, 2)
+b = sg.blocks[1]
+SampledSubgraph.from_blocks([{"dst": b.dst, "column_offset": b.column_offset, "row_indices": b.row_indices,
+                              "weight": b.weight, "src": b.src}])
+op = ops.MiniBatchFuseOp(sg, 1)
+op.backward(op.forward(torch.rand((b.n_src, 41), device=dev)))
 torch.cuda.synchronize()
 print("sanitizer smoke done, launches:", _lib.load().nts_kernel_launch_count())
