@@ -620,7 +620,16 @@ int nts_graph_build_destroy(nts_graph_build *build);
  * function of (graph, seed, step, h, d).  A hop's sources are its distinct source ids ascending; local source ids
  * index them.  Scratch is allocated once, at create, for max_seeds seeds; 1 <= fanout[h] <= 64, 1 <= hops <= 8.
  * nts_sampler_sample synchronises `stream` once per hop (to read the hop's edge and source counts) and reports a seed
- * >= V as an error after hop 0.  Hop views point into the sampler's memory and stay valid until the next sample. */
+ * >= V as an error after hop 0.  Hop views point into the sampler's memory and stay valid until the next sample.
+ *
+ * NTS_SAMPLER_INCLUDE_DST (nts_sampler_create_ex): every hop's sources include its destinations, the block layout a
+ * layer needs when a destination reads its own previous-layer row (a GAT layer's destination score).  A hop keeps
+ * exactly the edges, weights and slot order of the default mode (no self-loop edge is added); its sources are the
+ * distinct ids of (kept sources U destinations), ascending, and nts_sampler_hop_dst_pos gives dst_pos[n_dst], each
+ * destination's local index in src (src[dst_pos[i]] == dst[i]).  Hop h+1's destinations are hop h's sources, so the
+ * destination set only grows with depth.  Scratch is sized for n_dst * (fanout + 1) pairs per hop.  With flags = 0
+ * the sampler is nts_sampler_create's, byte for byte. */
+#define NTS_SAMPLER_INCLUDE_DST 1u
 typedef struct nts_sampler nts_sampler;
 typedef struct nts_sample_hop_view {
   nts_vid_t n_dst, n_src;
@@ -638,9 +647,16 @@ typedef struct nts_sample_hop_view {
 nts_sampler *nts_sampler_create(const nts_vid_t *column_offset, const nts_vid_t *row_indices, const float *edge_weight,
                                 nts_vid_t n_vertices, uint64_t n_edges, nts_vid_t max_seeds, int hops,
                                 const int *fanout, void *stream);
+/* flags: 0 or NTS_SAMPLER_INCLUDE_DST; other bits are an argument error.  nts_sampler_create is flags = 0. */
+nts_sampler *nts_sampler_create_ex(const nts_vid_t *column_offset, const nts_vid_t *row_indices,
+                                   const float *edge_weight, nts_vid_t n_vertices, uint64_t n_edges,
+                                   nts_vid_t max_seeds, int hops, const int *fanout, uint32_t flags, void *stream);
 int nts_sampler_sample(nts_sampler *sampler, const nts_vid_t *seeds, nts_vid_t n_seeds, uint64_t seed, uint64_t step,
                        void *stream);
 int nts_sampler_hop_view(const nts_sampler *sampler, int hop, nts_sample_hop_view *view);
+/* *dst_pos = the hop's dst_pos[n_dst] (device, local source index of every destination); an error unless the sampler
+ * was created with NTS_SAMPLER_INCLUDE_DST.  Valid until the next sample, like the hop view. */
+int nts_sampler_hop_dst_pos(const nts_sampler *sampler, int hop, const nts_vid_t **dst_pos);
 /* peak device bytes the sampler holds (scratch and hop storage) */
 uint64_t nts_sampler_bytes(const nts_sampler *sampler);
 int nts_sampler_destroy(nts_sampler *sampler);

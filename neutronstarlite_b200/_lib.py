@@ -222,8 +222,10 @@ class SampleHopView(C.Structure):
 
 SIGNATURES.update({
     "nts_sampler_create": (_vp, [_vp, _vp, _vp, _u32, _u64, _u32, _int, C.POINTER(_int), _vp]),
+    "nts_sampler_create_ex": (_vp, [_vp, _vp, _vp, _u32, _u64, _u32, _int, C.POINTER(_int), _u32, _vp]),
     "nts_sampler_sample": (_int, [_vp, _vp, _u32, _u64, _u64, _vp]),
     "nts_sampler_hop_view": (_int, [_vp, _int, C.POINTER(SampleHopView)]),
+    "nts_sampler_hop_dst_pos": (_int, [_vp, _int, C.POINTER(_vp)]),
     "nts_sampler_bytes": (_u64, [_vp]),
     "nts_sampler_destroy": (_int, [_vp]),
     "nts_sample_transpose": (_int, [_vp, _vp, _vp, _u32, _u32, _u64, _vp, _vp, _vp, _vp]),

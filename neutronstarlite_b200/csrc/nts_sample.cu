@@ -13,6 +13,12 @@
 //            edge order, stable by edge position), in one pass
 // then one 12-byte device-to-host copy (edge count, source count, bad-seed flag) sizes the next hop.  No atomics on
 // floats anywhere; the only atomic is the bad-seed flag.
+//
+// NTS_SAMPLER_INCLUDE_DST: the count pass also appends one marker pair (destination id, kMarker | i) per destination
+// after the n_dst * k edge pairs, so the same sort puts every destination among the sources; the stable sort leaves a
+// key's markers after its edges.  One inclusive scan over 64-bit flags (head count in the high word, marker count in
+// the low word) gives each pair its local source id and each edge pair its transposed position (sorted position minus
+// the markers before it), so the transposed block is still stable by edge position.  Markers write dst_pos.
 #include <cub/cub.cuh>
 
 #include <vector>
@@ -28,6 +34,7 @@ constexpr int kMaxFanout = 64;
 constexpr int kMaxHops = 8;
 constexpr int kSelectWarps = 8;
 constexpr int kThreads = 256;
+constexpr u32 kMarker = 0x80000000u;   // value bit of a destination marker pair (edge positions are < 2^31)
 
 __host__ __device__ __forceinline__ u64 splitmix64(u64 z) {
   z += 0x9E3779B97F4A7C15ull;
@@ -37,7 +44,8 @@ __host__ __device__ __forceinline__ u64 splitmix64(u64 z) {
 }
 
 __global__ void count_kernel(const u32 *__restrict__ dst, u32 n_dst, const u32 *__restrict__ g_col, u32 V, u32 k,
-                             u32 *__restrict__ cnt, u32 *__restrict__ bad) {
+                             u32 *__restrict__ cnt, u32 *__restrict__ bad, u32 *__restrict__ marker_keys,
+                             u32 *__restrict__ marker_vals) {
   const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (i > n_dst) return;
   u32 c = 0;
@@ -47,6 +55,10 @@ __global__ void count_kernel(const u32 *__restrict__ dst, u32 n_dst, const u32 *
       c = min(g_col[v + 1] - g_col[v], k);
     } else {
       atomicOr(bad, 1u);
+    }
+    if (marker_keys) {            // NTS_SAMPLER_INCLUDE_DST; a bad id sorts with the unused pairs
+      marker_keys[i] = min(v, V);
+      marker_vals[i] = kMarker | (u32)i;
     }
   }
   cnt[i] = c;   // cnt[n_dst] = 0: the exclusive scan's last element is the edge count
@@ -142,6 +154,57 @@ __global__ void finish_kernel(const u32 *__restrict__ skeys, const u32 *__restri
   }
 }
 
+// NTS_SAMPLER_INCLUDE_DST: flag[i] = (head << 32) | marker over the n_tot sorted pairs; keys >= V (unused pairs, bad
+// seeds) are neither
+__global__ void head_dst_kernel(const u32 *__restrict__ skeys, const u32 *__restrict__ svals, u64 n_tot, u32 V,
+                                u64 *__restrict__ flag) {
+  const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_tot) return;
+  const u32 key = skeys[i];
+  const bool valid = key < V;
+  const bool head = valid && (i == 0 || key != skeys[i - 1]);
+  const bool marker = valid && (svals[i] & kMarker);
+  flag[i] = ((u64)head << 32) | (u64)marker;
+}
+
+__global__ void finish_dst_kernel(const u32 *__restrict__ skeys, const u32 *__restrict__ svals,
+                                  const u64 *__restrict__ pos, u64 n_tot, const u32 *__restrict__ col, u32 n_dst,
+                                  u32 V, const u32 *__restrict__ edge_dst, const float *__restrict__ weight,
+                                  u32 *__restrict__ row_local, u32 *__restrict__ src, u32 *__restrict__ row_offset,
+                                  u32 *__restrict__ col_t, float *__restrict__ w_t, u32 *__restrict__ dst_pos,
+                                  u32 *__restrict__ counts) {
+  const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  const u32 n_edges = col[n_dst];
+  if (i == 0 && (n_tot == 0 || skeys[0] >= V)) {
+    row_offset[0] = 0;
+    counts[0] = 0;
+    counts[1] = 0;
+  }
+  if (i >= n_tot) return;
+  const u32 key = skeys[i];
+  if (key >= V) return;
+  const u64 p = pos[i];
+  const u32 l = (u32)(p >> 32) - 1, val = svals[i];
+  const u32 mk = val >> 31;
+  const u32 t = (u32)i - (u32)p + mk;   // edge pairs before sorted position i: its transposed position
+  if (mk) {
+    dst_pos[val & ~kMarker] = l;
+  } else {
+    row_local[val] = l;
+    col_t[t] = edge_dst[val];
+    w_t[t] = weight[val];
+  }
+  if (i == 0 || key != skeys[i - 1]) {
+    src[l] = key;
+    row_offset[l] = t;
+  }
+  if (i + 1 == n_tot || skeys[i + 1] >= V) {
+    row_offset[l + 1] = n_edges;
+    counts[0] = n_edges;
+    counts[1] = l + 1;
+  }
+}
+
 // nts_sample_transpose: the destination of every edge, and lower bounds of each source in the sorted keys
 __global__ void edge_dst_kernel(const u32 *__restrict__ col, u32 n_dst, u32 *__restrict__ edge_dst,
                                 u32 *__restrict__ iota) {
@@ -189,12 +252,14 @@ struct nts_sampler {
   u32 V = 0;
   u32 max_seeds = 0;
   int hops = 0;
+  bool include_dst = false;   // NTS_SAMPLER_INCLUDE_DST
   u32 fanout[kMaxHops] = {};
   u64 cap_dst[kMaxHops] = {}, cap_pad[kMaxHops] = {}, cap_src[kMaxHops] = {};
   struct Hop {
     u32 *dst = nullptr, *col = nullptr, *row_local = nullptr, *row_global = nullptr, *edge_dst = nullptr;
     float *weight = nullptr, *w_t = nullptr;
     u32 *src = nullptr, *row_offset = nullptr, *col_t = nullptr;
+    u32 *dst_pos = nullptr;   // include_dst only
     u32 n_dst = 0, n_src = 0;
     u64 n_edges = 0;
   } hop[kMaxHops];
@@ -202,6 +267,7 @@ struct nts_sampler {
   // scratch shared by the hops
   u32 *cnt = nullptr, *keys = nullptr, *keys_alt = nullptr, *vals = nullptr, *vals_alt = nullptr, *flag = nullptr,
       *pos = nullptr, *counts = nullptr;
+  u64 *flag64 = nullptr, *pos64 = nullptr;   // include_dst: replace flag / pos
   void *tmp = nullptr;
   size_t tmp_bytes = 0;
   u32 *counts_host = nullptr;
@@ -227,9 +293,12 @@ int sampler_setup(nts_sampler *s, cudaStream_t st) {
   u64 max_dst = 0, max_pad = 0;
   for (int h = 0; h < s->hops; ++h) {
     s->cap_dst[h] = h == 0 ? s->max_seeds : s->cap_src[h - 1];
-    s->cap_pad[h] = s->cap_dst[h] * s->fanout[h];
+    // include_dst: one marker pair per destination after the edge pairs, and up to n_dst more sources
+    s->cap_pad[h] = s->cap_dst[h] * (s->fanout[h] + (s->include_dst ? 1 : 0));
     s->cap_src[h] = std::min<u64>(s->V, s->cap_pad[h]);
-    NTS_ARG_CHECK(s->cap_pad[h] < (1ull << 31), "sampler worst case n_dst * fanout reaches 2^31 edges in one hop");
+    NTS_ARG_CHECK(s->cap_pad[h] < (1ull << 31),
+                  s->include_dst ? "sampler worst case n_dst * (fanout + 1) reaches 2^31 pairs in one hop"
+                                 : "sampler worst case n_dst * fanout reaches 2^31 edges in one hop");
     max_dst = std::max(max_dst, s->cap_dst[h]);
     max_pad = std::max(max_pad, s->cap_pad[h]);
   }
@@ -247,18 +316,27 @@ int sampler_setup(nts_sampler *s, cudaStream_t st) {
         (rc = s->alloc(&H.w_t, E)) || (rc = s->alloc(&H.col_t, E)) || (rc = s->alloc(&H.src, S)) ||
         (rc = s->alloc(&H.row_offset, S + 1)))
       return rc;
+    if (s->include_dst && (rc = s->alloc(&H.dst_pos, s->cap_dst[h]))) return rc;
   }
   int rc = 0;
   if ((rc = s->alloc(&s->cnt, max_dst + 1)) || (rc = s->alloc(&s->keys, max_pad)) ||
       (rc = s->alloc(&s->keys_alt, max_pad)) || (rc = s->alloc(&s->vals, max_pad)) ||
-      (rc = s->alloc(&s->vals_alt, max_pad)) || (rc = s->alloc(&s->flag, max_pad)) ||
-      (rc = s->alloc(&s->pos, max_pad)) || (rc = s->alloc(&s->counts, 4)))
+      (rc = s->alloc(&s->vals_alt, max_pad)) || (rc = s->alloc(&s->counts, 4)))
     return rc;
+  if (s->include_dst) {
+    if ((rc = s->alloc(&s->flag64, max_pad)) || (rc = s->alloc(&s->pos64, max_pad))) return rc;
+  } else if ((rc = s->alloc(&s->flag, max_pad)) || (rc = s->alloc(&s->pos, max_pad))) {
+    return rc;
+  }
   // CUB scratch for the largest scan and sort (queried again, and checked, at every call)
   size_t b0 = 0, b1 = 0, b2 = 0;
   cub::DoubleBuffer<u32> kd(s->keys, s->keys_alt), vd(s->vals, s->vals_alt);
   NTS_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, b0, s->cnt, s->cnt, (int64_t)(max_dst + 1), st));
-  NTS_CUDA_OK(cub::DeviceScan::InclusiveSum(nullptr, b1, s->flag, s->pos, (int64_t)std::max<u64>(max_pad, 1), st));
+  if (s->include_dst)
+    NTS_CUDA_OK(cub::DeviceScan::InclusiveSum(nullptr, b1, s->flag64, s->pos64, (int64_t)std::max<u64>(max_pad, 1),
+                                              st));
+  else
+    NTS_CUDA_OK(cub::DeviceScan::InclusiveSum(nullptr, b1, s->flag, s->pos, (int64_t)std::max<u64>(max_pad, 1), st));
   NTS_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, b2, kd, vd, (int64_t)std::max<u64>(max_pad, 1), 0, 32, st));
   s->tmp_bytes = std::max(b0, std::max(b1, b2));
   if ((rc = s->alloc(reinterpret_cast<char **>(&s->tmp), s->tmp_bytes))) return rc;
@@ -271,12 +349,23 @@ int check_tmp(const nts_sampler *s, size_t need) {
   return 0;
 }
 
+template <class T> int inclusive_sum(nts_sampler *s, const T *in, T *out, u64 n, cudaStream_t st) {
+  size_t need = 0;
+  NTS_CUDA_OK(cub::DeviceScan::InclusiveSum(nullptr, need, in, out, (int64_t)n, st));
+  if (int rc = check_tmp(s, need)) return rc;
+  NTS_CUDA_OK(cub::DeviceScan::InclusiveSum(s->tmp, need, in, out, (int64_t)n, st));
+  return 0;
+}
+
 int sample_hop(nts_sampler *s, int h, u64 step_key, cudaStream_t st) {
   nts_sampler::Hop &H = s->hop[h];
   const u32 n_dst = H.n_dst, k = s->fanout[h];
+  const bool inc = s->include_dst;
   const u64 n_pad = (u64)n_dst * k;
+  const u64 n_sort = inc ? n_pad + n_dst : n_pad;   // include_dst: the marker pairs follow the edge pairs
   count_kernel<<<blocks_for((u64)n_dst + 1), kThreads, 0, st>>>(H.dst, n_dst, s->g_col, s->V, k, s->cnt,
-                                                                  s->counts + 2);
+                                                                  s->counts + 2, inc ? s->keys + n_pad : nullptr,
+                                                                  inc ? s->vals + n_pad : nullptr);
   NTS_LAUNCH_CHECK();
   size_t need = 0;
   NTS_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, need, s->cnt, H.col, (int64_t)n_dst + 1, st));
@@ -290,20 +379,29 @@ int sample_hop(nts_sampler *s, int h, u64 step_key, cudaStream_t st) {
     NTS_LAUNCH_CHECK();
     cub::DoubleBuffer<u32> kd(s->keys, s->keys_alt), vd(s->vals, s->vals_alt);
     const int end_bit = bits_for(s->V);
-    NTS_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, need, kd, vd, (int64_t)n_pad, 0, end_bit, st));
+    NTS_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, need, kd, vd, (int64_t)n_sort, 0, end_bit, st));
     if (int rc = check_tmp(s, need)) return rc;
-    NTS_CUDA_OK(cub::DeviceRadixSort::SortPairs(s->tmp, need, kd, vd, (int64_t)n_pad, 0, end_bit, st));
+    NTS_CUDA_OK(cub::DeviceRadixSort::SortPairs(s->tmp, need, kd, vd, (int64_t)n_sort, 0, end_bit, st));
     skeys = kd.Current();
     svals = vd.Current();
-    head_kernel<<<blocks_for(n_pad), kThreads, 0, st>>>(skeys, n_pad, H.col, n_dst, s->flag);
-    NTS_LAUNCH_CHECK();
-    NTS_CUDA_OK(cub::DeviceScan::InclusiveSum(nullptr, need, s->flag, s->pos, (int64_t)n_pad, st));
-    if (int rc = check_tmp(s, need)) return rc;
-    NTS_CUDA_OK(cub::DeviceScan::InclusiveSum(s->tmp, need, s->flag, s->pos, (int64_t)n_pad, st));
+    if (inc) {
+      head_dst_kernel<<<blocks_for(n_sort), kThreads, 0, st>>>(skeys, svals, n_sort, s->V, s->flag64);
+      NTS_LAUNCH_CHECK();
+      if (int rc = inclusive_sum(s, s->flag64, s->pos64, n_sort, st)) return rc;
+    } else {
+      head_kernel<<<blocks_for(n_pad), kThreads, 0, st>>>(skeys, n_pad, H.col, n_dst, s->flag);
+      NTS_LAUNCH_CHECK();
+      if (int rc = inclusive_sum(s, s->flag, s->pos, n_pad, st)) return rc;
+    }
   }
-  finish_kernel<<<blocks_for(std::max<u64>(n_pad, 1)), kThreads, 0, st>>>(
-      skeys, svals, s->pos, n_pad, H.col, n_dst, H.edge_dst, H.weight, H.row_local, H.src, H.row_offset, H.col_t,
-      H.w_t, s->counts);
+  if (inc)
+    finish_dst_kernel<<<blocks_for(std::max<u64>(n_sort, 1)), kThreads, 0, st>>>(
+        skeys, svals, s->pos64, n_sort, H.col, n_dst, s->V, H.edge_dst, H.weight, H.row_local, H.src, H.row_offset,
+        H.col_t, H.w_t, H.dst_pos, s->counts);
+  else
+    finish_kernel<<<blocks_for(std::max<u64>(n_pad, 1)), kThreads, 0, st>>>(
+        skeys, svals, s->pos, n_pad, H.col, n_dst, H.edge_dst, H.weight, H.row_local, H.src, H.row_offset, H.col_t,
+        H.w_t, s->counts);
   NTS_LAUNCH_CHECK();
   NTS_CUDA_OK(cudaMemcpyAsync(s->counts_host, s->counts, 3 * sizeof(u32), cudaMemcpyDeviceToHost, st));
   NTS_CUDA_OK(cudaStreamSynchronize(st));
@@ -320,6 +418,13 @@ extern "C" {
 nts_sampler *nts_sampler_create(const nts_vid_t *column_offset, const nts_vid_t *row_indices, const float *edge_weight,
                                 nts_vid_t n_vertices, uint64_t n_edges, nts_vid_t max_seeds, int hops,
                                 const int *fanout, void *stream) {
+  return nts_sampler_create_ex(column_offset, row_indices, edge_weight, n_vertices, n_edges, max_seeds, hops, fanout,
+                               0, stream);
+}
+
+nts_sampler *nts_sampler_create_ex(const nts_vid_t *column_offset, const nts_vid_t *row_indices,
+                                   const float *edge_weight, nts_vid_t n_vertices, uint64_t n_edges,
+                                   nts_vid_t max_seeds, int hops, const int *fanout, uint32_t flags, void *stream) {
   auto bad = [](const char *msg) -> nts_sampler * {
     nts::fail(-1, msg, __FILE__, __LINE__);
     return nullptr;
@@ -331,7 +436,9 @@ nts_sampler *nts_sampler_create(const nts_vid_t *column_offset, const nts_vid_t 
   if (n_vertices == 0 || n_vertices >= (1u << 31)) return bad("sampler needs 1 <= V < 2^31");
   if (n_edges >= (1ull << 32)) return bad("sampler needs fewer than 2^32 edges");
   if (!column_offset || (n_edges && (!row_indices || !edge_weight))) return bad("null graph array passed to sampler");
+  if (flags & ~(uint32_t)NTS_SAMPLER_INCLUDE_DST) return bad("unknown sampler flag bits");
   nts_sampler *s = new nts_sampler;
+  s->include_dst = (flags & NTS_SAMPLER_INCLUDE_DST) != 0;
   s->g_col = column_offset;
   s->g_row = row_indices;
   s->g_w = edge_weight;
@@ -381,6 +488,15 @@ int nts_sampler_hop_view(const nts_sampler *s, int hop, nts_sample_hop_view *v) 
   v->row_offset = H.row_offset;
   v->column_indices = H.col_t;
   v->weight_backward = H.w_t;
+  return 0;
+}
+
+int nts_sampler_hop_dst_pos(const nts_sampler *s, int hop, const nts_vid_t **dst_pos) {
+  NTS_ARG_CHECK(s != nullptr && dst_pos != nullptr, "null sampler or dst_pos");
+  NTS_ARG_CHECK(s->include_dst, "the sampler was created without NTS_SAMPLER_INCLUDE_DST");
+  NTS_ARG_CHECK(hop >= 0 && hop < s->hops, "hop out of range");
+  NTS_ARG_CHECK(s->sampled, "the sampler holds no complete sample");
+  *dst_pos = s->hop[hop].dst_pos;
   return 0;
 }
 

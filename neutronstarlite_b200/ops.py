@@ -581,6 +581,120 @@ class DistGPUAggregateDstFuseWeight(_EdgeOp):
         return self.e_weight_grad
 
 
+class _FusedGAT:
+    """The K7 launches of one GAT layer on one topology, shared by DistGPUFusedGATOp (a partition's CSC and its
+    mirror-slot CSR) and MiniBatchGATOp (a sampled block and its transposed block).  Edge e of destination d
+    (column_offset[d] <= e < column_offset[d+1]) reads row slots[e] of the gathered matrix, which has n_src rows; the
+    two-pass backward lists the out-edges of every row in (slot_row_offset, slot_column_indices), edges of a row in
+    edge order.  forward(x, s, d) runs the statistics and the aggregation and keeps what the backward needs;
+    backward_two_pass(g, slot_row_offset, slot_column_indices) returns (dx, ds, dd)."""
+
+    def __init__(self, column_offset, slots, n_dst, n_src, n_edges, slope, gather_dtype):
+        self.column_offset, self.slots = column_offset, slots
+        self.n_dst, self.n_src, self.n_edges = int(n_dst), int(n_src), int(n_edges)
+        self.slope, self.gather_dtype = slope, gather_dtype
+        self.saved = None
+
+    def forward(self, x, s, d):
+        H = int(s.shape[1])
+        seg_max = torch.empty((self.n_dst, H), dtype=torch.float32, device=x.device)
+        seg_sum = torch.empty_like(seg_max)
+        with _timed("gat_stats", x.shape[1], self.n_edges, self.n_dst):
+            _lib.call("nts_gat_softmax_stats", _ptr(seg_max), _ptr(seg_sum), _ptr(s), _ptr(d), _ptr(self.slots),
+                      _ptr(self.column_offset), 0, self.n_dst, H, self.slope, _stream())
+        F = int(x.shape[1])
+        if self.gather_dtype is not None:
+            return self._forward_bf16(x, s, d, seg_max, seg_sum, H, F)
+        xk, Fk = x, F
+        if H == 1 and F % 4 != 0:
+            # odd single-head width (the 41-wide output layer of config D): gather from a copy padded to a multiple
+            # of 4 columns so that the kernel uses 16-byte loads and packed virtual warps instead of 4-byte gathers
+            # (11.9 -> ~4 ms per call on config D); the zero columns are dropped again below
+            Fk = (F + 3) // 4 * 4
+            xk = torch.nn.functional.pad(x, (0, Fk - F))
+        out = torch.zeros((self.n_dst, Fk), dtype=torch.float32, device=x.device)
+        with _timed("gat_fwd", F, self.n_edges, self.n_dst):
+            _lib.call("nts_gat_fused_aggregate_forward", _ptr(xk), _ptr(out), _ptr(s), _ptr(d), _ptr(seg_max),
+                      _ptr(seg_sum), _ptr(self.slots), _ptr(self.column_offset), 0,
+                      self.n_dst, self.n_edges, Fk, H, self.slope, _stream())
+        if Fk != F:
+            out = out[:, :F].contiguous()
+        self.saved = (x, s, d, seg_max, seg_sum, out)
+        return out
+
+    @staticmethod
+    def _to_bf16_rows(t, ld):
+        """bf16(t) as rows of ld values, the columns past t's width zero (nts_rows_to_bf16)."""
+        n, F = t.shape
+        r = torch.empty((n, ld), dtype=torch.bfloat16, device=t.device)
+        with _timed("gat_bf16_round", F, 0, n):
+            _lib.call("nts_rows_to_bf16", _ptr(t), _DTYPE_CODE[torch.float32], F, _ptr(r), n, F, ld, _stream())
+        return r
+
+    def _forward_bf16(self, x, s, d, seg_max, seg_sum, H, F):
+        # rows of ld = ceil(F/8)*8 BF16 values: 16-byte chunks of 8, and for the 41-wide layer this replaces the
+        # padded FP32 copy of the FP32 path; out shares the row stride and loses its zero pad columns below
+        ld = (F + 7) // 8 * 8
+        mt = self._to_bf16_rows(x, ld)
+        out = torch.zeros((self.n_dst, ld), dtype=torch.float32, device=x.device)
+        with _timed("gat_fwd", F, self.n_edges, self.n_dst):
+            _lib.call("nts_gat_fused_aggregate_forward_bf16", _ptr(mt), _ptr(out), _ptr(s), _ptr(d), _ptr(seg_max),
+                      _ptr(seg_sum), _ptr(self.slots), _ptr(self.column_offset), 0, self.n_dst, self.n_edges,
+                      F, ld, H, self.slope, _stream())
+        if ld != F:
+            out = out[:, :F].contiguous()
+        self.saved = (mt, s, d, seg_max, seg_sum, out)   # m~ is what the backward gathers: the FP32 input is not kept
+        return out
+
+    def _backward_bf16(self, g, slot_off, slot_dst):
+        mt, s, d, seg_max, seg_sum, out = self.saved
+        H = int(s.shape[1])
+        M, ld = mt.shape
+        F = int(out.shape[1])
+        gt = self._to_bf16_rows(g, ld)
+        # <out, g~>, not <out, g>: the passes rely on sum_e a <m~, g~> == <out, g~>; mixing g and g~ would bias the
+        # score gradients by about 2^-8
+        out_dot_g = (out.detach() * gt[:, :F].float()).view(-1, H, F // H).sum(-1).contiguous()
+        dm = torch.zeros((M, ld), dtype=torch.float32, device=g.device)
+        ds = torch.zeros_like(s)
+        dd = torch.zeros_like(d)
+        pack = torch.empty((self.n_dst, H, 4), dtype=torch.float32, device=g.device)
+        with _timed("gat_bwd", F, 2 * self.n_edges, self.n_dst):
+            _lib.call("nts_gat_fused_aggregate_backward_two_pass_bf16", _ptr(dm), _ptr(ds), _ptr(dd), _ptr(pack),
+                      _ptr(mt), _ptr(s), _ptr(d), _ptr(seg_max), _ptr(seg_sum), _ptr(out_dot_g), _ptr(gt),
+                      _ptr(self.slots), _ptr(self.column_offset), 0, _ptr(slot_off), _ptr(slot_dst),
+                      self.n_dst, M, F, ld, H, self.slope, _stream())
+        if ld != F:
+            dm = dm[:, :F].contiguous()
+        return dm, ds, dd
+
+    def out_dot_grad(self, g):
+        """<out[d,h], g[d,h]> of the FP32 layer: sum_e a[e,h] <x[slot(e),h], g[d,h]>, so the softmax backward needs
+        no edge pass."""
+        x, s, _, _, _, out = self.saved
+        H = int(s.shape[1])
+        return (out.detach() * g).view(-1, H, x.shape[1] // H).sum(-1).contiguous()
+
+    def backward_two_pass(self, g, slot_off, slot_dst):
+        """No per-edge atomics: a destination-major and a source-major pass, each with register accumulators."""
+        if self.gather_dtype is not None:
+            return self._backward_bf16(g, slot_off, slot_dst)
+        x, s, d, seg_max, seg_sum, out = self.saved
+        H = int(s.shape[1])
+        out_dot_g = self.out_dot_grad(g)
+        dm = torch.zeros_like(x)
+        ds = torch.zeros_like(s)
+        dd = torch.zeros_like(d)
+        pack = torch.empty((self.n_dst, H, 4), dtype=torch.float32, device=x.device)
+        with _timed("gat_bwd", x.shape[1], 2 * self.n_edges, self.n_dst):
+            _lib.call("nts_gat_fused_aggregate_backward_two_pass", _ptr(dm), _ptr(ds), _ptr(dd), _ptr(pack),
+                      _ptr(x), _ptr(s), _ptr(d), _ptr(seg_max), _ptr(seg_sum), _ptr(out_dot_g), _ptr(g),
+                      _ptr(self.slots), _ptr(self.column_offset), 0,
+                      _ptr(slot_off), _ptr(slot_dst), self.n_dst, x.shape[0], x.shape[1], H, self.slope,
+                      _stream())
+        return dm, ds, dd
+
+
 class DistGPUFusedGATOp(_EdgeOp):
     """K7: the whole attention + aggregation of one GAT layer in two kernels forward and two passes backward, never
     materialising an edge-sized tensor (toolkits/GAT_CPU_DIST_OPTM.hpp:196-241 keeps [E,1] logits / attention;
@@ -605,7 +719,7 @@ class DistGPUFusedGATOp(_EdgeOp):
         self.gather_dtype = _check_gather_dtype(gather_dtype)
         if self.gather_dtype is not None and not self.two_pass_backward:
             raise _lib.NtsError("BF16 gathers of the fused GAT layer need two_pass_backward=True")
-        self._saved = None
+        self._k7 = None
 
     @staticmethod
     def slot_indices(pg):
@@ -640,106 +754,93 @@ class DistGPUFusedGATOp(_EdgeOp):
         x = _check_input(mirror, "mirror")
         s = _check_input(src_score, "src_score")
         d = _check_input(dst_score, "dst_score")
-        H = int(s.shape[1])
-        seg_max = torch.empty((pg.owned_vertices, H), dtype=torch.float32, device=x.device)
-        seg_sum = torch.empty_like(seg_max)
-        slots = self.slot_indices(pg)
-        with _timed("gat_stats", x.shape[1], pg.owned_edges, pg.owned_vertices):
-            _lib.call("nts_gat_softmax_stats", _ptr(seg_max), _ptr(seg_sum), _ptr(s), _ptr(d), _ptr(slots),
-                      _ptr(pg.column_offset_gpu), 0, pg.owned_vertices, H, self.slope, _stream())
-        F = int(x.shape[1])
-        if self.gather_dtype is not None:
-            return self._forward_bf16(pg, x, s, d, seg_max, seg_sum, slots, H, F)
-        xk, Fk = x, F
-        if H == 1 and F % 4 != 0:
-            # odd single-head width (the 41-wide output layer of config D): gather from a copy padded to a multiple
-            # of 4 columns so that the kernel uses 16-byte loads and packed virtual warps instead of 4-byte gathers
-            # (11.9 -> ~4 ms per call on config D); the zero columns are dropped again below
-            Fk = (F + 3) // 4 * 4
-            xk = torch.nn.functional.pad(x, (0, Fk - F))
-        out = torch.zeros((pg.owned_vertices, Fk), dtype=torch.float32, device=x.device)
-        with _timed("gat_fwd", F, pg.owned_edges, pg.owned_vertices):
-            _lib.call("nts_gat_fused_aggregate_forward", _ptr(xk), _ptr(out), _ptr(s), _ptr(d), _ptr(seg_max),
-                      _ptr(seg_sum), _ptr(slots), _ptr(pg.column_offset_gpu), 0,
-                      pg.owned_vertices, pg.owned_edges, Fk, H, self.slope, _stream())
-        if Fk != F:
-            out = out[:, :F].contiguous()
-        self._saved = (x, s, d, seg_max, seg_sum, out)
-        return out
+        self._k7 = _FusedGAT(pg.column_offset_gpu, self.slot_indices(pg), pg.owned_vertices, x.shape[0],
+                             pg.owned_edges, self.slope, self.gather_dtype)
+        return self._k7.forward(x, s, d)
 
-    @staticmethod
-    def _to_bf16_rows(t, ld):
-        """bf16(t) as rows of ld values, the columns past t's width zero (nts_rows_to_bf16)."""
-        n, F = t.shape
-        r = torch.empty((n, ld), dtype=torch.bfloat16, device=t.device)
-        with _timed("gat_bf16_round", F, 0, n):
-            _lib.call("nts_rows_to_bf16", _ptr(t), _DTYPE_CODE[torch.float32], F, _ptr(r), n, F, ld, _stream())
-        return r
-
-    def _forward_bf16(self, pg, x, s, d, seg_max, seg_sum, slots, H, F):
-        # rows of ld = ceil(F/8)*8 BF16 values: 16-byte chunks of 8, and for the 41-wide layer this replaces the
-        # padded FP32 copy of the FP32 path; out shares the row stride and loses its zero pad columns below
-        ld = (F + 7) // 8 * 8
-        mt = self._to_bf16_rows(x, ld)
-        out = torch.zeros((pg.owned_vertices, ld), dtype=torch.float32, device=x.device)
-        with _timed("gat_fwd", F, pg.owned_edges, pg.owned_vertices):
-            _lib.call("nts_gat_fused_aggregate_forward_bf16", _ptr(mt), _ptr(out), _ptr(s), _ptr(d), _ptr(seg_max),
-                      _ptr(seg_sum), _ptr(slots), _ptr(pg.column_offset_gpu), 0, pg.owned_vertices, pg.owned_edges,
-                      F, ld, H, self.slope, _stream())
-        if ld != F:
-            out = out[:, :F].contiguous()
-        self._saved = (mt, s, d, seg_max, seg_sum, out)   # m~ is what the backward gathers: the FP32 mirror is not kept
-        return out
-
-    def _backward_bf16(self, pg, g):
-        mt, s, d, seg_max, seg_sum, out = self._saved
-        H = int(s.shape[1])
-        M, ld = mt.shape
-        F = int(out.shape[1])
-        gt = self._to_bf16_rows(g, ld)
-        # <out, g~>, not <out, g>: the passes rely on sum_e a <m~, g~> == <out, g~>; mixing g and g~ would bias the
-        # score gradients by about 2^-8
-        out_dot_g = (out.detach() * gt[:, :F].float()).view(-1, H, F // H).sum(-1).contiguous()
-        dm = torch.zeros((M, ld), dtype=torch.float32, device=g.device)
-        ds = torch.zeros_like(s)
-        dd = torch.zeros_like(d)
-        slot_off, slot_dst = self.slot_csr(pg)
-        pack = torch.empty((pg.owned_vertices, H, 4), dtype=torch.float32, device=g.device)
-        with _timed("gat_bwd", F, 2 * pg.owned_edges, pg.owned_vertices):
-            _lib.call("nts_gat_fused_aggregate_backward_two_pass_bf16", _ptr(dm), _ptr(ds), _ptr(dd), _ptr(pack),
-                      _ptr(mt), _ptr(s), _ptr(d), _ptr(seg_max), _ptr(seg_sum), _ptr(out_dot_g), _ptr(gt),
-                      _ptr(self.slot_indices(pg)), _ptr(pg.column_offset_gpu), 0, _ptr(slot_off), _ptr(slot_dst),
-                      pg.owned_vertices, M, F, ld, H, self.slope, _stream())
-        if ld != F:
-            dm = dm[:, :F].contiguous()
-        return dm, ds, dd
+    @property
+    def _saved(self):
+        """(mirror or m~, src_score, dst_score, seg_max, seg_sum, out) of the last forward; None before the first."""
+        return None if self._k7 is None else self._k7.saved
 
     def backward(self, f_output_grad):
         pg = self._topo()
         g = _check_input(f_output_grad, "output_grad")
-        if self.gather_dtype is not None:
-            return self._backward_bf16(pg, g)
-        x, s, d, seg_max, seg_sum, out = self._saved
+        if self.two_pass_backward:
+            return self._k7.backward_two_pass(g, *self.slot_csr(pg))
+        x, s, d, seg_max, seg_sum, out = self._k7.saved
         H = int(s.shape[1])
-        D = x.shape[1] // H
-        # sum_e a[e,h] * <mirror[slot(e),h], g[d,h]> == <out[d,h], g[d,h]>: the softmax backward needs no edge pass
-        out_dot_g = (out.detach() * g).view(-1, H, D).sum(-1).contiguous()
+        out_dot_g = self._k7.out_dot_grad(g)
         dm = torch.zeros_like(x)
         ds = torch.zeros_like(s)
         dd = torch.zeros_like(d)
-        if self.two_pass_backward:
-            # no per-edge atomics: a destination-major and a source-major pass, each with register accumulators
-            slot_off, slot_dst = self.slot_csr(pg)
-            pack = torch.empty((pg.owned_vertices, H, 4), dtype=torch.float32, device=x.device)
-            with _timed("gat_bwd", x.shape[1], 2 * pg.owned_edges, pg.owned_vertices):
-                _lib.call("nts_gat_fused_aggregate_backward_two_pass", _ptr(dm), _ptr(ds), _ptr(dd), _ptr(pack),
-                          _ptr(x), _ptr(s), _ptr(d), _ptr(seg_max), _ptr(seg_sum), _ptr(out_dot_g), _ptr(g),
-                          _ptr(self.slot_indices(pg)), _ptr(pg.column_offset_gpu), 0,
-                          _ptr(slot_off), _ptr(slot_dst), pg.owned_vertices, x.shape[0], x.shape[1], H, self.slope,
-                          _stream())
-            return dm, ds, dd
         _lib.call("nts_gat_fused_aggregate_backward", _ptr(dm), _ptr(ds), _ptr(dd), _ptr(x), _ptr(s), _ptr(d),
                   _ptr(seg_max), _ptr(seg_sum), _ptr(out_dot_g), _ptr(g), _ptr(pg.row_indices_gpu),
                   _ptr(pg.column_offset_gpu), _ptr(pg.mirror_index_gpu), pg.owned_vertices, x.shape[1], H,
                   self.slope, _stream())
         return dm, ds, dd
+
+
+# the refusal of nts_gat_fused_aggregate_forward_bf16 (check_gat_bf16_layout) for a head width D % 8 != 0
+BF16_HEAD_WIDTH_ERROR = ("BF16 rows with heads > 1 need a head width D % 8 == 0 (a 16-byte chunk never straddles two "
+                         "heads) and ld == feature_size")
+
+
+class MiniBatchGATOp(ntsGraphOp):
+    """K7 on one block of a sample whose sources include its destinations (sample.NeighborSampler(...,
+    include_dst=True)): the GAT layer of DistGPUFusedGATOp with the block as topology.  Edge e of local destination d
+    reads source row row_indices[e] (local ids: the block's slots, no mirror lookup); the two-pass backward walks the
+    transposed block (row_offset, column_indices), whose edges of a source are in edge order.
+
+        forward(x_trans [n_src, H*D], src_score [n_src, H], dst_score [n_dst, H]) -> out [n_dst, H*D]
+        backward(grad_out [n_dst, H*D]) -> (d_x_trans, d_src_score, d_dst_score)
+
+    The caller forms dst_score from the destinations' own rows, x_trans[block.dst_pos]; a block without dst_pos is
+    refused.  A destination without kept edges gets a zero output row and zero gradients.  gather_dtype=torch.bfloat16
+    gathers BF16 rows with FP32 accumulation exactly as DistGPUFusedGATOp does, with the same shape limits."""
+
+    def __init__(self, sampled_subgraph, hop, negative_slope=0.2, gather_dtype=None):
+        super().__init__(sampled_subgraph, None)
+        self.hop = int(hop)
+        self.block = sampled_subgraph.blocks[self.hop]
+        if self.block.dst_pos is None:
+            raise _lib.NtsError("MiniBatchGATOp needs a block whose sources include its destinations (dst_pos): "
+                                "sample with NeighborSampler(..., include_dst=True)")
+        self.slope = float(negative_slope)
+        self.gather_dtype = _check_gather_dtype(gather_dtype)
+        self._k7 = None
+
+    def forward(self, x_trans, src_score, dst_score):
+        b = self.block
+        x = _check_input(x_trans, "x_trans")
+        s = _check_input(src_score, "src_score")
+        d = _check_input(dst_score, "dst_score")
+        if x.shape[0] != b.n_src or s.shape[0] != b.n_src:
+            raise _lib.NtsError("x_trans and src_score need %d rows (hop %d sources), got %d and %d"
+                                % (b.n_src, self.hop, x.shape[0], s.shape[0]))
+        if d.shape[0] != b.n_dst:
+            raise _lib.NtsError("dst_score needs %d rows (hop %d destinations), got %d"
+                                % (b.n_dst, self.hop, d.shape[0]))
+        H, F = int(s.shape[1]), int(x.shape[1])
+        if d.shape[1] != H or H < 1 or F % H != 0:
+            raise _lib.NtsError("scores need the same head count, and x_trans a width that is a multiple of it")
+        if b.n_edges == 0:
+            # no edge anywhere in the block: every output row is an empty sum, and no K7 entry runs.  A BF16 shape
+            # that the entries refuse (nts_gat_fused_aggregate_forward_bf16) is refused here with their words
+            if self.gather_dtype is not None and H > 1 and (F // H) % 8 != 0:
+                raise _lib.NtsError(BF16_HEAD_WIDTH_ERROR)
+            self._shapes = (x, s, d)
+            return torch.zeros((b.n_dst, F), dtype=torch.float32, device=x.device)
+        self._k7 = _FusedGAT(b.column_offset, b.row_indices, b.n_dst, b.n_src, b.n_edges, self.slope,
+                             self.gather_dtype)
+        return self._k7.forward(x, s, d)
+
+    def backward(self, f_output_grad):
+        b = self.block
+        g = _check_input(f_output_grad, "output_grad")
+        if g.shape[0] != b.n_dst:
+            raise _lib.NtsError("output_grad has %d rows, hop %d has %d destinations" % (g.shape[0], self.hop, b.n_dst))
+        if self._k7 is None:
+            x, s, d = self._shapes
+            return torch.zeros_like(x), torch.zeros_like(s), torch.zeros_like(d)
+        return self._k7.backward_two_pass(g, b.row_offset, b.column_indices)

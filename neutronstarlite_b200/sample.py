@@ -7,8 +7,12 @@ uniform subset by Floyd's algorithm on a counter hash of (seed, step, hop, desti
 destinations are hop h's distinct sources, ascending by global id.  A sample is a pure function of (graph, seed, step)
 and the seeds: it does not depend on launch configuration, batch composition or the position of a vertex in the batch.
 
-`SampledSubgraph` holds the blocks of one sample as `SampledBlock`s (device tensors); `ops.MiniBatchFuseOp`
-aggregates over them."""
+`NeighborSampler(..., include_dst=True)` (NTS_SAMPLER_INCLUDE_DST) keeps the same edges but makes every hop's sources
+include its destinations, and records each destination's position among them in `SampledBlock.dst_pos`: the block
+layout of a layer whose destinations read their own previous-layer rows (a GAT layer's destination scores).
+
+`SampledSubgraph` holds the blocks of one sample as `SampledBlock`s (device tensors); `ops.MiniBatchFuseOp` and
+`ops.MiniBatchGATOp` aggregate over them."""
 from __future__ import annotations
 
 import ctypes as C
@@ -40,12 +44,14 @@ class SampledBlock:
     dst [n_dst] global destination ids; column_offset [n_dst+1]; row_indices [n_edges] local source ids (into src);
     weight [n_edges]; src [n_src] global source ids; row_offset [n_src+1], column_indices [n_edges] (local destinations)
     and weight_backward [n_edges]: the transposed block.  row_global [n_edges] (global source ids) may be None.
+    dst_pos [n_dst] (local source index of every destination, src[dst_pos] == dst) is None unless the sources
+    include the destinations (NeighborSampler(..., include_dst=True)).
     Index arrays are int32 tensors holding uint32 values."""
 
     def __init__(self, dst, column_offset, row_indices, weight, src, row_offset=None, column_indices=None,
-                 weight_backward=None, row_global=None):
+                 weight_backward=None, row_global=None, dst_pos=None):
         self.dst, self.column_offset, self.row_indices, self.weight = dst, column_offset, row_indices, weight
-        self.src, self.row_global = src, row_global
+        self.src, self.row_global, self.dst_pos = src, row_global, dst_pos
         self.n_dst, self.n_src, self.n_edges = int(dst.numel()), int(src.numel()), int(row_indices.numel())
         if row_offset is None:
             row_offset, column_indices, weight_backward = transpose(column_offset, row_indices, weight, self.n_dst,
@@ -56,7 +62,7 @@ class SampledBlock:
         """Host copies of every array (uint32 index arrays, float32 weights)."""
         out = {}
         for name in ("dst", "column_offset", "row_indices", "row_global", "weight", "src", "row_offset",
-                     "column_indices", "weight_backward"):
+                     "column_indices", "weight_backward", "dst_pos"):
             t = getattr(self, name)
             if t is not None:
                 a = t.cpu().numpy()
@@ -92,10 +98,11 @@ class SampledSubgraph:
     @staticmethod
     def from_blocks(blocks, vertices=None):
         """From dicts of device tensors with keys dst, column_offset, row_indices (local), weight, src (sources in any
-        order) and optionally row_global; the transposed blocks are built on the device (nts_sample_transpose).
-        `vertices` (the graph's V) is needed for table gathers."""
+        order) and optionally row_global and dst_pos; the transposed blocks are built on the device
+        (nts_sample_transpose).  `vertices` (the graph's V) is needed for table gathers."""
         return SampledSubgraph([SampledBlock(b["dst"], b["column_offset"], b["row_indices"], b["weight"], b["src"],
-                                             row_global=b.get("row_global")) for b in blocks], vertices=vertices)
+                                             row_global=b.get("row_global"), dst_pos=b.get("dst_pos"))
+                                for b in blocks], vertices=vertices)
 
 
 def transpose(column_offset, row_indices, weight, n_dst, n_src):
@@ -128,9 +135,14 @@ class NeighborSampler:
     """K8 on the CSC of a single-partition graph (chunk 0's column_offset_gpu / row_indices_gpu /
     edge_weight_forward_gpu).  Device scratch for max_seeds seeds is allocated once, here.  `sample()` synchronises
     the stream once per hop; the blocks it returns are views that the next `sample()` overwrites (clone() them to keep
-    them)."""
+    them).
 
-    def __init__(self, partitioned_graph, fanout, max_seeds):
+    include_dst=True: every hop's sources include its destinations and each block carries dst_pos (module docstring);
+    the edges are those of the default mode, bit for bit."""
+
+    SAMPLER_INCLUDE_DST = 1   # NTS_SAMPLER_INCLUDE_DST of include/nts_b200.h
+
+    def __init__(self, partitioned_graph, fanout, max_seeds, include_dst=False):
         pg = partitioned_graph
         if pg.partitions != 1:
             raise _lib.NtsError("NeighborSampler needs a single-partition graph (partitions == 1), got %d"
@@ -141,15 +153,17 @@ class NeighborSampler:
             raise _lib.NtsError("the graph has no device arrays (generate_all(device=...))")
         self.V = int(pg.global_vertices)
         self.max_seeds = int(max_seeds)
+        self.include_dst = bool(include_dst)
         self.device = c.column_offset_gpu.device
         self._graph = (c.column_offset_gpu, c.row_indices_gpu, c.edge_weight_forward_gpu)
         L = _lib.load()
         ks = (C.c_int * len(self.fanout))(*self.fanout)
-        self.handle = L.nts_sampler_create(c.column_offset_gpu.data_ptr(), c.row_indices_gpu.data_ptr(),
-                                           c.edge_weight_forward_gpu.data_ptr(), self.V, int(c.edge_size),
-                                           self.max_seeds, len(self.fanout), ks, _stream())
+        self.handle = L.nts_sampler_create_ex(c.column_offset_gpu.data_ptr(), c.row_indices_gpu.data_ptr(),
+                                              c.edge_weight_forward_gpu.data_ptr(), self.V, int(c.edge_size),
+                                              self.max_seeds, len(self.fanout), ks,
+                                              self.SAMPLER_INCLUDE_DST if self.include_dst else 0, _stream())
         if not self.handle:
-            raise _lib.NtsError("nts_sampler_create failed: " + L.nts_last_error().decode(errors="replace"))
+            raise _lib.NtsError("nts_sampler_create_ex failed: " + L.nts_last_error().decode(errors="replace"))
 
     def bytes(self):
         return int(_lib.load().nts_sampler_bytes(self.handle))
@@ -190,9 +204,15 @@ class NeighborSampler:
             return torch.as_tensor(_DeviceArray(ptr, n, typestr), device=self.device)
 
         nd, ns, ne = int(v.n_dst), int(v.n_src), int(v.n_edges)
+        dst_pos = None
+        if self.include_dst:
+            p = C.c_void_p()
+            _lib.call("nts_sampler_hop_dst_pos", self.handle, int(hop), C.byref(p))
+            dst_pos = arr(p.value, nd)
         return SampledBlock(arr(v.dst, nd), arr(v.column_offset, nd + 1), arr(v.row_indices, ne),
                             arr(v.weight, ne, "<f4"), arr(v.src, ns), arr(v.row_offset, ns + 1),
-                            arr(v.column_indices, ne), arr(v.weight_backward, ne, "<f4"), arr(v.row_global, ne))
+                            arr(v.column_indices, ne), arr(v.weight_backward, ne, "<f4"), arr(v.row_global, ne),
+                            dst_pos)
 
     def __del__(self):
         try:

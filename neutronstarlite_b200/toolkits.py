@@ -8,6 +8,8 @@
   * `GATImpl`    <-> the flow of toolkits/GAT_CPU_DIST_OPTM.hpp on the fused multi-head aggregation (K7).
   * `GCNSampleImpl` <-> toolkits/GCN_CPU_SAMPLE.hpp (neighbour-sampled mini-batch GCN) on the K8 sampler and
                      ops.MiniBatchFuseOp, one GPU.
+  * `GATSampleImpl` <-> GATImpl's layers on GCNSampleImpl's batch loop: neighbour-sampled mini-batch GAT on the K8
+                     sampler (destination-inclusive blocks) and K7 through ops.MiniBatchGATOp, one GPU.
 
 Dense NN work (mm, relu, log_softmax, nll_loss, Adam element-wise) stays on torch/cuBLAS exactly as in the
 reference (libtorch); the aggregation goes through libnts_b200."""
@@ -467,3 +469,160 @@ class GATImpl:
         self.Update()
         self.epoch += 1
         return self.loss
+
+
+def _minibatch_gat_op(sampled_subgraph, active, hop, gather_dtype=None):
+    return ops.MiniBatchGATOp(sampled_subgraph, hop, gather_dtype=gather_dtype)
+
+
+class GATSampleImpl:
+    """Neighbour-sampled mini-batch multi-head GAT: GATImpl's layers on GCNSampleImpl's batch loop.  The train vertices
+    (mask == 0), in id order, are cut into batches of `batch_size` seeds; each batch is sampled with
+    NeighborSampler(..., include_dst=True), so that every hop's sources include its destinations, and runs the L layers
+    over hops L-1 .. 0.  Layer l on hop h = L-1-l takes x [n_src, in] (the features of the hop's sources for l = 0,
+    else the previous layer's output, whose rows are exactly this hop's sources), x_trans = x W_l, per-head scores
+    src = <x_trans, al_l> and dst = <x_trans[dst_pos], ar_l>, and ops.MiniBatchGATOp (K7 on the block), then relu, or
+    log_softmax on the last layer; nll_loss on the seeds, tape backward, one Adam step per parameter.  `layers` are
+    total widths and the heads split as in GATImpl (hidden layers of `heads` heads, a single-head output layer);
+    len(fanout) == len(layers) - 1.  No dropout, as in GATImpl.  gather_dtype=torch.bfloat16: K7 gathers BF16 rows
+    with FP32 accumulation (ops.MiniBatchGATOp's option; hidden head widths must then be multiples of 8).
+
+    Reproducibility: step t of a run samples with (sample_seed, t), and a block is a pure function of (graph,
+    sample_seed, t, seeds), so two runs see the same blocks bit for bit.  K7 splits the edges into quanta and finishes
+    a row cut by a quantum boundary with atomic adds onto a zeroed row; two pieces give the same bits in either order,
+    three or more may not.  The forward's quantum is a power of two of at least 32 edges (exactly 32 on small blocks:
+    it shrinks until the grid fills the GPU), the statistics' is 512 and both backward passes' 256.  So losses and
+    weights are bit-identical between runs while every fanout is at most 33 (a destination row of at most 33 edges
+    spans at most two forward quanta), no source has more than 257 out-edges in a block (the backward's source-major
+    pass), and no layer has a fallback shape of the backward (heads > 1 with a non-power-of-two head width in 4-float
+    vectors, or rows wider than 128 vectors), which adds per edge with atomics.  Beyond these limits, rows may differ
+    in the last bits between runs: fanouts of 34 to 64, hub sources of a large block (config B's deeper hops), fallback
+    shapes.  On one H100, two Cora runs (1433-64-7, 8 heads, fanout 10-10, batch 64; the largest source has 17
+    out-edges in a block) gave bit-identical losses and weights over three epochs with FP32 and with BF16 gathers
+    (DESIGN.md §3 K8)."""
+
+    def __init__(self, partitioned_graph, layers, features, labels, mask, fanout, batch_size, heads=8,
+                 learn_rate=0.01, weight_decay=0.0001, decay_rate=0.97, decay_epoch=100, seed=0, sample_seed=0,
+                 gather_dtype=None):
+        self.layers = list(layers)
+        if len(fanout) != len(self.layers) - 1:
+            raise _lib.NtsError("fanout needs one entry per layer (%d), got %d" % (len(self.layers) - 1, len(fanout)))
+        self.batch_size = int(batch_size)
+        if self.batch_size < 1:
+            raise _lib.NtsError("batch_size must be >= 1")
+        self.gather_dtype = ops._check_gather_dtype(gather_dtype)
+        self.heads = [heads] * (len(self.layers) - 2) + [1]
+        for i, H in enumerate(self.heads):
+            if self.layers[i + 1] % H:
+                raise _lib.NtsError("layer width %d is not a multiple of %d heads" % (self.layers[i + 1], H))
+        from .sample import NeighborSampler
+        self.sampler = NeighborSampler(partitioned_graph, fanout, self.batch_size, include_dst=True)
+        self.device = features.device
+        self.sample_seed = int(sample_seed)
+        self.step = 0
+        self.ctx = NtsContext()
+        gen = torch.Generator().manual_seed(seed)
+        self.P, self.al, self.ar = [], [], []
+        for i in range(len(self.layers) - 1):
+            H = self.heads[i]
+            D = self.layers[i + 1] // H
+            for lst, shape in ((self.P, (self.layers[i], H * D)), (self.al, (H, D)), (self.ar, (H, D))):
+                prm = Parameter(*shape, learn_rate, 0.9, 0.999, 1e-9, weight_decay, device=self.device, generator=gen)
+                prm.init_parameter()
+                prm.set_decay(decay_rate, decay_epoch)
+                lst.append(prm)
+        self.features = ops._check_input(features.detach(), "features")
+        self.L_GT = labels.to(self.device)
+        mask = torch.as_tensor(mask).cpu()
+        self.nids = [(mask == s).nonzero().view(-1) for s in (0, 1, 2)]    # train / val / test ids, ascending
+        self.subgraph = None
+        self.loss = None
+        self.epoch = 0
+
+    def params(self):
+        return self.P + self.al + self.ar
+
+    def Forward(self, seeds):
+        """Sample the batch and run the layers; returns the last layer's [n_seeds, classes] log-probabilities."""
+        self.subgraph = sg = self.sampler.sample(seeds, self.sample_seed, self.step)
+        self.step += 1
+        ctx = self.ctx
+        L = len(self.layers) - 1
+        x = None
+        for l in range(L):
+            hop = L - 1 - l
+            b = sg.blocks[hop]
+            H = self.heads[l]
+            D = self.layers[l + 1] // H
+            if l == 0:
+                x = self.features.index_select(0, b.src.long())
+            x_trans = ctx.runVertexForward(lambda t, _l=l: self.P[_l].forward(t), x)
+            # the destination score reads the destinations' own rows; it is recorded before the source score, whose
+            # input x_trans would otherwise chain onto x_trans's own tape entry (NtsContext.appendNNOp) and leave
+            # d_x_trans without a producer to go to
+            x_dst = x_trans.index_select(0, b.dst_pos.long())
+            dst_att = ctx.runVertexForward(
+                lambda t, _l=l, _H=H, _D=D: (t.view(-1, _H, _D) * self.ar[_l].W).sum(-1).contiguous(), x_dst)
+            src_att = ctx.runVertexForward(
+                lambda t, _l=l, _H=H, _D=D: (t.view(-1, _H, _D) * self.al[_l].W).sum(-1).contiguous(), x_trans)
+            nbr = ctx.runGraphOpN(_minibatch_gat_op, sg, None, [x_trans, src_att, dst_att], hop=hop,
+                                  gather_dtype=self.gather_dtype)
+            if l == L - 1:
+                x = ctx.runVertexForward(lambda t: t.log_softmax(1), nbr)
+            else:
+                x = ctx.runVertexForward(lambda t: torch.relu(t), nbr)
+        return x
+
+    def Loss(self, out, seeds_dev):
+        self.loss = torch.nn.functional.nll_loss(out, self.L_GT.index_select(0, seeds_dev))
+        self.ctx.appendNNOp(out, self.loss)
+        return self.loss
+
+    def Update(self):
+        for p in self.params():
+            if p.W.grad is None:
+                continue
+            p.all_reduce_to_gradient(p.W.grad)
+            p.learn_with_decay_Adam()
+            p.next()
+
+    def train_step(self, seeds):
+        """One batch: zero the gradients, sample, forward, loss, tape backward, Adam.  Returns (loss, correct)."""
+        for p in self.params():
+            p.zero_grad()
+        self.ctx.train()
+        out = self.Forward(seeds)
+        seeds_dev = self.subgraph.seeds().long()
+        loss = self.Loss(out, seeds_dev)
+        correct = (out.argmax(1) == self.L_GT.index_select(0, seeds_dev)).sum()
+        # the three NN segments of a layer share x_trans's autograd graph: keep it until the last of them has run
+        self.ctx.self_backward(True)
+        self.Update()
+        return loss.detach(), correct
+
+    def evaluate(self, s):
+        """Accuracy over mask == s from sampled forwards (no update)."""
+        self.ctx.eval()
+        correct = torch.zeros((), dtype=torch.int64, device=self.device)
+        ids = self.nids[s]
+        with torch.no_grad():
+            for b in range(0, ids.numel(), self.batch_size):
+                out = self.Forward(ids[b:b + self.batch_size])
+                correct += (out.argmax(1) == self.L_GT.index_select(0, self.subgraph.seeds().long())).sum()
+        self.ctx.train()
+        return float(correct) / max(ids.numel(), 1)
+
+    def run_epoch(self, test=True):
+        """One pass over the train batches (one Adam step each) and, with test=True, sampled validation and test
+        forwards.  Returns (mean train loss, [train, val, test] accuracy) - val / test are None with test=False."""
+        ids = self.nids[0]
+        losses, correct = [], torch.zeros((), dtype=torch.int64, device=self.device)
+        for b in range(0, ids.numel(), self.batch_size):
+            loss, c = self.train_step(ids[b:b + self.batch_size])
+            losses.append(loss)
+            correct += c
+        mean_loss = float(torch.stack(losses).mean()) if losses else float("nan")
+        acc = [float(correct) / max(ids.numel(), 1)]
+        acc += [self.evaluate(1), self.evaluate(2)] if test else [None, None]
+        self.epoch += 1
+        return mean_loss, acc
