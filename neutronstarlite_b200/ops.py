@@ -786,6 +786,22 @@ BF16_HEAD_WIDTH_ERROR = ("BF16 rows with heads > 1 need a head width D % 8 == 0 
                          "heads) and ld == feature_size")
 
 
+def gat_bf16_shape_error(feature_size, heads):
+    """Why the BF16 K7 entries refuse a layer of feature_size = heads * D columns (gathered as rows of
+    ld = ceil(F/8)*8 BF16 values, as _FusedGAT does), or None when both accept it.  The entries give the verdict
+    themselves: both check layout and shape before their batch_size == 0 return, so a call with batch 0 and null
+    pointers does no device work.  Returns "<entry>: <its error message>"."""
+    F, H = int(feature_size), int(heads)
+    ld = (F + 7) // 8 * 8
+    lib = _lib.load()
+    # (pointers, then batch 0 and 0 edges / mirror rows, F, ld, H, slope, stream)
+    for name, n_ptrs in (("nts_gat_fused_aggregate_forward_bf16", 9),
+                         ("nts_gat_fused_aggregate_backward_two_pass_bf16", 16)):
+        if getattr(lib, name)(*([None] * n_ptrs), 0, 0, F, ld, H, 0.2, None) != 0:
+            return "%s: %s" % (name, lib.nts_last_error().decode(errors="replace"))
+    return None
+
+
 class MiniBatchGATOp(ntsGraphOp):
     """K7 on one block of a sample whose sources include its destinations (sample.NeighborSampler(...,
     include_dst=True)): the GAT layer of DistGPUFusedGATOp with the block as topology.  Edge e of local destination d

@@ -376,7 +376,8 @@ class GATImpl:
 
     gather_dtype=torch.bfloat16 (needs fused_kernel=True and two_pass_backward=True): every fused layer gathers BF16
     mirror and gradient rows with FP32 accumulation (ops.DistGPUFusedGATOp's option).  The input features stay float32
-    (they feed the first GEMM), and so do the mirror fetch, activations, weights and gradients."""
+    (they feed the first GEMM), and so do the mirror fetch, activations, weights and gradients.  A layer shape that
+    either BF16 entry refuses (ops.gat_bf16_shape_error: e.g. 8 heads x 24) raises NtsError at construction."""
 
     def __init__(self, partitioned_graph, layers, features, labels, mask, heads=8, learn_rate=0.01,
                  weight_decay=0.0001, exchange=None, seed=0, sum_fanout_grads=True, fused_kernel=False,
@@ -390,6 +391,8 @@ class GATImpl:
         self.layers = list(layers)
         self.device = features.device
         self.heads = [heads] * (len(self.layers) - 2) + [1]
+        if self.gather_dtype is not None:
+            _refuse_bf16_gat_layers(self.layers, self.heads)
         self.ctx = NtsContext(sum_fanout_grads=sum_fanout_grads)
         gen = torch.Generator().manual_seed(seed)
         self.P, self.al, self.ar = [], [], []
@@ -471,6 +474,16 @@ class GATImpl:
         return self.loss
 
 
+def _refuse_bf16_gat_layers(layers, heads):
+    """NtsError, before any device work, for the first layer whose shape a BF16 K7 entry refuses (the backward has no
+    fallback, so such a layer would otherwise run a whole forward and fail at its first backward)."""
+    for i, H in enumerate(heads):
+        why = ops.gat_bf16_shape_error(layers[i + 1], H)
+        if why is not None:
+            raise _lib.NtsError("layer %d (width %d, %d heads) cannot gather BF16 rows: %s"
+                                % (i, layers[i + 1], H, why))
+
+
 def _minibatch_gat_op(sampled_subgraph, active, hop, gather_dtype=None):
     return ops.MiniBatchGATOp(sampled_subgraph, hop, gather_dtype=gather_dtype)
 
@@ -485,7 +498,8 @@ class GATSampleImpl:
     log_softmax on the last layer; nll_loss on the seeds, tape backward, one Adam step per parameter.  `layers` are
     total widths and the heads split as in GATImpl (hidden layers of `heads` heads, a single-head output layer);
     len(fanout) == len(layers) - 1.  No dropout, as in GATImpl.  gather_dtype=torch.bfloat16: K7 gathers BF16 rows
-    with FP32 accumulation (ops.MiniBatchGATOp's option; hidden head widths must then be multiples of 8).
+    with FP32 accumulation (ops.MiniBatchGATOp's option; hidden head widths must then be multiples of 8, and a layer
+    shape that either BF16 entry refuses raises NtsError at construction, as in GATImpl).
 
     Reproducibility: step t of a run samples with (sample_seed, t), and a block is a pure function of (graph,
     sample_seed, t, seeds), so two runs see the same blocks bit for bit.  K7 splits the edges into quanta and finishes
@@ -515,6 +529,8 @@ class GATSampleImpl:
         for i, H in enumerate(self.heads):
             if self.layers[i + 1] % H:
                 raise _lib.NtsError("layer width %d is not a multiple of %d heads" % (self.layers[i + 1], H))
+        if self.gather_dtype is not None:
+            _refuse_bf16_gat_layers(self.layers, self.heads)
         from .sample import NeighborSampler
         self.sampler = NeighborSampler(partitioned_graph, fanout, self.batch_size, include_dst=True)
         self.device = features.device

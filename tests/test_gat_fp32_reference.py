@@ -211,10 +211,10 @@ def layer_inputs(M, V, H, D, seed, score=2.0, device="cpu"):
             mk(rng.uniform(-score, score, (V, H))), mk(rng.uniform(-1, 1, (V, F))))
 
 
-def run_k7(pg, mirror, s, d, g, slope, two_pass):
+def run_k7(pg, mirror, s, d, g, slope, two_pass, gather_dtype=None):
     """(out, dm, ds, dd), (seg_max, seg_sum) and the forward's launch record (grid, block, smem, variant)."""
     from neutronstarlite_b200 import _lib, ops
-    op = ops.DistGPUFusedGATOp(pg, negative_slope=slope, two_pass_backward=two_pass)
+    op = ops.DistGPUFusedGATOp(pg, negative_slope=slope, two_pass_backward=two_pass, gather_dtype=gather_dtype)
     out = op.forward(mirror, s, d)
     rec = [ctypes.c_int() for _ in range(4)]
     _lib.call("nts_aggregate_last_launch", *[ctypes.byref(r) for r in rec])
