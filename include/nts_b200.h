@@ -116,28 +116,31 @@ int nts_segment_gather_sum_range(const float *input, float *output, const float 
 typedef struct nts_gather_plan nts_gather_plan;
 int nts_gather_plan_pick_slabs(nts_vid_t gather_rows, uint64_t n_edges, nts_vid_t n_rows, nts_vid_t feature_size,
                                uint64_t l2_budget_bytes /* 0 = default */);
-nts_gather_plan *nts_gather_plan_create(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
-                                        const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows,
-                                        uint64_t n_edges, nts_vid_t gather_rows, int n_slabs, void *stream);
-/* The same with up to two dense FP32 hub blocks beside the slab-bucketed residual: the n_hub_cols most referenced
- * gathered rows (ties: smaller id) become a column block [n_rows x n_hub_cols] that takes every edge gathering one of
- * them, the n_hub_rows longest output rows a row block [n_hub_rows x gather_rows] that takes their remaining edges;
- * each dense cell holds the sum of its edges' weights.  A run computes the blocks as GEMMs before the slab launches.
- * Counts above the rows available are clamped (nts_gather_plan_hubs reports the result); 0, 0 = nts_gather_plan_create. */
+/* A plan of one chunk with up to two dense FP32 hub blocks beside the slab-bucketed residual: the n_hub_cols most
+ * referenced gathered rows (ties: smaller id) become a column block [n_rows x n_hub_cols] that takes every edge
+ * gathering one of them, the n_hub_rows longest output rows a row block [n_hub_rows x gather_rows] that takes their
+ * remaining edges; each dense cell holds the sum of its edges' weights.  A run computes the blocks as GEMMs before the
+ * slab launches.  Counts above the rows available are clamped (nts_gather_plan_hubs reports the result); 0, 0 = no
+ * hub blocks. */
 nts_gather_plan *nts_gather_plan_create_hybrid(const nts_vid_t *offsets, const nts_vid_t *indices,
                                                const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
                                                nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows, int n_slabs,
                                                int n_hub_cols, int n_hub_rows, void *stream);
-/* slab count chosen by MEASUREMENT on the real arrays at this feature width (candidates 1, 2, 4, ... built and timed
- * once; hub-dominated graphs prefer no bucketing, uniform ones 8-16 slabs), then the hub counts of
- * nts_gather_plan_create_hybrid the same way among rows dense enough to be candidates (NTS_PLAN_HUBS=0: none) */
-nts_gather_plan *nts_gather_plan_create_tuned(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
-                                              const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows,
-                                              uint64_t n_edges, nts_vid_t gather_rows, nts_vid_t feature_size,
-                                              void *stream);
+/* A plan of one chunk with the slab count chosen by MEASUREMENT on the real arrays at this feature width (candidates
+ * 1, 2, 4, ... built and timed once; hub-dominated graphs prefer no bucketing, uniform ones 8-16 slabs), then the hub
+ * counts of nts_gather_plan_create_hybrid the same way among rows dense enough to be candidates (NTS_PLAN_HUBS=0:
+ * none).  The candidates are timed as gathers of gather_dtype: NTS_DTYPE_F32, or NTS_DTYPE_BF16 (BF16 rows; the L2
+ * slab bound counts 2-byte rows), in the run mode the plan will be used in: run_flags 0 (accumulate) or
+ * NTS_PLAN_OVERWRITE. */
+nts_gather_plan *nts_gather_plan_create_tuned_ex(const nts_vid_t *offsets, const nts_vid_t *indices,
+                                                 const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
+                                                 nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows,
+                                                 nts_vid_t feature_size, int gather_dtype, int run_flags,
+                                                 void *stream);
 /* Several chunks merged into ONE plan: part-local output row r becomes row_add + r, a mapped index g becomes index_add
  * + g; inside a (slab, row) segment the parts follow each other in the order given.  n_slabs = 0 measures the slab
- * count for feature_size.  Used by the exchange engine to aggregate all remote chunks of a rank in one launch. */
+ * count for feature_size on accumulating FP32 gathers.  Merged plans have no hub blocks.  Used by the exchange engine
+ * to aggregate all remote chunks of a rank in one launch. */
 typedef struct nts_plan_part {
   const nts_vid_t *offsets, *indices;   /* [n_rows+1], [n_edges] of this part */
   const float *weight;                  /* [n_edges] or NULL */
@@ -157,10 +160,8 @@ int nts_gather_plan_hubs(const nts_gather_plan *plan, int *cols, int *rows); /* 
 int nts_gather_plan_overlap(const nts_gather_plan *plan);
 int nts_gather_plan_set_overlap(nts_gather_plan *plan, int overlap);
 uint64_t nts_gather_plan_bytes(const nts_gather_plan *plan);
-/* output[r,:] += sum_e input[row(e),:] * w(e)   (accumulates; one launch per non-empty slab, in stream order) */
-int nts_gather_plan_run(nts_gather_plan *plan, const float *input, float *output, nts_vid_t feature_size,
-                        void *stream);
 /* Run flags of the _ex entries.
+ * NTS_PLAN_ACCUMULATE (0): output[r,:] += sum_e input[row(e),:] * w(e), one launch per non-empty slab, in stream order.
  * NTS_PLAN_OVERWRITE: output[r,:] = sum_e ... instead of +=; output may hold anything before the call (NaN included).
  *   The hub column block, which covers every output element and runs first, stores instead of adding; a plan without
  *   hub columns zeroes the output first.  Each element gets the value an accumulating run into zeros gives, up to the
@@ -168,7 +169,7 @@ int nts_gather_plan_run(nts_gather_plan *plan, const float *input, float *output
  * NTS_PLAN_COPY_INPUT: gather from a zero-padded copy of the input even where it could be gathered in place (for an
  *   input whose storage ends before the last row's input_ld-th value). */
 enum { NTS_PLAN_ACCUMULATE = 0, NTS_PLAN_OVERWRITE = 1, NTS_PLAN_COPY_INPUT = 2 };
-/* nts_gather_plan_run on input rows of pitch input_ld floats (>= feature_size).  The input is gathered in place when
+/* Run a plan on input rows of pitch input_ld floats (>= feature_size).  The input is gathered in place when
  * input_ld % 4 == 0 and it is 16-byte aligned: the gather then reads all input_ld values of every row, the last one
  * included, and never writes values past feature_size to an output.  Otherwise its rows are copied into the plan's
  * zero-padded workspace first (the copy reads feature_size values per row).  The output keeps the pitch
@@ -176,32 +177,16 @@ enum { NTS_PLAN_ACCUMULATE = 0, NTS_PLAN_OVERWRITE = 1, NTS_PLAN_COPY_INPUT = 2 
 int nts_gather_plan_run_ex(nts_gather_plan *plan, const float *input, nts_vid_t input_ld, float *output,
                            nts_vid_t feature_size, int flags, void *stream);
 int nts_gather_plan_last_launch(const nts_gather_plan *plan, int *launches, int *grid, int *k, int *u, int *outv);
-/* BF16 gathers with FP32 accumulation: output[r,:] += sum_e w(e) * float(bf16(input[row(e),:])).  bf16() rounds to
- * nearest even (what torch's x.to(torch.bfloat16) computes, incl. inf, NaN and subnormals); weights, accumulation
- * and output stay FP32.  An NTS_DTYPE_F32 input is converted once per call into the plan's BF16 workspace (rows
- * padded to a multiple of 8 values); an NTS_DTYPE_BF16 input is gathered in place when feature_size % 8 == 0 and it
- * is 16-byte aligned, else re-strided into the workspace.  Hub blocks read BF16 rows and compute in FP32.  Returns an
- * error under nts_gather_plan_set_variant(1) (the TMA row-staging variant is FP32 only). */
+/* BF16 gathers with FP32 accumulation: output[r,:] += sum_e w(e) * float(bf16(input[row(e),:])) (or = with
+ * NTS_PLAN_OVERWRITE).  bf16() rounds to nearest even (what torch's x.to(torch.bfloat16) computes, incl. inf, NaN and
+ * subnormals); weights, accumulation and output stay FP32.  Input rows of pitch input_ld elements of input_dtype:
+ * an NTS_DTYPE_F32 input is converted once per call into the plan's BF16 workspace (rows padded to a multiple of 8
+ * values); an NTS_DTYPE_BF16 input is gathered in place when input_ld % 8 == 0 and it is 16-byte aligned, else
+ * re-strided into the workspace.  Flags as for nts_gather_plan_run_ex.  Hub blocks read BF16 rows and compute in
+ * FP32.  Returns an error under nts_gather_plan_set_variant(1) (the TMA row-staging variant is FP32 only). */
 enum { NTS_DTYPE_F32 = 0, NTS_DTYPE_BF16 = 1 };
-int nts_gather_plan_run_bf16(nts_gather_plan *plan, const void *input, int input_dtype, float *output,
-                             nts_vid_t feature_size, void *stream);
-/* nts_gather_plan_run_bf16 on input rows of pitch input_ld elements of input_dtype, with the flags of
- * nts_gather_plan_run_ex (a BF16 input is gathered in place when input_ld % 8 == 0 and it is 16-byte aligned) */
 int nts_gather_plan_run_bf16_ex(nts_gather_plan *plan, const void *input, int input_dtype, nts_vid_t input_ld,
                                 float *output, nts_vid_t feature_size, int flags, void *stream);
-/* nts_gather_plan_create_tuned with the candidates timed as BF16 gathers (and the L2 slab bound counting 2-byte rows):
- * the slab and hub counts that suit BF16 rows of this width */
-nts_gather_plan *nts_gather_plan_create_tuned_bf16(const nts_vid_t *offsets, const nts_vid_t *indices,
-                                                   const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
-                                                   nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows,
-                                                   nts_vid_t feature_size, void *stream);
-/* nts_gather_plan_create_tuned (gather_dtype NTS_DTYPE_F32) or _bf16 (NTS_DTYPE_BF16) with the candidates timed in
- * the run mode the plan will be used in: run_flags 0 (accumulate) or NTS_PLAN_OVERWRITE */
-nts_gather_plan *nts_gather_plan_create_tuned_ex(const nts_vid_t *offsets, const nts_vid_t *indices,
-                                                 const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
-                                                 nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows,
-                                                 nts_vid_t feature_size, int gather_dtype, int run_flags,
-                                                 void *stream);
 int nts_gather_plan_set_tuning(int u, int min_blocks, int edges_per_warp); /* measurement hook, 0 = default */
 /* 0 = gathered rows through registers (default); 1 = rows staged in shared memory by per-row cp.async.bulk (TMA) into
  * a per-warp ring, U of set_tuning = ring depth - the north star's "feature tiles via TMA", kept for measurement */
@@ -357,7 +342,7 @@ int nts_gat_fused_aggregate_backward_two_pass_bf16(float *mirror_grad, float *sr
                                                    nts_vid_t heads, float negative_slope, void *stream);
 /* dst[r, 0:ld] = {bf16(src[r, 0:feature_size]), 0 ...} for n_rows rows of stride lds (elements of src_dtype,
  * NTS_DTYPE_F32 rounded to nearest even, NTS_DTYPE_BF16 copied); ld % 8 == 0, ld >= feature_size, dst 16-byte aligned.
- * The conversion pass of nts_gather_plan_run_bf16, exported for the BF16 rows of the K7 entries above. */
+ * The conversion pass of nts_gather_plan_run_bf16_ex, exported for the BF16 rows of the K7 entries above. */
 int nts_rows_to_bf16(const void *src, int src_dtype, nts_vid_t lds, void *dst, nts_vid_t n_rows, nts_vid_t feature_size,
                      nts_vid_t ld, void *stream);
 
@@ -468,7 +453,7 @@ int nts_exchange_open_peers(nts_exchange *ex, const unsigned char *window_handle
 int nts_exchange_forward(nts_exchange *ex, const float *x, float *y, nts_vid_t feature_size, void *stream);
 /* dX_p += sum_j A_{j<-p}^T dY_j (ForwardGPUfuseOp::backward, :75-90); dx zeroed by caller */
 int nts_exchange_backward(nts_exchange *ex, const float *g, float *dx, nts_vid_t feature_size, void *stream);
-/* BF16 gathers with FP32 accumulation (the contract of nts_gather_plan_run_bf16) across partitions.  Forward: the
+/* BF16 gathers with FP32 accumulation (the contract of nts_gather_plan_run_bf16_ex) across partitions.  Forward: the
  * sender rounds its X (NTS_DTYPE_F32, or NTS_DTYPE_BF16 used as is when F % 8 == 0 and 16-byte aligned) once per call
  * into BF16 rows of stride ceil(F/8)*8 and pushes them (half the bytes), every chunk gathers BF16 rows.  Backward: dY
  * is rounded once locally; partial gradients are computed, pushed and added in FP32.  Every chunk runs through a plan

@@ -50,9 +50,7 @@ SIGNATURES = {
     "nts_gather_by_src_from_dst": (_int, [_vp, _vp, _vp, _vp, _vp, _u32, _u32, _u32, _u32, _u32, _u32, _u32, _int, _vp]),
     "nts_segment_gather_sum_range": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _u64, _u64, _u32, _vp]),
     "nts_gather_plan_pick_slabs": (_int, [_u32, _u64, _u32, _u32, _u64]),
-    "nts_gather_plan_create": (_vp, [_vp, _vp, _vp, _vp, _u32, _u32, _u64, _u32, _int, _vp]),
     "nts_gather_plan_create_hybrid": (_vp, [_vp, _vp, _vp, _vp, _u32, _u32, _u64, _u32, _int, _int, _int, _vp]),
-    "nts_gather_plan_create_tuned": (_vp, [_vp, _vp, _vp, _vp, _u32, _u32, _u64, _u32, _u32, _vp]),
     "nts_gather_plan_create_parts": (_vp, [_vp, _int, _u32, _u32, _int, _u32, _vp]),
     "nts_gather_plan_tuned_ms": (C.c_float, [_vp]),
     "nts_gather_plan_destroy": (_int, [_vp]),
@@ -61,11 +59,8 @@ SIGNATURES = {
     "nts_gather_plan_overlap": (_int, [_vp]),
     "nts_gather_plan_set_overlap": (_int, [_vp, _int]),
     "nts_gather_plan_bytes": (_u64, [_vp]),
-    "nts_gather_plan_run": (_int, [_vp, _vp, _vp, _u32, _vp]),
-    "nts_gather_plan_run_bf16": (_int, [_vp, _vp, _int, _vp, _u32, _vp]),
     "nts_gather_plan_run_ex": (_int, [_vp, _vp, _u32, _vp, _u32, _int, _vp]),
     "nts_gather_plan_run_bf16_ex": (_int, [_vp, _vp, _int, _u32, _vp, _u32, _int, _vp]),
-    "nts_gather_plan_create_tuned_bf16": (_vp, [_vp, _vp, _vp, _vp, _u32, _u32, _u64, _u32, _u32, _vp]),
     "nts_gather_plan_create_tuned_ex": (_vp, [_vp, _vp, _vp, _vp, _u32, _u32, _u64, _u32, _u32, _int, _int, _vp]),
     "nts_gather_plan_last_launch": (_int, [_vp] + [C.POINTER(_int)] * 5),
     "nts_gather_plan_set_tuning": (_int, [_int, _int, _int]),

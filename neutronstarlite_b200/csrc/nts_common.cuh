@@ -7,6 +7,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <functional>
+
 #include "nts_b200.h"
 
 namespace nts {
@@ -51,9 +53,15 @@ inline bool aligned_to(const void *p, size_t a) { return (reinterpret_cast<uintp
 
 int sm_count();
 
-// BF16 gathers of nts_plan.cu for the exchange engine: rows of an explicit stride (lds elements of the input type),
-// and the conversion pass that writes BF16 rows of stride ld (ld % 8 == 0, zero past F, dst 16-byte aligned);
-// flags as for nts_gather_plan_run_bf16_ex (0: accumulate)
+// Minimum of two timed run() calls after one warm-up call, with CUDA events on st (synchronises).  Returns run()'s
+// error, or nonzero when an event call fails.
+int time_min_of_two(const std::function<int()> &run, cudaStream_t st, float *ms);
+
+// Gathers of nts_plan.cu for the exchange engine, on rows of an explicit stride (lds elements of the input type);
+// flags as for nts_gather_plan_run_ex / _run_bf16_ex (0: accumulate).  FP32 rows, and BF16 gathers of FP32 or BF16
+// rows.  Plus the conversion pass that writes BF16 rows of stride ld (ld % 8 == 0, zero past F, dst 16-byte aligned).
+int run_plan(nts_gather_plan *pl, const float *input, uint32_t lds, float *output, uint32_t F, int flags,
+             cudaStream_t st);
 int run_plan_bf16(nts_gather_plan *pl, const void *input, int dtype, uint32_t lds, float *output, uint32_t F,
                   cudaStream_t st, int flags = 0);
 int to_bf16_rows(const void *src, int dtype, uint32_t lds, void *dst, uint32_t n_rows, uint32_t F, uint32_t ld,
@@ -92,9 +100,10 @@ __device__ __forceinline__ float4 widen(uint2 u) {
 }
 __device__ __forceinline__ float8v widen(uint4 u) { return {widen(make_uint2(u.x, u.y)), widen(make_uint2(u.z, u.w))}; }
 
-} // namespace nts
+// A plan of parts (checked by the caller) with its slab count, and with hubs_allowed (a single part) its hub counts
+// and schedule, chosen by timing candidates for width feature_size in run mode run_flags (0 or NTS_PLAN_OVERWRITE),
+// as FP32 gathers or, with bf16, as BF16 gathers of BF16 rows (nts_plan.cu)
+nts_gather_plan *tune_plan(const nts_plan_part *parts, int n_parts, nts_vid_t n_rows, nts_vid_t gather_rows,
+                           nts_vid_t feature_size, bool bf16, int run_flags, bool hubs_allowed, cudaStream_t st);
 
-// nts_gather_plan_create_parts with the slab count measured on BF16 gathers when bf16 != 0 (nts_plan.cu)
-extern "C" nts_gather_plan *nts_plan_create_parts_typed(const nts_plan_part *parts, int n_parts, nts_vid_t n_rows,
-                                                        nts_vid_t gather_rows, int n_slabs, nts_vid_t feature_size,
-                                                        int bf16, void *stream);
+} // namespace nts

@@ -389,8 +389,8 @@ static int aggregate_chunk(nts_exchange *ex, int i, bool forward, const void *in
       if (e.first == plan_key(F, gt.bf16))
         pl = e.second;
     if (!pl) { // first use of this width and type: slab and hub counts by measurement, built once and kept
-      pl = gt.bf16 ? nts_gather_plan_create_tuned_bf16(off, idx, w, nullptr, base, n_rows, c.edges, gather_rows, F, st)
-                   : nts_gather_plan_create_tuned(off, idx, w, nullptr, base, n_rows, c.edges, gather_rows, F, st);
+      const nts_plan_part pt = {off, idx, w, nullptr, base, 0, n_rows, 0, c.edges};
+      pl = tune_plan(&pt, 1, n_rows, gather_rows, F, gt.bf16, 0, true, st);
       if (!pl)
         return -1;
       int hc = 0, hr = 0, ehc = 0, ehr = 0;
@@ -406,31 +406,9 @@ static int aggregate_chunk(nts_exchange *ex, int i, bool forward, const void *in
     }
     if (gt.bf16)
       return run_plan_bf16(pl, in_rows, NTS_DTYPE_BF16, gt.ld, out, F, st);
-    return nts_gather_plan_run(pl, in, out, F, st);
+    return run_plan(pl, in, F, out, F, 0, st);
   }
   return nts_segment_gather_sum(in, out, w, idx, off, base, n_rows, c.edges, F, st);
-}
-
-// min of 2 timed launches after 1 warm one (CUDA events on st; synchronises)
-template <class Fn> static int time_launches(Fn run, cudaStream_t st, float *ms) {
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  NTS_CUDA_OK(cudaEventCreate(&e0));
-  NTS_CUDA_OK(cudaEventCreate(&e1));
-  *ms = 1e30f;
-  int rc = 0;
-  for (int it = 0; it < 3 && !rc; it++) {
-    float t = 0.f;
-    if (cudaEventRecord(e0, st) != cudaSuccess || (rc = run()) != 0 || cudaEventRecord(e1, st) != cudaSuccess ||
-        cudaEventSynchronize(e1) != cudaSuccess || cudaEventElapsedTime(&t, e0, e1) != cudaSuccess) {
-      rc = rc ? rc : -1;
-      break;
-    }
-    if (it > 0 && t < *ms)
-      *ms = t;
-  }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  return rc;
 }
 
 // Pipeline or merged?  One launch per source partition hides the transfer behind the earlier chunks, but small
@@ -484,7 +462,7 @@ static int decide_mode(nts_exchange *ex, bool forward, uint32_t F, cudaStream_t 
     parts.push_back(pt);
   }
   const uint32_t out_rows = forward ? Vp : ex->recv_total, in_rows = forward ? ex->recv_total : Vp;
-  m.merged = nts_plan_create_parts_typed(parts.data(), (int)parts.size(), out_rows, in_rows, 0, F, gt.bf16, st);
+  m.merged = tune_plan(parts.data(), (int)parts.size(), out_rows, in_rows, F, gt.bf16, 0, false, st);
   if (!m.merged)
     return -1;
   if (ex->forced_mode == 2) {
@@ -503,16 +481,16 @@ static int decide_mode(nts_exchange *ex, bool forward, uint32_t F, cudaStream_t 
   cudaMemsetAsync(a, 0, a_bytes, st);
   cudaMemsetAsync(b, 0, rows_max * F * sizeof(float), st);
   float L = 0.f, M = 0.f, sum_c = 0.f;
-  int rc = time_launches([&]() { return aggregate_chunk(ex, p, forward, a, b, F, st, gt); }, st, &L);
+  int rc = time_min_of_two([&]() { return aggregate_chunk(ex, p, forward, a, b, F, st, gt); }, st, &L);
   if (!rc)
-    rc = time_launches([&]() {
-      return gt.bf16 ? run_plan_bf16(m.merged, a, NTS_DTYPE_BF16, gt.ld, b, F, st) : nts_gather_plan_run(m.merged, a, b, F, st);
+    rc = time_min_of_two([&]() {
+      return gt.bf16 ? run_plan_bf16(m.merged, a, NTS_DTYPE_BF16, gt.ld, b, F, st) : run_plan(m.merged, a, F, b, F, 0, st);
     }, st, &M);
   for (int i = 0; i < P && !rc; i++) {
     if (i == p || !ex->chunks[i].edges || !ex->need_count[i])
       continue;
     float c = 0.f;
-    rc = time_launches([&]() { return aggregate_chunk(ex, i, forward, a, b, F, st, gt); }, st, &c);
+    rc = time_min_of_two([&]() { return aggregate_chunk(ex, i, forward, a, b, F, st, gt); }, st, &c);
     sum_c += c;
   }
   cudaFree(a);
@@ -817,7 +795,7 @@ static int forward_impl(nts_exchange *ex, const void *x_in, int x_dtype, float *
   NTS_ARG_CHECK(d.owned_vertices == 0 || (x && y), "null feature pointer");
   cudaStream_t st = as_stream(stream);
   const int P = ex->P, p = ex->p;
-  NTS_ARG_CHECK(!bf16 || P > 1, "BF16 gathers on one partition run through nts_gather_plan_run_bf16");
+  NTS_ARG_CHECK(!bf16 || P > 1, "BF16 gathers on one partition run through nts_gather_plan_run_bf16_ex");
   if (P == 1)
     return nts_gather_by_dst_from_src(x, y, d.local_weight_forward, d.local_row_indices, d.local_column_offset,
                                       d.dst_start, d.dst_start + d.owned_vertices, d.dst_start,
@@ -865,7 +843,7 @@ static int forward_impl(nts_exchange *ex, const void *x_in, int x_dtype, float *
     if (bf16)
       NTS_TRY(run_plan_bf16(mode->merged, ex->window + buf, NTS_DTYPE_BF16, gt.ld, y, F, st));
     else
-      NTS_TRY(nts_gather_plan_run(mode->merged, ex->window + buf, y, F, st));
+      NTS_TRY(run_plan(mode->merged, ex->window + buf, F, y, F, 0, st));
     if (tr)
       for (int s = 1; s < P; s++) { // the merged launch is reported under ring step 1, the other steps read 0
         NTS_CUDA_OK(cudaEventRecord(ex->tev[5 + 2 * (s - 1)], st));
@@ -898,7 +876,7 @@ static int backward_impl(nts_exchange *ex, const float *g, float *dx, nts_vid_t 
   NTS_ARG_CHECK(d.owned_vertices == 0 || (g && dx), "null gradient pointer");
   cudaStream_t st = as_stream(stream);
   const int P = ex->P, p = ex->p;
-  NTS_ARG_CHECK(!bf16 || P > 1, "BF16 gathers on one partition run through nts_gather_plan_run_bf16");
+  NTS_ARG_CHECK(!bf16 || P > 1, "BF16 gathers on one partition run through nts_gather_plan_run_bf16_ex");
   if (P == 1)
     return nts_gather_by_src_from_dst(g, dx, d.local_weight_backward, d.local_row_offset, d.local_column_indices,
                                       d.dst_start, d.dst_start + d.owned_vertices, d.dst_start,
@@ -923,7 +901,7 @@ static int backward_impl(nts_exchange *ex, const float *g, float *dx, nts_vid_t 
     if (bf16)
       NTS_TRY(run_plan_bf16(mode->merged, gin, NTS_DTYPE_BF16, gt.ld, ex->bsend, F, st));
     else
-      NTS_TRY(nts_gather_plan_run(mode->merged, g, ex->bsend, F, st));
+      NTS_TRY(run_plan(mode->merged, g, F, ex->bsend, F, 0, st));
     NTS_CUDA_OK(cudaEventRecord(ex->ev_peer[p], st));
     NTS_CUDA_OK(cudaStreamWaitEvent(ex->comm, ex->ev_peer[p], 0));
     for (int s = 1; s < P; s++) {
@@ -1102,7 +1080,7 @@ int nts_exchange_backward(nts_exchange *ex, const float *g, float *dx, nts_vid_t
   return check_wait_error(ex, backward_impl(ex, g, dx, F, stream));
 }
 
-// BF16 gathers with FP32 accumulation (nts_gather_plan_run_bf16's contract) across partitions: the rows travel as BF16
+// BF16 gathers with FP32 accumulation (nts_gather_plan_run_bf16_ex's contract) across partitions: the rows travel as BF16
 int nts_exchange_forward_bf16(nts_exchange *ex, const void *x, int x_dtype, float *y, nts_vid_t F, void *stream) {
   NTS_ARG_CHECK(ex != nullptr, "null engine");
   NTS_ARG_CHECK(x_dtype == NTS_DTYPE_F32 || x_dtype == NTS_DTYPE_BF16, "x_dtype must be NTS_DTYPE_F32 or NTS_DTYPE_BF16");

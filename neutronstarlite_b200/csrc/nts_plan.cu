@@ -27,7 +27,7 @@
 // Plan construction (hand-written kernels + one CUB radix sort) replaces nothing in the reference: its chunks are
 // built on the host by single-threaded loops (core/PartitionedGraph.hpp:324-420) and never re-bucketed.
 //
-// BF16 gathers (nts_gather_plan_run_bf16): the gathered operand is read as BF16 rows (round-to-nearest-even of the
+// BF16 gathers (nts_gather_plan_run_bf16_ex): the gathered operand is read as BF16 rows (round-to-nearest-even of the
 // FP32 input, one conversion pass per call into the plan's workspace at a stride of ceil(F/8)*8) and widened to FP32
 // in registers; weights, accumulators and outputs stay FP32.  A 16-byte load then carries 8 values instead of 4, so
 // every gathered edge moves half the bytes through L2 and the L1 data stage.
@@ -62,7 +62,7 @@ struct nts_gather_plan {
   size_t dense_floats = 0;
   int overlap = 0;                 // 1: the row block runs inside the slab launches (planned_slab_hub_kernel)
   int last_grid = 0, last_launches = 0, last_k = 0, last_u = 0, last_outv = 0;
-  float tuned_ms = 0.f;        // nts_gather_plan_create_tuned: time of the winning candidate
+  float tuned_ms = 0.f;        // measured plans (tune_plan): time of the winning candidate
 };
 
 namespace nts {
@@ -82,60 +82,57 @@ __device__ __forceinline__ uint32_t plan_find_row(const uint32_t *__restrict__ o
   return lo;
 }
 
-// key[e] = slab(e) * n_rows + row(e), val[e] = e
-__global__ void plan_keys_kernel(const uint32_t *__restrict__ off, const uint32_t *__restrict__ idx,
-                                 const uint32_t *__restrict__ slot_of, uint32_t base, uint32_t n_rows, uint32_t n_edges,
-                                 uint32_t slab_rows, uint32_t slabs, uint32_t *__restrict__ key,
+// The mapped (gathered) row of edge e of a part: index_add + (slot_of[idx[e]] or idx[e] - index_base)
+__device__ __forceinline__ uint32_t plan_gathered_row(const nts_plan_part &pt, uint32_t e) {
+  const uint32_t id = __ldg(pt.indices + e);
+  return (pt.slot_of ? __ldg(pt.slot_of + id) : id - pt.index_base) + pt.index_add;
+}
+
+constexpr uint32_t kNoHub = 0xffffffffu;
+
+// Edge e of part pt is plan edge e_off + e, its output row row_add + (part-local row):
+// key[e_off + e] = slab(gathered row) * n_rows + output row, val[e_off + e] = e_off + e.
+// KeyT = uint64_t (a single part with hub blocks): an edge whose gathered row is a hub column goes to cell (slot, row)
+// of the column block D_c^T [hub_cols x lda_c]; else an edge of a hub row goes to cell (gathered row, slot) of the row
+// block D_r^T [gather_rows x lda_r]; both as n_keys + the cell's offset in the dense buffer, so they sort past every
+// residual (slab, row) key and voff[n_keys] is the residual edge count.
+template <class KeyT>
+__global__ void plan_keys_kernel(nts_plan_part pt, uint32_t e_off, uint32_t n_rows, uint32_t slab_rows, uint32_t slabs,
+                                 const uint32_t *__restrict__ col_slot, const uint32_t *__restrict__ row_slot,
+                                 uint32_t lda_c, uint64_t dc_cells, uint32_t lda_r, KeyT *__restrict__ key,
                                  uint32_t *__restrict__ val) {
-  for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n_edges; e += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t r = plan_find_row(off, n_rows, (uint32_t)e);
-    const uint32_t id = __ldg(idx + e);
-    const uint32_t g = slot_of ? __ldg(slot_of + id) : id - base;
+  for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < pt.n_edges; e += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t r = plan_find_row(pt.offsets, pt.n_rows, (uint32_t)e) + pt.row_add;
+    const uint32_t g = plan_gathered_row(pt, (uint32_t)e);
     uint32_t s = g / slab_rows;
     if (s >= slabs)
       s = slabs - 1;
-    key[e] = s * n_rows + r;
-    val[e] = (uint32_t)e;
+    KeyT k = (KeyT)s * n_rows + r;
+    if constexpr (sizeof(KeyT) == 8) {
+      const uint64_t n_keys = (uint64_t)slabs * n_rows;
+      const uint32_t cs = __ldg(col_slot + g), rs = __ldg(row_slot + r);
+      if (cs != kNoHub)
+        k = n_keys + (uint64_t)cs * lda_c + r;
+      else if (rs != kNoHub)
+        k = n_keys + dc_cells + (uint64_t)g * lda_r + rs;
+    }
+    key[e_off + e] = k;
+    val[e_off + e] = e_off + (uint32_t)e;
   }
 }
 
-// pairs[i] = {row(perm[i]), w[perm[i]]}   (perm == nullptr: identity)
-__global__ void plan_pairs_kernel(const uint32_t *__restrict__ perm, const uint32_t *__restrict__ idx,
-                                  const float *__restrict__ w, const uint32_t *__restrict__ slot_of, uint32_t base,
+// pairs[i] = {gathered row, weight} of plan edge perm[i] (perm == nullptr: identity); parts: the device copy of the
+// plan's parts, whose edges are numbered consecutively in the order given
+__global__ void plan_pairs_kernel(const uint32_t *__restrict__ perm, const nts_plan_part *__restrict__ parts,
                                   uint32_t n_edges, uint2 *__restrict__ pairs) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_edges; i += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t e = perm ? __ldg(perm + i) : (uint32_t)i;
-    const uint32_t id = __ldg(idx + e);
-    const uint32_t g = slot_of ? __ldg(slot_of + id) : id - base;
-    const float wt = w ? __ldg(w + e) : 1.f;
-    pairs[i] = make_uint2(g, __float_as_uint(wt));
+    uint32_t e = perm ? __ldg(perm + i) : (uint32_t)i;
+    const nts_plan_part *pt = parts;
+    for (; e >= pt->n_edges; pt++)
+      e -= (uint32_t)pt->n_edges;
+    const float wt = pt->weight ? __ldg(pt->weight + e) : 1.f;
+    pairs[i] = make_uint2(plan_gathered_row(*pt, e), __float_as_uint(wt));
   }
-}
-
-// Multi-part variants (several chunks merged into one plan): part-local row r -> output row row_add + r, mapped index
-// g -> index_add + g; edge e of the part is global edge e_off + e.
-__global__ void plan_part_keys_kernel(const uint32_t *__restrict__ off, const uint32_t *__restrict__ idx,
-                                      const uint32_t *__restrict__ slot_of, const float *__restrict__ w, uint32_t base,
-                                      uint32_t index_add, uint32_t n_rows_part, uint32_t row_add, uint32_t n_edges,
-                                      uint32_t e_off, uint32_t n_rows_total, uint32_t slab_rows, uint32_t slabs,
-                                      uint32_t *__restrict__ key, uint32_t *__restrict__ val,
-                                      uint2 *__restrict__ unsorted) {
-  for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n_edges; e += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t r = plan_find_row(off, n_rows_part, (uint32_t)e) + row_add;
-    const uint32_t id = __ldg(idx + e);
-    const uint32_t g = (slot_of ? __ldg(slot_of + id) : id - base) + index_add;
-    uint32_t s = g / slab_rows;
-    if (s >= slabs)
-      s = slabs - 1;
-    key[e_off + e] = s * n_rows_total + r;
-    val[e_off + e] = e_off + (uint32_t)e;
-    unsorted[e_off + e] = make_uint2(g, __float_as_uint(w ? __ldg(w + e) : 1.f));
-  }
-}
-__global__ void plan_permute_pairs_kernel(const uint32_t *__restrict__ perm, const uint2 *__restrict__ unsorted,
-                                          uint32_t n_edges, uint2 *__restrict__ pairs) {
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_edges; i += (uint64_t)gridDim.x * blockDim.x)
-    pairs[i] = unsorted[__ldg(perm + i)];
 }
 
 // voff[k] = number of sorted keys < k, k in [0, n_keys]
@@ -156,46 +153,12 @@ __global__ void plan_offsets_kernel(const KeyT *__restrict__ sorted_key, uint32_
 }
 
 // ---- hub blocks (nts_gather_plan_create_hybrid) --------------------------------------------------------------------
-constexpr uint32_t kNoHub = 0xffffffffu;
-
 // cnt[g] = number of edges that gather row g (integer atomics: the counts are exact and order-independent)
 __global__ void plan_ref_count_kernel(const uint32_t *__restrict__ idx, const uint32_t *__restrict__ slot_of,
                                       uint32_t base, uint32_t n_edges, uint32_t *__restrict__ cnt) {
   for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n_edges; e += (uint64_t)gridDim.x * blockDim.x) {
     const uint32_t id = __ldg(idx + e);
     atomicAdd(cnt + (slot_of ? __ldg(slot_of + id) : id - base), 1u);
-  }
-}
-
-// 64-bit key per edge: an edge whose gathered row is a hub column goes to cell (slot, row) of the column block D_c^T
-// [hub_cols x lda_c]; else an edge of a hub row goes to cell (gathered row, slot) of the row block D_r^T
-// [gather_rows x lda_r]; both as n_keys + the cell's offset in the dense buffer, so they sort past every residual
-// (slab, row) key and voff[n_keys] is the residual edge count.
-__global__ void plan_hybrid_keys_kernel(const uint32_t *__restrict__ off, const uint32_t *__restrict__ idx,
-                                        const uint32_t *__restrict__ slot_of, uint32_t base, uint32_t n_rows,
-                                        uint32_t n_edges, uint32_t slab_rows, uint32_t slabs,
-                                        const uint32_t *__restrict__ col_slot, const uint32_t *__restrict__ row_slot,
-                                        uint32_t lda_c, uint64_t dc_cells, uint32_t lda_r, uint64_t *__restrict__ key,
-                                        uint32_t *__restrict__ val) {
-  const uint64_t n_keys = (uint64_t)slabs * n_rows;
-  for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n_edges; e += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t r = plan_find_row(off, n_rows, (uint32_t)e);
-    const uint32_t id = __ldg(idx + e);
-    const uint32_t g = slot_of ? __ldg(slot_of + id) : id - base;
-    const uint32_t cs = __ldg(col_slot + g), rs = __ldg(row_slot + r);
-    uint64_t k;
-    if (cs != kNoHub) {
-      k = n_keys + (uint64_t)cs * lda_c + r;
-    } else if (rs != kNoHub) {
-      k = n_keys + dc_cells + (uint64_t)g * lda_r + rs;
-    } else {
-      uint32_t s = g / slab_rows;
-      if (s >= slabs)
-        s = slabs - 1;
-      k = (uint64_t)s * n_rows + r;
-    }
-    key[e] = k;
-    val[e] = (uint32_t)e;
   }
 }
 
@@ -972,7 +935,7 @@ static int launch_hub_blocks(nts_gather_plan *pl, const TB *in, uint32_t ldb, fl
 // ---- fused slab launches (nts_gather_plan.overlap): the row block's tiles run inside the slab launches --------------
 // The row block is FFMA-bound, the residual gather bound by gathered rows moving from L2 to the SMs; run one after the
 // other, each leaves idle what the other needs.  They can share a launch because they write disjoint output rows: the
-// row block takes every non-column-block edge of its hub rows (build_hybrid), so those rows have empty residual
+// row block takes every non-column-block edge of its hub rows (plan_keys_kernel), so those rows have empty residual
 // segments and no gather warp writes them, while the row block writes hub rows only.  Its split-K is cut at the slab
 // boundaries, so the tiles in slab s's launch read B rows [s * slab_rows, (s+1) * slab_rows) of the gathered matrix:
 // the rows slab s's gather is making L2-resident.  (The column block writes every output row with a plain
@@ -1256,8 +1219,8 @@ static int run_prologue(nts_gather_plan *pl, const void *input, uint32_t lds, fl
 // FP32 rows of stride lds.  16-byte loads need 16-byte aligned rows: the input is gathered in place when lds % 4 == 0
 // and it is aligned (the gather then reads columns F..lds of every row, the last one included, but never writes them
 // to an output); otherwise, or with NTS_PLAN_COPY_INPUT, from a zero-padded copy (ld = F rounded up to 4).
-static int run_plan(nts_gather_plan *pl, const float *input, uint32_t lds, float *output, uint32_t F, int flags,
-                    cudaStream_t st) {
+int run_plan(nts_gather_plan *pl, const float *input, uint32_t lds, float *output, uint32_t F, int flags,
+             cudaStream_t st) {
   bool done = false;
   if (const int rc = run_prologue(pl, input, lds, output, F, flags, &done, st))
     return rc;
@@ -1318,12 +1281,6 @@ int run_plan_bf16(nts_gather_plan *pl, const void *input, int dtype, uint32_t ld
   return run_gather<__nv_bfloat16>(pl, pl->workspace_bf16, ld, output, F, overwrite, st);
 }
 
-} // namespace nts
-
-using namespace nts;
-
-extern "C" {
-
 // Slab-count bound for gathered rows of row_bytes bytes each (FP32: F rounded up to 4 floats, BF16: to 8 values).
 static int pick_slabs_for_rows(nts_vid_t gather_rows, uint64_t n_edges, nts_vid_t n_rows, uint64_t row_bytes,
                                uint64_t l2_budget_bytes) {
@@ -1338,11 +1295,6 @@ static int pick_slabs_for_rows(nts_vid_t gather_rows, uint64_t n_edges, nts_vid_
   if (s > 64)
     s = 64;
   return s < 1 ? 1 : (int)s;
-}
-
-int nts_gather_plan_pick_slabs(nts_vid_t gather_rows, uint64_t n_edges, nts_vid_t n_rows, nts_vid_t feature_size,
-                               uint64_t l2_budget_bytes) {
-  return pick_slabs_for_rows(gather_rows, n_edges, n_rows, ((feature_size + 3ull) & ~3ull) * 4ull, l2_budget_bytes);
 }
 
 // Exact reference counts of the gathered rows and segment lengths of the output rows, on the host.
@@ -1381,70 +1333,85 @@ static std::vector<uint32_t> top_ids(const std::vector<uint32_t> &cnt, size_t h)
   return ids;
 }
 
-// Hybrid construction: hub columns / hub rows are picked, the edges split into the two dense blocks and the residual
-// by one stable 64-bit radix sort, the residual bucketed as usual and each dense cell the sum of its edges' weights.
-static bool build_hybrid(nts_gather_plan *pl, const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
-                         const nts_vid_t *slot_of, nts_vid_t index_base, int n_hub_cols, int n_hub_rows,
-                         cudaStream_t st) {
-  const uint32_t E = (uint32_t)pl->n_edges, n_rows = pl->n_rows, G = pl->gather_rows;
-  std::vector<uint32_t> col_cnt, seg;
-  if (!hub_counts(offsets, indices, slot_of, index_base, n_rows, E, G, col_cnt, seg, st))
-    return false;
-  const std::vector<uint32_t> cols = top_ids(col_cnt, (size_t)n_hub_cols), rows = top_ids(seg, (size_t)n_hub_rows);
-  pl->hub_cols = (int)cols.size();
-  pl->hub_rows = (int)rows.size();
-  pl->lda_c = (n_rows + 3u) & ~3u;
-  pl->lda_r = ((uint32_t)pl->hub_rows + 3u) & ~3u;
-  const uint64_t dc_cells = (uint64_t)pl->hub_cols * pl->lda_c;
-  pl->dense_floats = dc_cells + (pl->hub_rows ? (uint64_t)G * pl->lda_r : 0);
-  std::vector<uint32_t> col_slot(G, kNoHub), row_slot(n_rows, kNoHub);
-  for (size_t i = 0; i < cols.size(); i++)
-    col_slot[cols[i]] = (uint32_t)i;
-  for (size_t i = 0; i < rows.size(); i++)
-    row_slot[rows[i]] = (uint32_t)i;
+static nts_gather_plan *refuse_plan(const char *what) {
+  fail(-1, what, __FILE__, __LINE__);
+  return nullptr;
+}
 
+// The sorted layout of pl (pairs and voff allocated, d_parts the device copy of the parts): one stable LSD radix sort
+// of all edges by key, so the edges of one (slab, row) segment or one dense cell keep the order of the parts and each
+// part its own edge order; then the residual pairs in sorted order, the segment offsets and the host copy of the slab
+// boundaries.  KeyT = uint32_t: (slab, row) keys only.  KeyT = uint64_t: hub columns / hub rows of the single part are
+// picked, the sort also splits off the edges of the two dense blocks and each dense cell is the sum of its edges'
+// weights.
+template <class KeyT>
+static bool sort_plan(nts_gather_plan *pl, const nts_plan_part *parts, int n_parts, const nts_plan_part *d_parts,
+                      int n_hub_cols, int n_hub_rows, cudaStream_t st) {
+  constexpr bool hubs = sizeof(KeyT) == 8;
+  const uint32_t E = (uint32_t)pl->n_edges, n_rows = pl->n_rows, G = pl->gather_rows;
   const uint64_t n_keys = (uint64_t)pl->slabs * n_rows;
+  uint64_t dc_cells = 0;
+  uint32_t *d_col_slot = nullptr, *d_row_slot = nullptr, *d_runs = nullptr;
+  bool ok = true;
+  if (hubs) {
+    const nts_plan_part &pt = parts[0];
+    std::vector<uint32_t> col_cnt, seg;
+    if (!hub_counts(pt.offsets, pt.indices, pt.slot_of, pt.index_base, n_rows, E, G, col_cnt, seg, st))
+      return false;
+    const std::vector<uint32_t> cols = top_ids(col_cnt, (size_t)n_hub_cols), rows = top_ids(seg, (size_t)n_hub_rows);
+    pl->hub_cols = (int)cols.size();
+    pl->hub_rows = (int)rows.size();
+    pl->lda_c = (n_rows + 3u) & ~3u;
+    pl->lda_r = ((uint32_t)pl->hub_rows + 3u) & ~3u;
+    dc_cells = (uint64_t)pl->hub_cols * pl->lda_c;
+    pl->dense_floats = dc_cells + (pl->hub_rows ? (uint64_t)G * pl->lda_r : 0);
+    std::vector<uint32_t> col_slot(G, kNoHub), row_slot(n_rows, kNoHub);
+    for (size_t i = 0; i < cols.size(); i++)
+      col_slot[cols[i]] = (uint32_t)i;
+    for (size_t i = 0; i < rows.size(); i++)
+      row_slot[rows[i]] = (uint32_t)i;
+    ok = cudaMalloc(reinterpret_cast<void **>(&pl->dense), pl->dense_floats * 4) == cudaSuccess &&
+         cudaMalloc(reinterpret_cast<void **>(&pl->hub_col_ids), cols.size() * 4 + 4) == cudaSuccess &&
+         cudaMalloc(reinterpret_cast<void **>(&pl->hub_row_ids), rows.size() * 4 + 4) == cudaSuccess &&
+         cudaMalloc(reinterpret_cast<void **>(&d_col_slot), (size_t)G * 4 + 4) == cudaSuccess &&
+         cudaMalloc(reinterpret_cast<void **>(&d_row_slot), (size_t)n_rows * 4 + 4) == cudaSuccess &&
+         cudaMalloc(reinterpret_cast<void **>(&d_runs), 4) == cudaSuccess &&
+         cudaMemcpyAsync(pl->hub_col_ids, cols.data(), cols.size() * 4, cudaMemcpyHostToDevice, st) == cudaSuccess &&
+         cudaMemcpyAsync(pl->hub_row_ids, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, st) == cudaSuccess &&
+         cudaMemcpyAsync(d_col_slot, col_slot.data(), (size_t)G * 4, cudaMemcpyHostToDevice, st) == cudaSuccess &&
+         cudaMemcpyAsync(d_row_slot, row_slot.data(), (size_t)n_rows * 4, cudaMemcpyHostToDevice, st) == cudaSuccess &&
+         cudaMemsetAsync(pl->dense, 0, pl->dense_floats * 4, st) == cudaSuccess;
+  }
   int bits = 1;
-  while (bits < 64 && (1ull << bits) < n_keys + pl->dense_floats)
+  while (bits < (int)(8 * sizeof(KeyT)) && (1ull << bits) < n_keys + pl->dense_floats)
     bits++;
-  uint64_t *key_in = nullptr, *key_out = nullptr;
-  uint32_t *val_in = nullptr, *val_out = nullptr, *d_col_slot = nullptr, *d_row_slot = nullptr, *d_runs = nullptr;
+  KeyT *key_in = nullptr, *key_out = nullptr;
+  uint32_t *val_in = nullptr, *val_out = nullptr;
   void *tmp = nullptr;
   size_t tmp_bytes = 0;
-  bool ok =
-      cudaMalloc(reinterpret_cast<void **>(&pl->pairs), (size_t)E * sizeof(uint2)) == cudaSuccess &&
-      cudaMalloc(reinterpret_cast<void **>(&pl->voff), ((size_t)n_keys + 1) * 4) == cudaSuccess &&
-      cudaMalloc(reinterpret_cast<void **>(&pl->dense), pl->dense_floats * 4) == cudaSuccess &&
-      cudaMalloc(reinterpret_cast<void **>(&pl->hub_col_ids), cols.size() * 4 + 4) == cudaSuccess &&
-      cudaMalloc(reinterpret_cast<void **>(&pl->hub_row_ids), rows.size() * 4 + 4) == cudaSuccess &&
-      cudaMalloc(reinterpret_cast<void **>(&d_col_slot), (size_t)G * 4 + 4) == cudaSuccess &&
-      cudaMalloc(reinterpret_cast<void **>(&d_row_slot), (size_t)n_rows * 4 + 4) == cudaSuccess &&
-      cudaMalloc(reinterpret_cast<void **>(&key_in), (size_t)E * 8) == cudaSuccess &&
-      cudaMalloc(reinterpret_cast<void **>(&key_out), (size_t)E * 8) == cudaSuccess &&
-      cudaMalloc(reinterpret_cast<void **>(&val_in), (size_t)E * 4) == cudaSuccess &&
-      cudaMalloc(reinterpret_cast<void **>(&val_out), (size_t)E * 4) == cudaSuccess &&
-      cudaMalloc(reinterpret_cast<void **>(&d_runs), 4) == cudaSuccess &&
-      cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, key_in, key_out, val_in, val_out, (int64_t)E, 0, bits, st) ==
-          cudaSuccess &&
-      cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 16) == cudaSuccess &&
-      cudaMemcpyAsync(pl->hub_col_ids, cols.data(), cols.size() * 4, cudaMemcpyHostToDevice, st) == cudaSuccess &&
-      cudaMemcpyAsync(pl->hub_row_ids, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, st) == cudaSuccess &&
-      cudaMemcpyAsync(d_col_slot, col_slot.data(), (size_t)G * 4, cudaMemcpyHostToDevice, st) == cudaSuccess &&
-      cudaMemcpyAsync(d_row_slot, row_slot.data(), (size_t)n_rows * 4, cudaMemcpyHostToDevice, st) == cudaSuccess &&
-      cudaMemsetAsync(pl->dense, 0, pl->dense_floats * 4, st) == cudaSuccess;
-  const unsigned blocks = (unsigned)std::min<uint64_t>(((uint64_t)E + 255) / 256, (uint64_t)sm_count() * 32);
-  if (ok) {
-    plan_hybrid_keys_kernel<<<blocks, 256, 0, st>>>(offsets, indices, slot_of, index_base, n_rows, E, pl->slab_rows,
-                                                    (uint32_t)pl->slabs, d_col_slot, d_row_slot, pl->lda_c, dc_cells,
-                                                    pl->lda_r, key_in, val_in);
+  ok = ok && cudaMalloc(reinterpret_cast<void **>(&key_in), (size_t)E * sizeof(KeyT)) == cudaSuccess &&
+       cudaMalloc(reinterpret_cast<void **>(&key_out), (size_t)E * sizeof(KeyT)) == cudaSuccess &&
+       cudaMalloc(reinterpret_cast<void **>(&val_in), (size_t)E * 4) == cudaSuccess &&
+       cudaMalloc(reinterpret_cast<void **>(&val_out), (size_t)E * 4) == cudaSuccess &&
+       cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, key_in, key_out, val_in, val_out, (int64_t)E, 0, bits, st) ==
+           cudaSuccess &&
+       cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 16) == cudaSuccess;
+  uint32_t e_off = 0;
+  for (int k = 0; k < n_parts && ok; k++) {
+    const nts_plan_part &pt = parts[k];
+    if (!pt.n_edges)
+      continue;
+    const unsigned blocks = (unsigned)std::min<uint64_t>((pt.n_edges + 255) / 256, (uint64_t)sm_count() * 32);
+    plan_keys_kernel<KeyT><<<blocks, 256, 0, st>>>(pt, e_off, n_rows, pl->slab_rows, (uint32_t)pl->slabs, d_col_slot,
+                                                   d_row_slot, pl->lda_c, dc_cells, pl->lda_r, key_in, val_in);
     count_launch();
-    // LSD radix sort: stable, so edges of one (slab, row) segment or one dense cell keep their original order
-    ok = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, key_in, key_out, val_in, val_out, (int64_t)E, 0, bits, st) ==
-         cudaSuccess;
+    e_off += (uint32_t)pt.n_edges;
   }
+  ok = ok && cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, key_in, key_out, val_in, val_out, (int64_t)E, 0, bits,
+                                             st) == cudaSuccess;
   if (ok) {
     const unsigned kb = (unsigned)std::min<uint64_t>((n_keys + 256) / 256, (uint64_t)sm_count() * 32);
-    plan_offsets_kernel<uint64_t><<<kb, 256, 0, st>>>(key_out, E, (uint32_t)n_keys, pl->voff);
+    plan_offsets_kernel<KeyT><<<kb, 256, 0, st>>>(key_out, E, (uint32_t)n_keys, pl->voff);
     count_launch();
     std::vector<uint32_t> h(pl->slabs + 1);
     ok = cudaStreamSynchronize(st) == cudaSuccess;
@@ -1455,164 +1422,61 @@ static bool build_hybrid(nts_gather_plan *pl, const nts_vid_t *offsets, const nt
   }
   const uint32_t n_res = (uint32_t)pl->slab_edge[pl->slabs], n_dense = E - n_res;
   if (ok && n_res) {
-    plan_pairs_kernel<<<blocks, 256, 0, st>>>(val_out, indices, weight, slot_of, index_base, n_res, pl->pairs);
+    const unsigned blocks = (unsigned)std::min<uint64_t>(((uint64_t)n_res + 255) / 256, (uint64_t)sm_count() * 32);
+    plan_pairs_kernel<<<blocks, 256, 0, st>>>(val_out, d_parts, n_res, pl->pairs);
     count_launch();
   }
-  if (ok && n_dense) { // runs of equal cell keys: (key, length), start = exclusive sum of the lengths (integers)
-    uint32_t n_runs = 0;
-    size_t b1 = 0, b2 = 0;
-    ok = cub::DeviceRunLengthEncode::Encode(nullptr, b1, key_out + n_res, key_in, val_in, d_runs, (int64_t)n_dense,
-                                            st) == cudaSuccess &&
-         cub::DeviceScan::ExclusiveSum(nullptr, b2, val_in, d_col_slot, (int64_t)n_dense, st) == cudaSuccess;
-    if (ok && std::max(b1, b2) > tmp_bytes) {
-      cudaFree(tmp);
-      tmp_bytes = std::max(b1, b2);
-      ok = cudaMalloc(&tmp, tmp_bytes) == cudaSuccess;
+  if constexpr (hubs) {
+    if (ok && n_dense) { // runs of equal cell keys: (key, length), start = exclusive sum of the lengths (integers)
+      uint32_t n_runs = 0;
+      size_t b1 = 0, b2 = 0;
+      ok = cub::DeviceRunLengthEncode::Encode(nullptr, b1, key_out + n_res, key_in, val_in, d_runs, (int64_t)n_dense,
+                                              st) == cudaSuccess &&
+           cub::DeviceScan::ExclusiveSum(nullptr, b2, val_in, d_col_slot, (int64_t)n_dense, st) == cudaSuccess;
+      if (ok && std::max(b1, b2) > tmp_bytes) {
+        cudaFree(tmp);
+        tmp_bytes = std::max(b1, b2);
+        ok = cudaMalloc(&tmp, tmp_bytes) == cudaSuccess;
+      }
+      uint32_t *run_start = nullptr;
+      ok = ok && cudaMalloc(reinterpret_cast<void **>(&run_start), (size_t)n_dense * 4) == cudaSuccess &&
+           cub::DeviceRunLengthEncode::Encode(tmp, b1, key_out + n_res, key_in, val_in, d_runs, (int64_t)n_dense, st) ==
+               cudaSuccess &&
+           cudaMemcpyAsync(&n_runs, d_runs, 4, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+           cudaStreamSynchronize(st) == cudaSuccess &&
+           cub::DeviceScan::ExclusiveSum(tmp, b2, val_in, run_start, (int64_t)n_runs, st) == cudaSuccess;
+      if (ok) {
+        const unsigned rb = (unsigned)std::min<uint64_t>(((uint64_t)n_runs * 32 + 255) / 256, (uint64_t)sm_count() * 32);
+        plan_cell_sum_kernel<<<rb, 256, 0, st>>>(key_in, run_start, val_in, n_runs, val_out + n_res, parts[0].weight,
+                                                 n_keys, pl->dense);
+        count_launch();
+        ok = cudaStreamSynchronize(st) == cudaSuccess;
+      }
+      cudaFree(run_start);
     }
-    uint32_t *run_start = nullptr;
-    ok = ok && cudaMalloc(reinterpret_cast<void **>(&run_start), (size_t)n_dense * 4) == cudaSuccess &&
-         cub::DeviceRunLengthEncode::Encode(tmp, b1, key_out + n_res, key_in, val_in, d_runs, (int64_t)n_dense, st) ==
-             cudaSuccess &&
-         cudaMemcpyAsync(&n_runs, d_runs, 4, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
-         cudaStreamSynchronize(st) == cudaSuccess &&
-         cub::DeviceScan::ExclusiveSum(tmp, b2, val_in, run_start, (int64_t)n_runs, st) == cudaSuccess;
-    if (ok) {
-      const unsigned rb = (unsigned)std::min<uint64_t>(((uint64_t)n_runs * 32 + 255) / 256, (uint64_t)sm_count() * 32);
-      plan_cell_sum_kernel<<<rb, 256, 0, st>>>(key_in, run_start, val_in, n_runs, val_out + n_res, weight, n_keys,
-                                               pl->dense);
-      count_launch();
-      ok = cudaStreamSynchronize(st) == cudaSuccess;
-    }
-    cudaFree(run_start);
   }
   cudaFree(key_in), cudaFree(key_out), cudaFree(val_in), cudaFree(val_out), cudaFree(tmp);
   cudaFree(d_col_slot), cudaFree(d_row_slot), cudaFree(d_runs);
   return ok;
 }
 
-nts_gather_plan *nts_gather_plan_create(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
-                                        const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows,
-                                        uint64_t n_edges, nts_vid_t gather_rows, int n_slabs, void *stream) {
-  return nts_gather_plan_create_hybrid(offsets, indices, weight, slot_of, index_base, n_rows, n_edges, gather_rows,
-                                       n_slabs, 0, 0, stream);
-}
-
-nts_gather_plan *nts_gather_plan_create_hybrid(const nts_vid_t *offsets, const nts_vid_t *indices,
-                                               const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
-                                               nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows, int n_slabs,
-                                               int n_hub_cols, int n_hub_rows, void *stream) {
-  auto bad = [](const char *m) -> nts_gather_plan * {
-    fail(-1, m, __FILE__, __LINE__);
-    return nullptr;
-  };
-  if (n_edges >= 0xffffffffull)
-    return bad("chunk edge count must fit uint32 offsets");
-  if (n_rows && n_edges && !(offsets && indices))
-    return bad("null graph array");
-  if (n_hub_cols < 0 || n_hub_rows < 0)
-    return bad("negative hub count");
-  if (n_slabs < 1)
-    n_slabs = 1;
-  if (gather_rows == 0)
-    n_slabs = 1;
-  if ((uint64_t)n_slabs * n_rows >= 0xffffffffull)
-    return bad("slabs * rows must fit 32-bit segment keys");
-  cudaStream_t st = as_stream(stream);
-  nts_gather_plan *pl = new nts_gather_plan();
-  pl->n_rows = n_rows;
-  pl->n_edges = n_edges;
-  pl->gather_rows = gather_rows;
-  pl->slabs = n_slabs;
-  pl->slab_rows = gather_rows ? (gather_rows + n_slabs - 1) / n_slabs : 1;
-  pl->slab_edge.assign(n_slabs + 1, 0);
-  if (n_rows == 0 || n_edges == 0)
-    return pl;
-  const uint32_t E = (uint32_t)n_edges;
-  const uint32_t n_keys = (uint32_t)n_slabs * n_rows;
-  uint32_t *key_in = nullptr, *key_out = nullptr, *val_in = nullptr, *val_out = nullptr;
-  void *tmp = nullptr;
-  const bool hubs = gather_rows > 0 && (n_hub_cols > 0 || n_hub_rows > 0);
-  bool ok = hubs || (cudaMalloc(reinterpret_cast<void **>(&pl->pairs), (size_t)E * sizeof(uint2)) == cudaSuccess &&
-                     cudaMalloc(reinterpret_cast<void **>(&pl->voff), ((size_t)n_keys + 1) * sizeof(uint32_t)) ==
-                         cudaSuccess);
-  const unsigned blocks = (unsigned)std::min<uint64_t>(((uint64_t)E + 255) / 256, (uint64_t)sm_count() * 32);
-  if (hubs) {
-    ok = build_hybrid(pl, offsets, indices, weight, slot_of, index_base, n_hub_cols, n_hub_rows, st);
-  } else if (ok && n_slabs == 1) {
-    plan_pairs_kernel<<<blocks, 256, 0, st>>>(nullptr, indices, weight, slot_of, index_base, E, pl->pairs);
-    count_launch();
-    ok = cudaMemcpyAsync(pl->voff, offsets, ((size_t)n_rows + 1) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st) ==
-         cudaSuccess;
-    pl->slab_edge[0] = 0;
-    pl->slab_edge[1] = n_edges;
-  } else if (ok) {
-    size_t tmp_bytes = 0;
-    int bits = 1;
-    while (bits < 32 && (1ull << bits) < (uint64_t)n_keys)
-      bits++;
-    ok = cudaMalloc(reinterpret_cast<void **>(&key_in), (size_t)E * 4) == cudaSuccess &&
-         cudaMalloc(reinterpret_cast<void **>(&key_out), (size_t)E * 4) == cudaSuccess &&
-         cudaMalloc(reinterpret_cast<void **>(&val_in), (size_t)E * 4) == cudaSuccess &&
-         cudaMalloc(reinterpret_cast<void **>(&val_out), (size_t)E * 4) == cudaSuccess &&
-         cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, key_in, key_out, val_in, val_out, (int64_t)E, 0, bits, st) ==
-             cudaSuccess &&
-         cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 16) == cudaSuccess;
-    if (ok) {
-      plan_keys_kernel<<<blocks, 256, 0, st>>>(offsets, indices, slot_of, index_base, n_rows, E, pl->slab_rows,
-                                               (uint32_t)n_slabs, key_in, val_in);
-      count_launch();
-      // LSD radix sort: stable, so edges of one (slab, row) segment keep their original order
-      ok = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, key_in, key_out, val_in, val_out, (int64_t)E, 0, bits, st) ==
-           cudaSuccess;
-    }
-    if (ok) {
-      plan_pairs_kernel<<<blocks, 256, 0, st>>>(val_out, indices, weight, slot_of, index_base, E, pl->pairs);
-      count_launch();
-      const unsigned kb = (unsigned)std::min<uint64_t>(((uint64_t)n_keys + 256) / 256, (uint64_t)sm_count() * 32);
-      plan_offsets_kernel<uint32_t><<<kb, 256, 0, st>>>(key_out, E, n_keys, pl->voff);
-      count_launch();
-      std::vector<uint32_t> h(n_slabs + 1);
-      ok = cudaStreamSynchronize(st) == cudaSuccess;
-      for (int s = 0; s <= n_slabs && ok; s++)
-        ok = cudaMemcpy(&h[s], pl->voff + (size_t)s * n_rows, 4, cudaMemcpyDeviceToHost) == cudaSuccess;
-      for (int s = 0; s <= n_slabs; s++)
-        pl->slab_edge[s] = h[s];
-    }
-  }
-  if (ok)
-    ok = cudaStreamSynchronize(st) == cudaSuccess && cudaGetLastError() == cudaSuccess;
-  cudaFree(key_in), cudaFree(key_out), cudaFree(val_in), cudaFree(val_out), cudaFree(tmp);
-  if (!ok) {
-    nts_gather_plan_destroy(pl);
-    fail(-1, "nts_gather_plan_create: device allocation or preprocessing failed", __FILE__, __LINE__);
-    return nullptr;
-  }
-  return pl;
-}
-
-// Several chunks merged into ONE plan (the exchange engine aggregates all remote chunks of a rank in one launch when
-// their rows arrive faster than one chunk computes): a stable sort of all parts' edges by (slab, output row); inside a
-// segment the parts follow each other in the order given, each keeping its own edge order.
-static nts_gather_plan *build_plan_parts(const nts_plan_part *parts, int n_parts, nts_vid_t n_rows, nts_vid_t gather_rows,
-                                         int n_slabs, cudaStream_t st) {
-  auto bad = [](const char *m) -> nts_gather_plan * {
-    fail(-1, m, __FILE__, __LINE__);
-    return nullptr;
-  };
+// The plan builder: the edges of parts (a single chunk is one part with row_add = index_add = 0) bucketed by (slab,
+// output row), with n_hub_cols / n_hub_rows dense hub blocks beside the residual (a single part only).  The caller has
+// checked the parts' arrays and row ranges.
+static nts_gather_plan *build_plan(const nts_plan_part *parts, int n_parts, nts_vid_t n_rows, nts_vid_t gather_rows,
+                                   int n_slabs, int n_hub_cols, int n_hub_rows, cudaStream_t st) {
   uint64_t total = 0;
-  for (int k = 0; k < n_parts; k++) {
-    if (parts[k].n_edges && !(parts[k].offsets && parts[k].indices))
-      return bad("null graph array in a plan part");
-    if ((uint64_t)parts[k].row_add + parts[k].n_rows > n_rows)
-      return bad("plan part rows exceed the output rows");
+  for (int k = 0; k < n_parts; k++)
     total += parts[k].n_edges;
-  }
   if (total >= 0xffffffffull)
-    return bad("merged edge count must fit uint32 offsets");
+    return refuse_plan("plan edge count must fit uint32 offsets");
   if (n_slabs < 1 || gather_rows == 0)
     n_slabs = 1;
   if ((uint64_t)n_slabs * n_rows >= 0xffffffffull)
-    return bad("slabs * rows must fit 32-bit segment keys");
+    return refuse_plan("slabs * rows must fit 32-bit segment keys");
+  const bool hubs = gather_rows > 0 && (n_hub_cols > 0 || n_hub_rows > 0);
+  if (hubs && n_parts != 1)
+    return refuse_plan("hub blocks need a plan of a single part");
   nts_gather_plan *pl = new nts_gather_plan();
   pl->n_rows = n_rows;
   pl->n_edges = total;
@@ -1622,145 +1486,33 @@ static nts_gather_plan *build_plan_parts(const nts_plan_part *parts, int n_parts
   pl->slab_edge.assign(n_slabs + 1, 0);
   if (n_rows == 0 || total == 0)
     return pl;
-  const uint32_t E = (uint32_t)total, n_keys = (uint32_t)n_slabs * n_rows;
-  uint32_t *key_in = nullptr, *key_out = nullptr, *val_in = nullptr, *val_out = nullptr;
-  uint2 *unsorted = nullptr;
-  void *tmp = nullptr;
-  size_t tmp_bytes = 0;
-  int bits = 1;
-  while (bits < 32 && (1ull << bits) < (uint64_t)n_keys)
-    bits++;
+  const uint32_t E = (uint32_t)total;
+  nts_plan_part *d_parts = nullptr;
   bool ok = cudaMalloc(reinterpret_cast<void **>(&pl->pairs), (size_t)E * sizeof(uint2)) == cudaSuccess &&
-            cudaMalloc(reinterpret_cast<void **>(&pl->voff), ((size_t)n_keys + 1) * sizeof(uint32_t)) == cudaSuccess &&
-            cudaMalloc(reinterpret_cast<void **>(&unsorted), (size_t)E * sizeof(uint2)) == cudaSuccess &&
-            cudaMalloc(reinterpret_cast<void **>(&key_in), (size_t)E * 4) == cudaSuccess &&
-            cudaMalloc(reinterpret_cast<void **>(&key_out), (size_t)E * 4) == cudaSuccess &&
-            cudaMalloc(reinterpret_cast<void **>(&val_in), (size_t)E * 4) == cudaSuccess &&
-            cudaMalloc(reinterpret_cast<void **>(&val_out), (size_t)E * 4) == cudaSuccess &&
-            cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, key_in, key_out, val_in, val_out, (int64_t)E, 0, bits, st) ==
-                cudaSuccess &&
-            cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 16) == cudaSuccess;
-  uint32_t e_off = 0;
-  for (int k = 0; k < n_parts && ok; k++) {
-    const nts_plan_part &pt = parts[k];
-    if (!pt.n_edges)
-      continue;
-    const unsigned blocks = (unsigned)std::min<uint64_t>((pt.n_edges + 255) / 256, (uint64_t)sm_count() * 32);
-    plan_part_keys_kernel<<<blocks, 256, 0, st>>>(pt.offsets, pt.indices, pt.slot_of, pt.weight, pt.index_base,
-                                                  pt.index_add, pt.n_rows, pt.row_add, (uint32_t)pt.n_edges, e_off, n_rows,
-                                                  pl->slab_rows, (uint32_t)n_slabs, key_in, val_in, unsorted);
-    count_launch();
-    e_off += (uint32_t)pt.n_edges;
-  }
-  if (ok)
-    ok = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, key_in, key_out, val_in, val_out, (int64_t)E, 0, bits, st) ==
-         cudaSuccess;
-  if (ok) {
+            cudaMalloc(reinterpret_cast<void **>(&pl->voff), ((size_t)n_slabs * n_rows + 1) * 4) == cudaSuccess &&
+            cudaMalloc(reinterpret_cast<void **>(&d_parts), n_parts * sizeof(nts_plan_part)) == cudaSuccess &&
+            cudaMemcpyAsync(d_parts, parts, n_parts * sizeof(nts_plan_part), cudaMemcpyHostToDevice, st) == cudaSuccess;
+  if (ok && n_slabs == 1 && !hubs && n_parts == 1 && parts[0].row_add == 0 && parts[0].n_rows == n_rows) {
+    // one part in its own row order: the stable sort would leave every edge in place
     const unsigned blocks = (unsigned)std::min<uint64_t>(((uint64_t)E + 255) / 256, (uint64_t)sm_count() * 32);
-    plan_permute_pairs_kernel<<<blocks, 256, 0, st>>>(val_out, unsorted, E, pl->pairs);
+    plan_pairs_kernel<<<blocks, 256, 0, st>>>(nullptr, d_parts, E, pl->pairs);
     count_launch();
-    const unsigned kb = (unsigned)std::min<uint64_t>(((uint64_t)n_keys + 256) / 256, (uint64_t)sm_count() * 32);
-    plan_offsets_kernel<uint32_t><<<kb, 256, 0, st>>>(key_out, E, n_keys, pl->voff);
-    count_launch();
-    std::vector<uint32_t> h(n_slabs + 1);
-    ok = cudaStreamSynchronize(st) == cudaSuccess;
-    for (int s = 0; s <= n_slabs && ok; s++)
-      ok = cudaMemcpy(&h[s], pl->voff + (size_t)s * n_rows, 4, cudaMemcpyDeviceToHost) == cudaSuccess;
-    for (int s = 0; s <= n_slabs; s++)
-      pl->slab_edge[s] = h[s];
+    ok = cudaMemcpyAsync(pl->voff, parts[0].offsets, ((size_t)n_rows + 1) * 4, cudaMemcpyDeviceToDevice, st) ==
+         cudaSuccess;
+    pl->slab_edge[1] = E;
+  } else if (ok) {
+    ok = hubs ? sort_plan<uint64_t>(pl, parts, n_parts, d_parts, n_hub_cols, n_hub_rows, st)
+              : sort_plan<uint32_t>(pl, parts, n_parts, d_parts, 0, 0, st);
   }
   if (ok)
     ok = cudaStreamSynchronize(st) == cudaSuccess && cudaGetLastError() == cudaSuccess;
-  cudaFree(key_in), cudaFree(key_out), cudaFree(val_in), cudaFree(val_out), cudaFree(tmp), cudaFree(unsorted);
+  cudaFree(d_parts);
   if (!ok) {
-    fail(-1, "nts_gather_plan_create_parts: device allocation or preprocessing failed", __FILE__, __LINE__);
-    cudaFree(pl->pairs), cudaFree(pl->voff);
-    delete pl;
-    return nullptr;
+    nts_gather_plan_destroy(pl);
+    return refuse_plan("nts_gather_plan: device allocation or preprocessing failed");
   }
   return pl;
 }
-
-// n_slabs >= 1: that slab count; n_slabs == 0: measured for feature_size like nts_gather_plan_create_tuned (bf16:
-// timed as BF16 gathers, slab bound on 2-byte rows, like nts_gather_plan_create_tuned_bf16)
-nts_gather_plan *nts_plan_create_parts_typed(const nts_plan_part *parts, int n_parts, nts_vid_t n_rows,
-                                             nts_vid_t gather_rows, int n_slabs, nts_vid_t feature_size, int bf16,
-                                             void *stream) {
-  if (!parts || n_parts < 1) {
-    fail(-1, "no plan parts", __FILE__, __LINE__);
-    return nullptr;
-  }
-  cudaStream_t st = as_stream(stream);
-  if (n_slabs >= 1)
-    return build_plan_parts(parts, n_parts, n_rows, gather_rows, n_slabs, st);
-  uint64_t total = 0;
-  for (int k = 0; k < n_parts; k++)
-    total += parts[k].n_edges;
-  const uint64_t row_bytes = bf16 ? ((feature_size + 7ull) & ~7ull) * 2ull : ((feature_size + 3ull) & ~3ull) * 4ull;
-  const int s_max = pick_slabs_for_rows(gather_rows, total, n_rows, row_bytes, 16ull << 20);
-  nts_gather_plan *best = build_plan_parts(parts, n_parts, n_rows, gather_rows, 1, st);
-  if (!best || s_max <= 1 || total == 0 || feature_size == 0)
-    return best;
-  float *x = nullptr, *y = nullptr;
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  const size_t xb = (size_t)gather_rows * feature_size * (bf16 ? 2 : sizeof(float)),
-               yb = (size_t)n_rows * feature_size * sizeof(float);
-  bool ok = cudaMalloc(reinterpret_cast<void **>(&x), xb) == cudaSuccess &&
-            cudaMalloc(reinterpret_cast<void **>(&y), yb) == cudaSuccess &&
-            cudaMemsetAsync(x, 0, xb, st) == cudaSuccess && cudaMemsetAsync(y, 0, yb, st) == cudaSuccess &&
-            cudaEventCreate(&e0) == cudaSuccess && cudaEventCreate(&e1) == cudaSuccess;
-  auto time_plan = [&](nts_gather_plan *pl, float *ms) -> bool {
-    *ms = 1e30f;
-    for (int it = 0; it < 3; it++) {
-      float t = 0.f;
-      if (cudaEventRecord(e0, st) != cudaSuccess ||
-          (bf16 ? run_plan_bf16(pl, x, NTS_DTYPE_BF16, feature_size, y, feature_size, st)
-                : run_plan(pl, x, feature_size, y, feature_size, 0, st)) != 0 ||
-          cudaEventRecord(e1, st) != cudaSuccess || cudaEventSynchronize(e1) != cudaSuccess ||
-          cudaEventElapsedTime(&t, e0, e1) != cudaSuccess)
-        return false;
-      if (it > 0 && t < *ms)
-        *ms = t;
-    }
-    return true;
-  };
-  float best_ms = 0.f;
-  ok = ok && time_plan(best, &best_ms);
-  for (int s = 2; ok; s *= 2) {
-    const int cand = s > s_max ? s_max : s;
-    nts_gather_plan *pl = build_plan_parts(parts, n_parts, n_rows, gather_rows, cand, st);
-    float ms = 0.f;
-    if (!pl || !time_plan(pl, &ms)) {
-      nts_gather_plan_destroy(pl);
-      break;
-    }
-    if (ms < best_ms) {
-      nts_gather_plan_destroy(best);
-      best = pl;
-      best_ms = ms;
-    } else {
-      nts_gather_plan_destroy(pl);
-      if (ms > 1.1f * best_ms)
-        break;
-    }
-    if (cand == s_max)
-      break;
-  }
-  cudaFree(x), cudaFree(y);
-  if (e0)
-    cudaEventDestroy(e0);
-  if (e1)
-    cudaEventDestroy(e1);
-  best->tuned_ms = best_ms;
-  return best;
-}
-
-nts_gather_plan *nts_gather_plan_create_parts(const nts_plan_part *parts, int n_parts, nts_vid_t n_rows,
-                                              nts_vid_t gather_rows, int n_slabs, nts_vid_t feature_size, void *stream) {
-  return nts_plan_create_parts_typed(parts, n_parts, n_rows, gather_rows, n_slabs, feature_size, 0, stream);
-}
-
-float nts_gather_plan_tuned_ms(const nts_gather_plan *pl) { return pl ? pl->tuned_ms : 0.f; }
 
 // Slab count by measurement.  Whether bucketing pays depends on how skewed the gathered rows are (hub sources stay in
 // L1/L2 by themselves: on an H100, the Zipf graph of config B at F=602 takes 24.8 ms unbucketed, 19.5 ms with 4 slabs
@@ -1780,53 +1532,35 @@ float nts_gather_plan_tuned_ms(const nts_gather_plan *pl) { return pl ? pl->tune
 static constexpr double kHubFloor = 0.05;
 static constexpr int kHubMax = 512;
 
-// bf16: candidates are timed with BF16 gathers (a BF16 input of width feature_size, gathered as a BF16 run gathers
-// it) and the slab bound counts rows of ceil(F/8)*8 2-byte values.  run_flags: the mode the candidates are timed in
-// (NTS_PLAN_OVERWRITE prices the column block at its store cost, not at a read-modify-write of the whole output).
-static nts_gather_plan *create_tuned(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
-                                     const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows, uint64_t n_edges,
-                                     nts_vid_t gather_rows, nts_vid_t feature_size, bool bf16, int run_flags,
-                                     void *stream) {
-  cudaStream_t st = as_stream(stream);
+nts_gather_plan *tune_plan(const nts_plan_part *parts, int n_parts, nts_vid_t n_rows, nts_vid_t gather_rows,
+                           nts_vid_t feature_size, bool bf16, int run_flags, bool hubs_allowed, cudaStream_t st) {
+  uint64_t n_edges = 0;
+  for (int k = 0; k < n_parts; k++)
+    n_edges += parts[k].n_edges;
   const uint64_t row_bytes = bf16 ? ((feature_size + 7ull) & ~7ull) * 2ull : ((feature_size + 3ull) & ~3ull) * 4ull;
   const int s_max = pick_slabs_for_rows(gather_rows, n_edges, n_rows, row_bytes, 16ull << 20);
   const char *hub_env = getenv("NTS_PLAN_HUBS");
-  const bool try_hubs = !(hub_env && strcmp(hub_env, "0") == 0) && n_rows > 0 && gather_rows > 0;
-  nts_gather_plan *best = nts_gather_plan_create(offsets, indices, weight, slot_of, index_base, n_rows, n_edges,
-                                                 gather_rows, 1, stream);
+  const bool try_hubs = hubs_allowed && !(hub_env && strcmp(hub_env, "0") == 0) && n_rows > 0 && gather_rows > 0;
+  nts_gather_plan *best = build_plan(parts, n_parts, n_rows, gather_rows, 1, 0, 0, st);
   if (!best || (s_max <= 1 && !try_hubs) || n_edges == 0 || feature_size == 0)
     return best;
   float *x = nullptr, *y = nullptr;
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
   const size_t xb = (size_t)gather_rows * feature_size * (bf16 ? 2 : sizeof(float)),
                yb = (size_t)n_rows * feature_size * sizeof(float);
   bool ok = cudaMalloc(reinterpret_cast<void **>(&x), xb) == cudaSuccess &&
             cudaMalloc(reinterpret_cast<void **>(&y), yb) == cudaSuccess &&
-            cudaMemsetAsync(x, 0, xb, st) == cudaSuccess && cudaMemsetAsync(y, 0, yb, st) == cudaSuccess &&
-            cudaEventCreate(&e0) == cudaSuccess && cudaEventCreate(&e1) == cudaSuccess;
-  auto run_one = [&](nts_gather_plan *pl) {
-    return bf16 ? run_plan_bf16(pl, x, NTS_DTYPE_BF16, feature_size, y, feature_size, st, run_flags)
-                : run_plan(pl, x, feature_size, y, feature_size, run_flags, st);
-  };
-  auto time_plan = [&](nts_gather_plan *pl, float *ms) -> bool {
-    *ms = 1e30f;
-    for (int it = 0; it < 3; it++) {
-      float t = 0.f;
-      if (cudaEventRecord(e0, st) != cudaSuccess || run_one(pl) != 0 ||
-          cudaEventRecord(e1, st) != cudaSuccess || cudaEventSynchronize(e1) != cudaSuccess ||
-          cudaEventElapsedTime(&t, e0, e1) != cudaSuccess)
-        return false;
-      if (it > 0 && t < *ms)
-        *ms = t;
-    }
-    return true;
+            cudaMemsetAsync(x, 0, xb, st) == cudaSuccess && cudaMemsetAsync(y, 0, yb, st) == cudaSuccess;
+  auto time_plan = [&](nts_gather_plan *pl, float *ms) {
+    return time_min_of_two([&] {
+      return bf16 ? run_plan_bf16(pl, x, NTS_DTYPE_BF16, feature_size, y, feature_size, st, run_flags)
+                  : run_plan(pl, x, feature_size, y, feature_size, run_flags, st);
+    }, st, ms) == 0;
   };
   float best_ms = 0.f;
   ok = ok && time_plan(best, &best_ms);
   // build and time one candidate, keep it if it is faster: 1 = kept, 0 = not kept (*ms its time), -1 = failed
   auto consider = [&](int s, int hc, int hr, float *ms, int overlap = 0) -> int {
-    nts_gather_plan *pl = nts_gather_plan_create_hybrid(offsets, indices, weight, slot_of, index_base, n_rows, n_edges,
-                                                        gather_rows, s, hc, hr, stream);
+    nts_gather_plan *pl = build_plan(parts, n_parts, n_rows, gather_rows, s, hc, hr, st);
     if (pl)
       pl->overlap = overlap;
     if (!pl || !time_plan(pl, ms)) {
@@ -1852,8 +1586,10 @@ static nts_gather_plan *create_tuned(const nts_vid_t *offsets, const nts_vid_t *
       break;
   }
   if (ok && try_hubs) {
+    const nts_plan_part &pt = parts[0];
     std::vector<uint32_t> col_cnt, seg;
-    ok = hub_counts(offsets, indices, slot_of, index_base, n_rows, (uint32_t)n_edges, gather_rows, col_cnt, seg, st);
+    ok = hub_counts(pt.offsets, pt.indices, pt.slot_of, pt.index_base, n_rows, (uint32_t)n_edges, gather_rows, col_cnt,
+                    seg, st);
     int n_c = 0, n_r = 0;
     for (uint32_t c : col_cnt)
       n_c += c > kHubFloor * n_rows;
@@ -1891,28 +1627,43 @@ static nts_gather_plan *create_tuned(const nts_vid_t *offsets, const nts_vid_t *
     }
   }
   cudaFree(x), cudaFree(y);
-  if (e0)
-    cudaEventDestroy(e0);
-  if (e1)
-    cudaEventDestroy(e1);
   best->tuned_ms = best_ms;
   return best;
 }
 
-nts_gather_plan *nts_gather_plan_create_tuned(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
-                                              const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows,
-                                              uint64_t n_edges, nts_vid_t gather_rows, nts_vid_t feature_size,
-                                              void *stream) {
-  return create_tuned(offsets, indices, weight, slot_of, index_base, n_rows, n_edges, gather_rows, feature_size, false,
-                      0, stream);
+} // namespace nts
+
+using namespace nts;
+
+extern "C" {
+
+int nts_gather_plan_pick_slabs(nts_vid_t gather_rows, uint64_t n_edges, nts_vid_t n_rows, nts_vid_t feature_size,
+                               uint64_t l2_budget_bytes) {
+  return pick_slabs_for_rows(gather_rows, n_edges, n_rows, ((feature_size + 3ull) & ~3ull) * 4ull, l2_budget_bytes);
 }
 
-nts_gather_plan *nts_gather_plan_create_tuned_bf16(const nts_vid_t *offsets, const nts_vid_t *indices,
-                                                   const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
-                                                   nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows,
-                                                   nts_vid_t feature_size, void *stream) {
-  return create_tuned(offsets, indices, weight, slot_of, index_base, n_rows, n_edges, gather_rows, feature_size, true,
-                      0, stream);
+// The arguments of a single-chunk entry as a plan part; false (error set) when they are refused.
+static bool chunk_part(const nts_vid_t *offsets, const nts_vid_t *indices, const float *weight,
+                       const nts_vid_t *slot_of, nts_vid_t index_base, nts_vid_t n_rows, uint64_t n_edges,
+                       nts_plan_part *pt) {
+  if (n_rows && n_edges && !(offsets && indices)) {
+    refuse_plan("null graph array");
+    return false;
+  }
+  *pt = {offsets, indices, weight, slot_of, index_base, 0, n_rows, 0, n_edges};
+  return true;
+}
+
+nts_gather_plan *nts_gather_plan_create_hybrid(const nts_vid_t *offsets, const nts_vid_t *indices,
+                                               const float *weight, const nts_vid_t *slot_of, nts_vid_t index_base,
+                                               nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows, int n_slabs,
+                                               int n_hub_cols, int n_hub_rows, void *stream) {
+  nts_plan_part pt;
+  if (!chunk_part(offsets, indices, weight, slot_of, index_base, n_rows, n_edges, &pt))
+    return nullptr;
+  if (n_hub_cols < 0 || n_hub_rows < 0)
+    return refuse_plan("negative hub count");
+  return build_plan(&pt, 1, n_rows, gather_rows, n_slabs, n_hub_cols, n_hub_rows, as_stream(stream));
 }
 
 nts_gather_plan *nts_gather_plan_create_tuned_ex(const nts_vid_t *offsets, const nts_vid_t *indices,
@@ -1920,14 +1671,32 @@ nts_gather_plan *nts_gather_plan_create_tuned_ex(const nts_vid_t *offsets, const
                                                  nts_vid_t n_rows, uint64_t n_edges, nts_vid_t gather_rows,
                                                  nts_vid_t feature_size, int gather_dtype, int run_flags,
                                                  void *stream) {
-  if ((gather_dtype != NTS_DTYPE_F32 && gather_dtype != NTS_DTYPE_BF16) || (run_flags & ~NTS_PLAN_OVERWRITE)) {
-    fail(-1, "nts_gather_plan_create_tuned_ex: gather_dtype must be NTS_DTYPE_F32 or NTS_DTYPE_BF16, run_flags 0 or "
-             "NTS_PLAN_OVERWRITE", __FILE__, __LINE__);
+  if ((gather_dtype != NTS_DTYPE_F32 && gather_dtype != NTS_DTYPE_BF16) || (run_flags & ~NTS_PLAN_OVERWRITE))
+    return refuse_plan("nts_gather_plan_create_tuned_ex: gather_dtype must be NTS_DTYPE_F32 or NTS_DTYPE_BF16, "
+                       "run_flags 0 or NTS_PLAN_OVERWRITE");
+  nts_plan_part pt;
+  if (!chunk_part(offsets, indices, weight, slot_of, index_base, n_rows, n_edges, &pt))
     return nullptr;
-  }
-  return create_tuned(offsets, indices, weight, slot_of, index_base, n_rows, n_edges, gather_rows, feature_size,
-                      gather_dtype == NTS_DTYPE_BF16, run_flags, stream);
+  return tune_plan(&pt, 1, n_rows, gather_rows, feature_size, gather_dtype == NTS_DTYPE_BF16, run_flags, true,
+                   as_stream(stream));
 }
+
+nts_gather_plan *nts_gather_plan_create_parts(const nts_plan_part *parts, int n_parts, nts_vid_t n_rows,
+                                              nts_vid_t gather_rows, int n_slabs, nts_vid_t feature_size, void *stream) {
+  if (!parts || n_parts < 1)
+    return refuse_plan("no plan parts");
+  for (int k = 0; k < n_parts; k++) {
+    if (parts[k].n_edges && !(parts[k].offsets && parts[k].indices))
+      return refuse_plan("null graph array in a plan part");
+    if ((uint64_t)parts[k].row_add + parts[k].n_rows > n_rows)
+      return refuse_plan("plan part rows exceed the output rows");
+  }
+  if (n_slabs >= 1)
+    return build_plan(parts, n_parts, n_rows, gather_rows, n_slabs, 0, 0, as_stream(stream));
+  return tune_plan(parts, n_parts, n_rows, gather_rows, feature_size, false, 0, false, as_stream(stream));
+}
+
+float nts_gather_plan_tuned_ms(const nts_gather_plan *pl) { return pl ? pl->tuned_ms : 0.f; }
 
 int nts_gather_plan_destroy(nts_gather_plan *pl) {
   if (!pl)
@@ -1985,23 +1754,12 @@ int nts_gather_plan_last_launch(const nts_gather_plan *pl, int *launches, int *g
   return 0;
 }
 
-int nts_gather_plan_run(nts_gather_plan *pl, const float *input, float *output, nts_vid_t feature_size, void *stream) {
-  NTS_ARG_CHECK(pl != nullptr, "null plan");
-  return run_plan(pl, input, feature_size, output, feature_size, 0, as_stream(stream));
-}
-
 int nts_gather_plan_run_ex(nts_gather_plan *pl, const float *input, nts_vid_t input_ld, float *output,
                            nts_vid_t feature_size, int flags, void *stream) {
   NTS_ARG_CHECK(input_ld >= feature_size, "input row pitch below the feature width");
   NTS_ARG_CHECK(output != nullptr || feature_size == 0, "null output pointer");
   NTS_ARG_CHECK(pl != nullptr, "null plan");
   return run_plan(pl, input, input_ld, output, feature_size, flags, as_stream(stream));
-}
-
-int nts_gather_plan_run_bf16(nts_gather_plan *pl, const void *input, int input_dtype, float *output,
-                             nts_vid_t feature_size, void *stream) {
-  NTS_ARG_CHECK(pl != nullptr, "null plan");
-  return run_plan_bf16(pl, input, input_dtype, feature_size, output, feature_size, as_stream(stream));
 }
 
 int nts_gather_plan_run_bf16_ex(nts_gather_plan *pl, const void *input, int input_dtype, nts_vid_t input_ld,

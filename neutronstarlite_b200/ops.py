@@ -149,7 +149,7 @@ class GatherPlan:
                 0 if tune_accumulate else PLAN_OVERWRITE, _stream())
         self.build_s = _time.perf_counter() - t0      # create synchronises the stream
         if not self.handle:
-            raise _lib.NtsError("nts_gather_plan_create failed: " + L.nts_last_error().decode(errors="replace"))
+            raise _lib.NtsError("gather plan construction failed: " + L.nts_last_error().decode(errors="replace"))
         self.slabs = int(L.nts_gather_plan_slabs(self.handle))
         hc, hr = C.c_int(0), C.c_int(0)
         _lib.call("nts_gather_plan_hubs", self.handle, C.byref(hc), C.byref(hr))

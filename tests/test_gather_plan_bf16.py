@@ -1,4 +1,4 @@
-"""BF16 gathers with FP32 accumulation (nts_gather_plan_run_bf16, csrc/nts_plan.cu) and the options above them.
+"""BF16 gathers with FP32 accumulation (nts_gather_plan_run_bf16_ex, csrc/nts_plan.cu) and the options above them.
 
 Precision contract: out[r,:] += sum_e w(e) * float(bf16(x[src(e),:])), bf16() = round to nearest even exactly as
 torch's x.to(torch.bfloat16); weights, accumulation and outputs FP32.  So every result is checked against the C oracle

@@ -39,7 +39,7 @@ for variant in (0, 1):
             ops.gather_by_src_from_dst(c, torch.zeros_like(x), x)
         c.__dict__.pop("_gather_plans", None)
 _lib.call("nts_gather_plan_set_variant", 0)
-ops.set_plan_mode("on", 0)                      # measured slab count (nts_gather_plan_create_tuned)
+ops.set_plan_mode("on", 0)                      # measured slab count (nts_gather_plan_create_tuned_ex)
 x = torch.rand((V, 128), device=dev)
 ops.gather_by_dst_from_src(c, torch.zeros_like(x), x)
 ops.set_plan_mode("auto")
