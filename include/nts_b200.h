@@ -96,8 +96,8 @@ int nts_gather_by_src_from_dst(const float *input, float *output, const float *w
 
 /* Row-range launch of the same contraction: `offsets` points at the first row of the range (offsets[0] ==
  * edge_begin, offsets[n_rows] == edge_end), `output` at its first output row; indices / weight stay the whole
- * arrays (addressed by absolute edge position).  Used by the exchange engine to aggregate the remote chunks in
- * pipeline stages (core/graph.hpp:3678-3719 processes one chunk per ring step). */
+ * arrays (addressed by absolute edge position), row(e) = slot_of ? slot_of[indices[e]] : indices[e] - index_base.
+ * Output rows outside the range are not touched, so a chunk can be aggregated one block of rows at a time. */
 int nts_segment_gather_sum_range(const float *input, float *output, const float *weight, const nts_vid_t *indices,
                                  const nts_vid_t *offsets, const nts_vid_t *slot_of, nts_vid_t index_base,
                                  nts_vid_t n_rows, uint64_t edge_begin, uint64_t edge_end, nts_vid_t feature_size,
@@ -214,6 +214,9 @@ int nts_segment_gather_sum_heads(const float *input, float *output, const float 
  * re-association): variant 0 = auto, see DESIGN.md "kernel variants". */
 int nts_aggregate_set_variant(int variant, int edges_per_warp);
 int nts_aggregate_last_launch(int *grid, int *block, int *smem_bytes, int *variant);
+/* Template point of the last launch: floats (BF16 values for the BF16 fused GAT forward) per vector load, vector chunks
+ * per lane, edges loaded before their FMAs (U), __launch_bounds__ minimum CTAs per SM, and column tiles. */
+int nts_aggregate_last_shape(int *vec, int *k, int *u, int *min_blocks, int *tiles);
 uint64_t nts_kernel_launch_count(void); /* kernels launched by this library since load */
 
 /* ---- edge-granular operators (GAT building blocks) -------------------------------------------------

@@ -69,6 +69,7 @@ SIGNATURES = {
     "nts_segment_gather_sum_heads": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _u64, _u32, _u32, _vp]),
     "nts_aggregate_set_variant": (_int, [_int, _int]),
     "nts_aggregate_last_launch": (_int, [C.POINTER(_int)] * 4),
+    "nts_aggregate_last_shape": (_int, [C.POINTER(_int)] * 5),
     "nts_kernel_launch_count": (_u64, []),
     "nts_scatter_src_mirror_to_msg": (_int, [_vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp]),
     "nts_gather_msg_to_src_mirror": (_int, [_vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp]),

@@ -38,6 +38,7 @@ namespace nts {
 static int g_variant = 0;          // 0 = auto
 static int g_edges_per_warp = 0;   // 0 = auto
 static int g_last_grid = 0, g_last_block = 0, g_last_smem = 0, g_last_variant = 0;
+static int g_last_vec = 0, g_last_k = 0, g_last_u = 0, g_last_minb = 0, g_last_tiles = 0; // instantiation of the last launch
 
 // ---- small device helpers --------------------------------------------------------------------------------
 __device__ __forceinline__ void fma_vec(float &a, float w, float x) { a = fmaf(w, x, a); }
@@ -498,6 +499,7 @@ static int launch_shape(bool bulk, const LaunchShape &sh, const float *in, float
   NTS_ARG_CHECK(blocks <= 0x7fffffffull, "aggregation grid too large");
   g_last_grid = (int)blocks;
   g_last_block = kWarpsPerBlock * 32;
+  g_last_vec = VEC, g_last_k = K, g_last_u = U, g_last_minb = MINB, g_last_tiles = (int)sh.tiles;
   if (att || sh.heads > 1) {
     if constexpr (MINB == 1) { // per-head kernels exist for the untuned occupancy points only
       g_last_smem = 0;
@@ -669,6 +671,7 @@ static int launch_gat_bf16(const LaunchShape &sh, const __nv_bfloat16 *in, float
   g_last_block = kWarpsPerBlock * 32;
   g_last_smem = (int)smem;
   g_last_variant = 2;
+  g_last_vec = 8, g_last_k = K, g_last_u = U, g_last_minb = 1, g_last_tiles = (int)sh.tiles;
   kern<<<(unsigned)blocks, kWarpsPerBlock * 32, smem, st>>>(in, out, nullptr, idx, off, slot_of, 0, n_rows, n_edges,
                                                             ld, Q, sh.tiles, sh.tile_vecs, 0, sh.heads, att, 0, 0);
   NTS_LAUNCH_CHECK();
@@ -843,6 +846,20 @@ int nts_aggregate_last_launch(int *grid, int *block, int *smem_bytes, int *varia
     *smem_bytes = nts::g_last_smem;
   if (variant)
     *variant = nts::g_last_variant;
+  return 0;
+}
+
+int nts_aggregate_last_shape(int *vec, int *k, int *u, int *min_blocks, int *tiles) {
+  if (vec)
+    *vec = nts::g_last_vec;
+  if (k)
+    *k = nts::g_last_k;
+  if (u)
+    *u = nts::g_last_u;
+  if (min_blocks)
+    *min_blocks = nts::g_last_minb;
+  if (tiles)
+    *tiles = nts::g_last_tiles;
   return 0;
 }
 

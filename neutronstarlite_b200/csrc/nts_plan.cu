@@ -1141,8 +1141,9 @@ static int run_gather(nts_gather_plan *pl, const T *in, uint32_t ld, float *outp
   const float4 *in4 = reinterpret_cast<const float4 *>(in);
   const uint32_t ld4 = ldc;
   if (g_plan_variant == 1) { // TMA row staging (measurement variant): U = ring depth
+    // occupancy as for variant 0 (or set_tuning's): 4 / 3 / 2 CTAs per SM at 1 / 2 / 3+ chunks per lane, each with a
+    // ring of 4 stages (2 at 4 chunks) at the default U
     const int stages = sh.u >= 8 ? 8 : (sh.u >= 4 ? 4 : 2);
-    sh.minb = g_plan_minb > 0 ? g_plan_minb : (sh.k >= 4 ? 2 : 4);
     NTS_PLAN_TMA_CASE(1, 8, 4)
     NTS_PLAN_TMA_CASE(1, 4, 4)
     NTS_PLAN_TMA_CASE(1, 8, 3)

@@ -46,6 +46,16 @@ def test_argument_errors_are_reported_not_swallowed():
     assert lib.nts_aggregate_set_variant(0, 0) == 0
 
 
+def test_aggregate_launch_record_takes_null_outputs():
+    """nts_aggregate_last_shape fills what it is given and skips null pointers; before any launch it reports zeros."""
+    import ctypes as C
+    lib = _lib.load()
+    assert lib.nts_aggregate_last_shape(None, None, None, None, None) == 0
+    vals = [C.c_int(-1) for _ in range(5)]
+    assert lib.nts_aggregate_last_shape(*[C.byref(v) for v in vals]) == 0
+    assert all(v.value >= 0 for v in vals)
+
+
 def test_empty_chunks_are_a_no_op_before_any_pointer_is_looked_at():
     """A rank that owns no vertices (or a chunk without edges) hands the aggregation entries empty tensors, whose data
     pointers are NULL: the entries must return success without touching CUDA or complaining about the pointers."""
