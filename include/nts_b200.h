@@ -366,6 +366,15 @@ int nts_aggregate_records(float *aggregate, const float *records, nts_vid_t n_re
 /* dst[k,:] = src[rows[k],:]   (sender-side compaction of mirror rows / pull from a peer's mapped buffer) */
 int nts_gather_rows(float *dst, const float *src, const nts_vid_t *rows, nts_vid_t n_rows,
                     nts_vid_t feature_size, void *stream);
+/* dst[k,:] = shards[o][ids[k] - shard_offsets[o], :feature_size] for k < n, o the shard that owns ids[k]: a gather by
+ * global row id from a table split into n_shards (1..32) row ranges [shard_offsets[o], shard_offsets[o+1]) (device
+ * array of n_shards+1 non-decreasing values; empty shards allowed), shard o stored at `shards[o]` (device array of
+ * pointers, local or peer memory, each 16-byte aligned) with shard_pitch floats per row (shard_pitch % 4 == 0,
+ * >= feature_size).  dst is [n, feature_size] contiguous.  Ids may repeat and come in any order; every id must lie in
+ * [shard_offsets[0], shard_offsets[n_shards]) (not checked on the device).  n == 0 launches nothing. */
+int nts_gather_rows_sharded(float *dst, const float *const *shards, const nts_vid_t *shard_offsets, int n_shards,
+                            nts_vid_t shard_pitch, const nts_vid_t *ids, nts_vid_t n, nts_vid_t feature_size,
+                            void *stream);
 /* dst[rows[k],:] += src[k,:]  (receiver-side add of partial gradients; rows must be unique) */
 int nts_scatter_add_rows(float *dst, const float *src, const nts_vid_t *rows, nts_vid_t n_rows,
                          nts_vid_t feature_size, void *stream);

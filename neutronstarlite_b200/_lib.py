@@ -90,6 +90,7 @@ SIGNATURES = {
     "nts_deserialize_records": (_int, [_vp, _vp, _u32, _u32, _u32, _u32, _vp]),
     "nts_aggregate_records": (_int, [_vp, _vp, _u32, _u32, _u32, _u32, _vp]),
     "nts_gather_rows": (_int, [_vp, _vp, _vp, _u32, _u32, _vp]),
+    "nts_gather_rows_sharded": (_int, [_vp, _vp, _vp, _int, _u32, _vp, _u32, _u32, _vp]),
     "nts_scatter_add_rows": (_int, [_vp, _vp, _vp, _u32, _u32, _vp]),
     "nts_scatter_add_rows_atomic": (_int, [_vp, _vp, _vp, _u32, _u32, _vp]),
     "nts_ipc_get_handle": (_int, [_vp, C.c_char_p]),

@@ -7,6 +7,8 @@
 // split by EDGES (a warp owns a quantum of consecutive edges and finds its destination rows by
 // binary search over column_offset), and uses atomics only where two edges of different
 // destinations meet in one mirror row.
+#include <algorithm>
+
 #include "nts_common.cuh"
 
 namespace nts {
@@ -111,6 +113,90 @@ __global__ void __launch_bounds__(kThreads)
       }
     }
   }
+}
+
+// ---- row gather from a table sharded by global row ranges ----------------------------------------------------
+// dst[k,:F] = shards[o][ids[k] - off[o], :F], o = the shard with off[o] <= ids[k] < off[o+1] (binary search over the
+// offsets staged in shared memory; empty shards have off[o] == off[o+1] and are never chosen).  Shard rows are `pitch`
+// floats with pitch % 4 == 0 and every shard 16-byte aligned, so each lane loads whole float4s, the last one of a row
+// reaching into its padding; stores are SVEC floats wide (dst is [n, F], so F's alignment decides).  A row takes
+// LANES lanes (a virtual warp of a warp for rows of at most 8 / 16 float4s, as in the planned kernel), and each lane
+// issues up to kGatherUnroll loads before it stores them.
+constexpr int kMaxShards = 32;
+constexpr int kGatherUnroll = 4;
+
+template <int SVEC> __device__ __forceinline__ void store_vec4(float *d, uint32_t col, float4 v, uint32_t F);
+template <> __device__ __forceinline__ void store_vec4<4>(float *d, uint32_t col, float4 v, uint32_t) {
+  *reinterpret_cast<float4 *>(d + col) = v;
+}
+template <> __device__ __forceinline__ void store_vec4<2>(float *d, uint32_t col, float4 v, uint32_t F) {
+  *reinterpret_cast<float2 *>(d + col) = make_float2(v.x, v.y);
+  if (col + 2 < F)
+    *reinterpret_cast<float2 *>(d + col + 2) = make_float2(v.z, v.w);
+}
+template <> __device__ __forceinline__ void store_vec4<1>(float *d, uint32_t col, float4 v, uint32_t F) {
+  d[col] = v.x;
+  if (col + 1 < F)
+    d[col + 1] = v.y;
+  if (col + 2 < F)
+    d[col + 2] = v.z;
+  if (col + 3 < F)
+    d[col + 3] = v.w;
+}
+
+template <int LANES, int SVEC>
+__global__ void __launch_bounds__(kThreads)
+    gather_rows_sharded_kernel(float *__restrict__ dst, const float *const *__restrict__ shards,
+                               const uint32_t *__restrict__ offsets, int n_shards, uint32_t pitch,
+                               const uint32_t *__restrict__ ids, uint32_t n, uint32_t F) {
+  __shared__ uint32_t s_off[kMaxShards + 1];
+  __shared__ const float *s_shard[kMaxShards];
+  for (int i = threadIdx.x; i <= n_shards; i += blockDim.x) {
+    s_off[i] = __ldg(offsets + i);
+    if (i < n_shards)
+      s_shard[i] = shards[i];
+  }
+  __syncthreads();
+  constexpr uint32_t kRowsPerBlock = kThreads / LANES;
+  const uint32_t sub = threadIdx.x & (LANES - 1);
+  const uint32_t nvec = (F + 3) / 4;
+  for (uint64_t k = (uint64_t)blockIdx.x * kRowsPerBlock + threadIdx.x / LANES; k < n;
+       k += (uint64_t)gridDim.x * kRowsPerBlock) {
+    const uint32_t id = __ldg(ids + k);
+    int lo = 0, hi = n_shards;
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (s_off[mid] <= id)
+        lo = mid;
+      else
+        hi = mid;
+    }
+    const float4 *s = reinterpret_cast<const float4 *>(s_shard[lo] + (size_t)(id - s_off[lo]) * pitch);
+    float *d = dst + (size_t)k * F;
+    for (uint32_t c0 = sub; c0 < nvec; c0 += kGatherUnroll * LANES) {
+      float4 v[kGatherUnroll];
+#pragma unroll
+      for (int u = 0; u < kGatherUnroll; u++)
+        if (c0 + u * LANES < nvec)
+          v[u] = __ldg(s + c0 + u * LANES);
+#pragma unroll
+      for (int u = 0; u < kGatherUnroll; u++)
+        if (c0 + u * LANES < nvec)
+          store_vec4<SVEC>(d, 4 * (c0 + u * LANES), v[u], F);
+    }
+  }
+}
+
+template <int LANES>
+static void launch_gather_rows_sharded(int svec, unsigned grid, cudaStream_t st, float *dst, const float *const *shards,
+                                       const uint32_t *offsets, int n_shards, uint32_t pitch, const uint32_t *ids,
+                                       uint32_t n, uint32_t F) {
+  if (svec == 4)
+    gather_rows_sharded_kernel<LANES, 4><<<grid, kThreads, 0, st>>>(dst, shards, offsets, n_shards, pitch, ids, n, F);
+  else if (svec == 2)
+    gather_rows_sharded_kernel<LANES, 2><<<grid, kThreads, 0, st>>>(dst, shards, offsets, n_shards, pitch, ids, n, F);
+  else
+    gather_rows_sharded_kernel<LANES, 1><<<grid, kThreads, 0, st>>>(dst, shards, offsets, n_shards, pitch, ids, n, F);
 }
 
 // msg[e,:] (=|+=) x[dst(e),:] : destination row broadcast over its CSC segment
@@ -910,6 +996,32 @@ extern "C" {
 int nts_gather_rows(float *dst, const float *src, const nts_vid_t *rows, nts_vid_t n_rows, nts_vid_t feature_size,
                     void *stream) {
   return move_rows<0>(dst, src, rows, nullptr, n_rows, nullptr, feature_size, as_stream(stream));
+}
+
+int nts_gather_rows_sharded(float *dst, const float *const *shards, const nts_vid_t *shard_offsets, int n_shards,
+                            nts_vid_t shard_pitch, const nts_vid_t *ids, nts_vid_t n, nts_vid_t feature_size,
+                            void *stream) {
+  if (n == 0 || feature_size == 0)
+    return 0;
+  NTS_ARG_CHECK(dst && shards && shard_offsets && ids, "null pointer passed to nts_gather_rows_sharded");
+  NTS_ARG_CHECK(n_shards >= 1 && n_shards <= kMaxShards, "nts_gather_rows_sharded needs 1..32 shards");
+  NTS_ARG_CHECK(shard_pitch % 4 == 0 && shard_pitch >= feature_size,
+                "nts_gather_rows_sharded: shard_pitch must be a multiple of 4 and at least feature_size");
+  const uint32_t F = feature_size, nvec = (F + 3) / 4;
+  const int svec = pick_vec(F, dst, dst);
+  const int lanes = nvec <= 8 ? 8 : (nvec <= 16 ? 16 : 32);
+  const uint64_t rows_per_block = kThreads / lanes;
+  const uint64_t cap = (uint64_t)sm_count() * 16;
+  const unsigned grid = (unsigned)std::min<uint64_t>((n + rows_per_block - 1) / rows_per_block, cap);
+  cudaStream_t st = as_stream(stream);
+  if (lanes == 8)
+    launch_gather_rows_sharded<8>(svec, grid, st, dst, shards, shard_offsets, n_shards, shard_pitch, ids, n, F);
+  else if (lanes == 16)
+    launch_gather_rows_sharded<16>(svec, grid, st, dst, shards, shard_offsets, n_shards, shard_pitch, ids, n, F);
+  else
+    launch_gather_rows_sharded<32>(svec, grid, st, dst, shards, shard_offsets, n_shards, shard_pitch, ids, n, F);
+  NTS_LAUNCH_CHECK();
+  return 0;
 }
 
 int nts_scatter_add_rows(float *dst, const float *src, const nts_vid_t *rows, nts_vid_t n_rows,

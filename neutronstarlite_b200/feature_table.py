@@ -1,0 +1,145 @@
+"""A [V, F] float32 feature table sharded by row ranges over the GPUs of one node, read by global row id from any rank.
+
+`ShardedFeatureTable(local_rows, offsets, group)` is collective over the process group: rank r owns rows
+[offsets[r], offsets[r+1]) (any non-decreasing split of [0, V), empty shards allowed; the callers' default is
+graph.partition_offsets_from_out_degree, the reference's partitioner) and keeps them in one device buffer of its own
+at a pitch of 4*ceil(F/4) floats.  The ranks exchange CUDA-IPC handles of these buffers once, so that every rank maps
+every other rank's shard (peer memory, reached over NVLink between GPUs), and `gather(ids)` reads the rows of any ids
+with one launch of nts_gather_rows_sharded (include/nts_b200.h).  A torch caching-allocator tensor cannot be exported
+as it is (an IPC handle names the allocation's base, not the sub-block), hence the table's own buffer.
+
+Scope is one node: at most 32 ranks in one CUDA-IPC domain, as for the exchange engine (exchange.py).  With one rank
+(or no process group) the table is a single shard and `gather` is a local gather."""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+import torch
+import torch.distributed as dist
+
+from . import _lib
+from .sample import _DeviceArray, _stream
+
+MAX_SHARDS = 32
+
+
+def _group_rank_world(group):
+    if not dist.is_initialized():
+        return 0, 1
+    return dist.get_rank(group), dist.get_world_size(group)
+
+
+class ShardedFeatureTable:
+    """See the module docstring.  Attributes: rows (V), F, pitch, offsets ([world+1] numpy), rank, world, group,
+    device."""
+
+    def __init__(self, local_rows, offsets, group=None):
+        self.group = group
+        self.rank, self.world = _group_rank_world(group)
+        if self.world > MAX_SHARDS:
+            raise _lib.NtsError("a sharded feature table spans at most %d ranks, the group has %d"
+                                % (MAX_SHARDS, self.world))
+        off = np.asarray(offsets, dtype=np.int64).reshape(-1)
+        if off.size != self.world + 1 or off[0] != 0 or (np.diff(off) < 0).any() or off[-1] >= 2 ** 32:
+            raise _lib.NtsError("offsets must be %d non-decreasing row ids starting at 0, got %s"
+                                % (self.world + 1, off.tolist()))
+        x = local_rows.detach()
+        if not x.is_cuda or x.dtype != torch.float32 or x.dim() != 2:
+            raise _lib.NtsError("local_rows must be a 2-D float32 CUDA tensor")
+        lo, hi = int(off[self.rank]), int(off[self.rank + 1])
+        if x.shape[0] != hi - lo:
+            raise _lib.NtsError("rank %d owns rows [%d, %d) but local_rows has %d rows" % (self.rank, lo, hi, x.shape[0]))
+        self.offsets, self.rows, self.F = off, int(off[-1]), int(x.shape[1])
+        self.pitch = (self.F + 3) // 4 * 4
+        self.device = x.device
+        self._peers = []
+        L = _lib.load()
+        n = (hi - lo) * self.pitch
+        self._buf = L.nts_malloc_device(max(n, 4) * 4)
+        if not self._buf:
+            raise _lib.NtsError("nts_malloc_device failed: " + L.nts_last_error().decode(errors="replace"))
+        try:
+            if n:
+                mine = torch.as_tensor(_DeviceArray(self._buf, n, "<f4"), device=self.device).view(hi - lo, self.pitch)
+                mine[:, self.F:].zero_()
+                mine[:, :self.F].copy_(x)
+            ptrs = [self._buf] * self.world
+            if self.world > 1:
+                # the copy is complete before any peer can map the buffer: every rank passes this point first
+                torch.cuda.current_stream(self.device).synchronize()
+                h = C.create_string_buffer(64)
+                _lib.call("nts_ipc_get_handle", self._buf, h)
+                info = [None] * self.world
+                dist.all_gather_object(info, (bytes(h.raw), self.F), group=group)
+                widths = sorted(set(f for _, f in info))
+                if len(widths) != 1:
+                    raise _lib.NtsError("the ranks' local_rows have different widths: %s" % widths)
+                for j, (hj, _) in enumerate(info):
+                    if j == self.rank:
+                        continue
+                    p = L.nts_ipc_open_handle(hj)
+                    if not p:
+                        raise _lib.NtsError("nts_ipc_open_handle failed: " + L.nts_last_error().decode(errors="replace"))
+                    self._peers.append(p)
+                    ptrs[j] = p
+            self._shards = torch.tensor(ptrs, dtype=torch.int64).to(self.device)
+            self._offsets = torch.from_numpy(off.astype(np.uint32).view(np.int32)).to(self.device)
+        except Exception:
+            self._release()
+            raise
+
+    def gather(self, ids):
+        """Rows of the global ids `ids` (any integer tensor, numpy array or list; any order, repeats allowed) as a
+        [n, F] float32 tensor on this rank's device.  Ids outside [0, V) raise NtsError before any device work."""
+        if torch.is_tensor(ids) and ids.is_cuda:
+            if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
+                raise _lib.NtsError("ids must be an integer tensor, not %s" % ids.dtype)
+            # range check in the caller's dtype: a cast first could wrap an int64 id >= 2^32 into [0, V)
+            if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= self.rows):
+                raise _lib.NtsError("row ids must be in [0, %d)" % self.rows)
+            t = ids.reshape(-1).to(device=self.device, dtype=torch.int32).contiguous()
+        else:
+            a = np.asarray(ids.numpy() if torch.is_tensor(ids) else ids).reshape(-1).astype(np.int64)
+            if a.size and (a.min() < 0 or a.max() >= self.rows):
+                raise _lib.NtsError("row ids must be in [0, %d)" % self.rows)
+            t = torch.from_numpy(a.astype(np.int32)).to(self.device)
+        return self._gather(t)
+
+    def _gather(self, ids):
+        """gather() without the range check, for ids known to be in [0, V): a contiguous int32 device tensor holding
+        uint32 values (a sampled block's src)."""
+        if self._buf is None:
+            raise _lib.NtsError("the feature table is closed")
+        n = int(ids.numel())
+        out = torch.empty((n, self.F), dtype=torch.float32, device=self.device)
+        _lib.call("nts_gather_rows_sharded", out.data_ptr(), self._shards.data_ptr(), self._offsets.data_ptr(),
+                  self.world, self.pitch, ids.data_ptr() if n else None, n, self.F, _stream())
+        return out
+
+    def close(self):
+        """Collective: synchronise this device, a barrier (no rank is still reading a peer's shard), then close the
+        peer mappings and free this rank's buffer."""
+        if self._buf is None:
+            return
+        torch.cuda.synchronize(self.device)
+        if self.world > 1:
+            dist.barrier(group=self.group)
+        self._release()
+
+    def _release(self):
+        L = _lib.load()
+        for p in self._peers:
+            L.nts_ipc_close_handle(p)
+        self._peers = []
+        if self._buf:
+            L.nts_free_device(self._buf)
+        self._buf = None
+
+    def __del__(self):
+        # without close() a peer may still read this rank's shard: free it only when there is no peer
+        try:
+            if getattr(self, "_buf", None) and self.world == 1:
+                self._release()
+        except Exception:
+            pass

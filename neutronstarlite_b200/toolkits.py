@@ -7,9 +7,10 @@
   * `GCNEagerImpl` <-> toolkits/GCN_EAGER_single.hpp / GCN_EAGER.hpp order (X.W first, aggregate the narrow result).
   * `GATImpl`    <-> the flow of toolkits/GAT_CPU_DIST_OPTM.hpp on the fused multi-head aggregation (K7).
   * `GCNSampleImpl` <-> toolkits/GCN_CPU_SAMPLE.hpp (neighbour-sampled mini-batch GCN) on the K8 sampler and
-                     ops.MiniBatchFuseOp, one GPU.
+                     ops.MiniBatchFuseOp, on one GPU or data-parallel over a feature_table.ShardedFeatureTable.
   * `GATSampleImpl` <-> GATImpl's layers on GCNSampleImpl's batch loop: neighbour-sampled mini-batch GAT on the K8
-                     sampler (destination-inclusive blocks) and K7 through ops.MiniBatchGATOp, one GPU.
+                     sampler (destination-inclusive blocks) and K7 through ops.MiniBatchGATOp, on one GPU or
+                     data-parallel like GCNSampleImpl.
 
 Dense NN work (mm, relu, log_softmax, nll_loss, Adam element-wise) stays on torch/cuBLAS exactly as in the
 reference (libtorch); the aggregation goes through libnts_b200."""
@@ -249,7 +250,119 @@ def _minibatch_op(sampled_subgraph, active, hop, table=False):
     return ops.MiniBatchFuseOp(sampled_subgraph, hop, table=table)
 
 
-class GCNSampleImpl:
+class _SampledRounds:
+    """The batch loop shared by GCNSampleImpl and GATSampleImpl, on one GPU or data-parallel over the ranks of a
+    feature_table.ShardedFeatureTable.
+
+    A pass cuts the ascending ids of one mask value into batches of batch_size.  Batch b of a pass samples with step
+    base + b, and base advances by the pass's batch count on every rank, so at world 1 the steps are those of a run
+    with a tensor.  With a table over N ranks the pass runs in rounds: round t runs batch t*N + r on rank r.  Every
+    training round ends in one Adam step per parameter on every rank, after Parameter.all_reduce_to_gradient has
+    SUM-reduced the gradients over the ranks in the same parameter order everywhere (the reference's semantics: the
+    effective step grows with N).  A rank without a batch in the last round contributes zero gradients and still joins
+    every collective.  Mean loss and accuracies are reduced over the ranks at the end of a pass, so every rank returns
+    the same numbers.  Topology, labels and mask are whole-graph on every rank (the reference's FullyRepGraph)."""
+
+    def _init_features(self, features, vertices):
+        from .feature_table import ShardedFeatureTable
+        if not isinstance(features, ShardedFeatureTable):
+            self.table, self.rank, self.world = None, 0, 1
+            self.features = ops._check_input(features.detach(), "features")
+            self.device = features.device
+            return
+        if features.rows != vertices:
+            raise _lib.NtsError("the feature table has %d rows, the graph has %d vertices" % (features.rows, vertices))
+        if features.world != (dist.get_world_size() if dist.is_initialized() else 1):
+            # Parameter reduces gradients over the default group
+            raise _lib.NtsError("the feature table's group must span every rank of the default process group")
+        self.table, self.features, self.device = features, None, features.device
+        self.rank, self.world = features.rank, features.world
+
+    def _input_rows(self, src):
+        """Features of the sampled sources `src` (global ids of a block, from the sampler: in range)."""
+        if self.table is None:
+            return self.features.index_select(0, src.long())
+        return self.table._gather(src)
+
+    def _batches(self, ids):
+        """The seeds this rank runs in each round of a pass over `ids` (None in a round without a batch for it); sets
+        the step of every batch and leaves self.step at the next pass's base."""
+        bs = self.batch_size
+        n_batches = -(-ids.numel() // bs)
+        base = self.step
+        for t in range(-(-n_batches // self.world)):
+            b = t * self.world + self.rank
+            if b < n_batches:
+                self.step = base + b
+                yield ids[b * bs:(b + 1) * bs]
+            else:
+                yield None
+        self.step = base + n_batches
+
+    def _totals(self, *values):
+        """The values (scalars or one-element tensors) summed over the ranks, as floats."""
+        if self.world == 1:
+            return [float(v) for v in values]
+        dev = self.device if dist.get_backend(self.table.group) == "nccl" else torch.device("cpu")
+        t = torch.tensor([float(v) for v in values], dtype=torch.float64, device=dev)
+        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.table.group)
+        return t.tolist()
+
+    def Update(self):
+        """all_reduce_to_gradient, Adam and next() for every parameter.  At world 1 a parameter without a gradient is
+        skipped; data-parallel, every rank reduces and steps every parameter (a missing gradient counts as zeros), so
+        that the collectives are the same on every rank."""
+        for p in self.params():
+            g = p.W.grad
+            if g is None:
+                if self.world == 1:
+                    continue
+                g = torch.zeros_like(p.W)
+            p.all_reduce_to_gradient(g)
+            p.learn_with_decay_Adam()
+            p.next()
+
+    def evaluate(self, s):
+        """Accuracy over mask == s from sampled forwards (no dropout, no update)."""
+        self.ctx.eval()
+        correct = torch.zeros((), dtype=torch.int64, device=self.device)
+        ids = self.nids[s]
+        with torch.no_grad():
+            for seeds in self._batches(ids):
+                if seeds is not None:
+                    out = self.Forward(seeds, False)
+                    correct += (out.argmax(1) == self.L_GT.index_select(0, self.subgraph.seeds().long())).sum()
+        self.ctx.train()
+        return self._totals(correct)[0] / max(ids.numel(), 1)
+
+    def run_epoch(self, test=True):
+        """One pass over the train batches (one Adam step per round) and, with test=True, sampled validation and test
+        forwards.  Returns (mean train loss, [train, val, test] accuracy) - val / test are None with test=False."""
+        ids = self.nids[0]
+        losses, correct = [], torch.zeros((), dtype=torch.int64, device=self.device)
+        for seeds in self._batches(ids):
+            if seeds is None:
+                for p in self.params():
+                    p.zero_grad()
+                self.Update()
+                continue
+            loss, c = self.train_step(seeds)
+            losses.append(loss)
+            correct += c
+        if self.world == 1:
+            mean_loss = float(torch.stack(losses).mean()) if losses else float("nan")
+            total = float(correct)
+        else:
+            n_batches = -(-ids.numel() // self.batch_size)
+            loss_sum, total = self._totals(torch.stack(losses).double().sum() if losses else 0.0, correct)
+            mean_loss = loss_sum / n_batches if n_batches else float("nan")
+        acc = [total / max(ids.numel(), 1)]
+        acc += [self.evaluate(1), self.evaluate(2)] if test else [None, None]
+        self.epoch += 1
+        return mean_loss, acc
+
+
+class GCNSampleImpl(_SampledRounds):
     """Neighbour-sampled mini-batch GCN: toolkits/GCN_CPU_SAMPLE.hpp:150-289 (ALGORITHM:GCNSAMPLESINGLE) on the GPU.
     The train vertices (mask == 0), in id order, are cut into batches of `batch_size` seeds; each batch is sampled
     (sample.NeighborSampler, hop h with fanout[h]) and runs an L-layer GCN over hops L-1 .. 0 (layer l aggregates hop
@@ -262,7 +375,12 @@ class GCNSampleImpl:
     (seed, t): two runs with the same seeds sample the same blocks, bit for bit.  Losses and weights agree bit for bit
     only while no aggregation row is cut into three or more pieces by K1's edge quanta (rows longer than the quantum,
     at least 32 edges on small blocks); such rows sum in scheduling order and may differ in the last bits between
-    runs (DESIGN.md §3 K8)."""
+    runs (DESIGN.md §3 K8).
+
+    features: the [V, F] tensor, or a feature_table.ShardedFeatureTable for data-parallel rounds over its ranks
+    (_SampledRounds); the first layer then gathers the deepest hop's distinct sources from the table once
+    (nts_gather_rows_sharded) and aggregates them on local ids with K1.  `partitioned_graph` is the whole graph as a
+    single partition on every rank."""
 
     def __init__(self, partitioned_graph, layers, features, labels, mask, fanout, batch_size, learn_rate=0.01,
                  weight_decay=0.0001, decay_rate=0.97, decay_epoch=100, drop_rate=0.5, seed=0, sample_seed=0):
@@ -274,7 +392,7 @@ class GCNSampleImpl:
             raise _lib.NtsError("batch_size must be >= 1")
         from .sample import NeighborSampler
         self.sampler = NeighborSampler(partitioned_graph, fanout, self.batch_size)
-        self.device = features.device
+        self._init_features(features, self.sampler.V)
         self.drop_rate = drop_rate
         self.sample_seed = int(sample_seed)
         self.step = 0
@@ -287,7 +405,6 @@ class GCNSampleImpl:
             p.init_parameter()
             p.set_decay(decay_rate, decay_epoch)
             self.P.append(p)
-        self.features = ops._check_input(features.detach(), "features")
         self.L_GT = labels.to(self.device)
         mask = torch.as_tensor(mask).cpu()
         self.nids = [(mask == s).nonzero().view(-1) for s in (0, 1, 2)]    # train / val / test ids, ascending
@@ -295,19 +412,23 @@ class GCNSampleImpl:
         self.loss = None
         self.epoch = 0
 
+    def params(self):
+        return self.P
+
     def Forward(self, seeds, training):
         """Sample the batch and run the layers; returns the last layer's [n_seeds, classes] output."""
         self.subgraph = sg = self.sampler.sample(seeds, self.sample_seed, self.step)
         self.step += 1
         L = len(self.layers) - 1
-        x = self.features
+        x = self.features if self.table is None else self._input_rows(sg.blocks[L - 1].src)
         for l in range(L):
             hop = L - 1 - l
             if l != 0 and training and self.drop_rate > 0:
                 dropped = torch.nn.functional.dropout(x, self.drop_rate, training=True)
                 self.ctx.appendNNOp(x, dropped)
                 x = dropped
-            y = self.ctx.runGraphOp(_minibatch_op, sg, None, x.contiguous(), hop=hop, table=l == 0)
+            y = self.ctx.runGraphOp(_minibatch_op, sg, None, x.contiguous(), hop=hop,
+                                    table=l == 0 and self.table is None)
             if l == L - 1:
                 x = self.ctx.runVertexForward(lambda n, _l=l: self.P[_l].forward(n), y)
             else:
@@ -319,12 +440,6 @@ class GCNSampleImpl:
         self.loss = torch.nn.functional.nll_loss(out.log_softmax(1), self.L_GT.index_select(0, seeds_dev))
         self.ctx.appendNNOp(out, self.loss)
         return self.loss
-
-    def Update(self):
-        for p in self.P:
-            p.all_reduce_to_gradient(p.W.grad)
-            p.learn_with_decay_Adam()
-            p.next()
 
     def train_step(self, seeds):
         """One batch: zero the gradients, sample, forward, loss, tape backward, Adam.  Returns (loss, correct)."""
@@ -338,33 +453,6 @@ class GCNSampleImpl:
         self.ctx.self_backward(False)
         self.Update()
         return loss.detach(), correct
-
-    def evaluate(self, s):
-        """Accuracy over mask == s from sampled forwards (no dropout, no update)."""
-        self.ctx.eval()
-        correct = torch.zeros((), dtype=torch.int64, device=self.device)
-        ids = self.nids[s]
-        with torch.no_grad():
-            for b in range(0, ids.numel(), self.batch_size):
-                out = self.Forward(ids[b:b + self.batch_size], False)
-                correct += (out.argmax(1) == self.L_GT.index_select(0, self.subgraph.seeds().long())).sum()
-        self.ctx.train()
-        return float(correct) / max(ids.numel(), 1)
-
-    def run_epoch(self, test=True):
-        """One pass over the train batches (one Adam step each) and, with test=True, sampled validation and test
-        forwards.  Returns (mean train loss, [train, val, test] accuracy) - val / test are None with test=False."""
-        ids = self.nids[0]
-        losses, correct = [], torch.zeros((), dtype=torch.int64, device=self.device)
-        for b in range(0, ids.numel(), self.batch_size):
-            loss, c = self.train_step(ids[b:b + self.batch_size])
-            losses.append(loss)
-            correct += c
-        mean_loss = float(torch.stack(losses).mean()) if losses else float("nan")
-        acc = [float(correct) / max(ids.numel(), 1)]
-        acc += [self.evaluate(1), self.evaluate(2)] if test else [None, None]
-        self.epoch += 1
-        return mean_loss, acc
 
 
 class GATImpl:
@@ -488,7 +576,7 @@ def _minibatch_gat_op(sampled_subgraph, active, hop, gather_dtype=None):
     return ops.MiniBatchGATOp(sampled_subgraph, hop, gather_dtype=gather_dtype)
 
 
-class GATSampleImpl:
+class GATSampleImpl(_SampledRounds):
     """Neighbour-sampled mini-batch multi-head GAT: GATImpl's layers on GCNSampleImpl's batch loop.  The train vertices
     (mask == 0), in id order, are cut into batches of `batch_size` seeds; each batch is sampled with
     NeighborSampler(..., include_dst=True), so that every hop's sources include its destinations, and runs the L layers
@@ -513,7 +601,11 @@ class GATSampleImpl:
     in the last bits between runs: fanouts of 34 to 64, hub sources of a large block (config B's deeper hops), fallback
     shapes.  On one H100, two Cora runs (1433-64-7, 8 heads, fanout 10-10, batch 64; the largest source has 17
     out-edges in a block) gave bit-identical losses and weights over three epochs with FP32 and with BF16 gathers
-    (DESIGN.md §3 K8)."""
+    (DESIGN.md §3 K8).
+
+    features: the [V, F] tensor, or a feature_table.ShardedFeatureTable for data-parallel rounds over its ranks
+    (_SampledRounds); the first layer then reads its sources' rows from the table (nts_gather_rows_sharded).
+    `partitioned_graph` is the whole graph as a single partition on every rank."""
 
     def __init__(self, partitioned_graph, layers, features, labels, mask, fanout, batch_size, heads=8,
                  learn_rate=0.01, weight_decay=0.0001, decay_rate=0.97, decay_epoch=100, seed=0, sample_seed=0,
@@ -533,7 +625,7 @@ class GATSampleImpl:
             _refuse_bf16_gat_layers(self.layers, self.heads)
         from .sample import NeighborSampler
         self.sampler = NeighborSampler(partitioned_graph, fanout, self.batch_size, include_dst=True)
-        self.device = features.device
+        self._init_features(features, self.sampler.V)
         self.sample_seed = int(sample_seed)
         self.step = 0
         self.ctx = NtsContext()
@@ -547,7 +639,6 @@ class GATSampleImpl:
                 prm.init_parameter()
                 prm.set_decay(decay_rate, decay_epoch)
                 lst.append(prm)
-        self.features = ops._check_input(features.detach(), "features")
         self.L_GT = labels.to(self.device)
         mask = torch.as_tensor(mask).cpu()
         self.nids = [(mask == s).nonzero().view(-1) for s in (0, 1, 2)]    # train / val / test ids, ascending
@@ -558,8 +649,9 @@ class GATSampleImpl:
     def params(self):
         return self.P + self.al + self.ar
 
-    def Forward(self, seeds):
-        """Sample the batch and run the layers; returns the last layer's [n_seeds, classes] log-probabilities."""
+    def Forward(self, seeds, training=True):
+        """Sample the batch and run the layers; returns the last layer's [n_seeds, classes] log-probabilities (the
+        same with training=False: there is no dropout)."""
         self.subgraph = sg = self.sampler.sample(seeds, self.sample_seed, self.step)
         self.step += 1
         ctx = self.ctx
@@ -571,7 +663,7 @@ class GATSampleImpl:
             H = self.heads[l]
             D = self.layers[l + 1] // H
             if l == 0:
-                x = self.features.index_select(0, b.src.long())
+                x = self._input_rows(b.src)
             x_trans = ctx.runVertexForward(lambda t, _l=l: self.P[_l].forward(t), x)
             # the destination score reads the destinations' own rows; it is recorded before the source score, whose
             # input x_trans would otherwise chain onto x_trans's own tape entry (NtsContext.appendNNOp) and leave
@@ -594,14 +686,6 @@ class GATSampleImpl:
         self.ctx.appendNNOp(out, self.loss)
         return self.loss
 
-    def Update(self):
-        for p in self.params():
-            if p.W.grad is None:
-                continue
-            p.all_reduce_to_gradient(p.W.grad)
-            p.learn_with_decay_Adam()
-            p.next()
-
     def train_step(self, seeds):
         """One batch: zero the gradients, sample, forward, loss, tape backward, Adam.  Returns (loss, correct)."""
         for p in self.params():
@@ -615,30 +699,3 @@ class GATSampleImpl:
         self.ctx.self_backward(True)
         self.Update()
         return loss.detach(), correct
-
-    def evaluate(self, s):
-        """Accuracy over mask == s from sampled forwards (no update)."""
-        self.ctx.eval()
-        correct = torch.zeros((), dtype=torch.int64, device=self.device)
-        ids = self.nids[s]
-        with torch.no_grad():
-            for b in range(0, ids.numel(), self.batch_size):
-                out = self.Forward(ids[b:b + self.batch_size])
-                correct += (out.argmax(1) == self.L_GT.index_select(0, self.subgraph.seeds().long())).sum()
-        self.ctx.train()
-        return float(correct) / max(ids.numel(), 1)
-
-    def run_epoch(self, test=True):
-        """One pass over the train batches (one Adam step each) and, with test=True, sampled validation and test
-        forwards.  Returns (mean train loss, [train, val, test] accuracy) - val / test are None with test=False."""
-        ids = self.nids[0]
-        losses, correct = [], torch.zeros((), dtype=torch.int64, device=self.device)
-        for b in range(0, ids.numel(), self.batch_size):
-            loss, c = self.train_step(ids[b:b + self.batch_size])
-            losses.append(loss)
-            correct += c
-        mean_loss = float(torch.stack(losses).mean()) if losses else float("nan")
-        acc = [float(correct) / max(ids.numel(), 1)]
-        acc += [self.evaluate(1), self.evaluate(2)] if test else [None, None]
-        self.epoch += 1
-        return mean_loss, acc
