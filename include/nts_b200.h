@@ -478,6 +478,17 @@ int nts_exchange_backward_bf16(nts_exchange *ex, const float *g, float *dx, nts_
  * nts_exchange_last_timeline synchronises the device */
 int nts_exchange_set_trace(nts_exchange *ex, int enable);
 int nts_exchange_last_timeline(nts_exchange *ex, float *ms, int capacity);
+/* What the last call on this engine did (host bookkeeping, known once the call returns; null outputs are skipped):
+ * kind 1 forward, 2 backward, 3 mirror fetch, 4 mirror return (0: no call yet); its epoch and window buffer
+ * (epoch % n_buffers); mode 1 = pipeline, 2 = merged receive (0 for fetch / return); kernel_peers / dma_peers = bit j
+ * set when peer j was served by the push kernel / by a copy-engine push (a peer that reads none of my rows still gets
+ * its flag from one of them); push_vec = floats per lane access of the push kernel (0: no kernel push); plan_chunks =
+ * bit i set when chunk i was aggregated through an nts_gather_plan (its own or the merged one) rather than K1;
+ * bf16_staging = 0 for FP32 gathers, 1 when this rank's operand was converted into BF16 staging rows, 2 when BF16
+ * input rows were used as they are.  A single-partition engine reports only the kind. */
+int nts_exchange_last_paths(const nts_exchange *ex, int *kind, int *epoch, int *buffer, int *mode,
+                            uint32_t *kernel_peers, uint32_t *dma_peers, int *push_vec, uint32_t *plan_chunks,
+                            int *bf16_staging);
 /* DistGPUGetDepNbrOp (core/ntsDistGPUGraphOp.hpp:48-143) on the same windows - the reference moves the whole feature
  * matrix GPU -> host -> MPI -> host -> GPU.  forward: mirror[MirrorIndex[s], :] = X[s, :] for every source s of a local
  * in-edge ([owned_mirrors, F], partition order); backward: dx[v, :] += every partition's mirror gradient of my vertex

@@ -163,6 +163,8 @@ SIGNATURES.update({
     "nts_exchange_required_floats_bf16": (_u64, [_vp, _u32]),
     "nts_exchange_set_trace": (_int, [_vp, _int]),
     "nts_exchange_last_timeline": (_int, [_vp, C.POINTER(C.c_float), _int]),
+    "nts_exchange_last_paths": (_int, [_vp] + [C.POINTER(_int)] * 4 + [C.POINTER(_u32)] * 2 +
+                                [C.POINTER(_int), C.POINTER(_u32), C.POINTER(_int)]),
     "nts_exchange_fetch_mirrors": (_int, [_vp, _vp, _vp, _u32, _vp]),
     "nts_exchange_return_mirror_grads": (_int, [_vp, _vp, _vp, _u32, _vp]),
 })

@@ -97,6 +97,11 @@ struct nts_exchange {
   bool trace = false;
   std::vector<cudaEvent_t> tev; // [0] call start, [1] push begin, [2] push end, [3] local chunk done,
                                 // then per ring step s: [4+2(s-1)] rows of (p+s) have landed, [5+2(s-1)] chunk aggregated
+  // which paths the last call took (nts_exchange_last_paths): host bookkeeping, filled while the call is enqueued
+  struct Paths {
+    int kind = 0, epoch = 0, buffer = 0, mode = 0, vec = 0, staging = 0;
+    uint32_t kernel_peers = 0, dma_peers = 0, plan_chunks = 0;
+  } last;
 };
 
 namespace nts {
@@ -284,6 +289,7 @@ static int launch_push(nts_exchange *ex, const PushArgs &a, const float *src, ui
   else if (F % 2 == 0 && a8)
     vec = 2;
   const int ctas = ex->push_ctas;
+  ex->last.vec = vec;
   if (vec == 4)
     push_rows_kernel<4><<<ctas, 256, 0, st>>>(a, src, F, ex->tickets, ex->timeout_ns, ex->err_dev);
   else if (vec == 2)
@@ -303,6 +309,7 @@ static int dma_push(nts_exchange *ex, int j, const float *src, size_t dst_row, u
   NTS_CUDA_OK(cudaEventRecord(ex->ev_dma[j], from));
   NTS_CUDA_OK(cudaStreamWaitEvent(st, ex->ev_dma[j], 0));
   ex->dma_used[j] = 1;
+  ex->last.dma_peers |= 1u << j;
   if (n_rows) {
     if (wait_epoch) {
       wait_consumed_kernel<<<1, 1, 0, st>>>(ex->flags + ex->P + j, wait_epoch, ex->timeout_ns, ex->err_dev, j);
@@ -345,6 +352,7 @@ static int push_my_rows(nts_exchange *ex, const float *x, uint32_t F, size_t buf
       NTS_TRY(dma_push(ex, j, x, ex->fwd_push_off[j], ex->send_count[j], F, buf, epoch, wait_epoch, ex->comm));
       continue;
     }
+    ex->last.kernel_peers |= 1u << j;
     PushTarget &t = a.t[a.n++];
     t.rows = ex->d.send_rows_all + ex->srecv_offs[j];
     t.n_rows = ex->send_count[j];
@@ -404,6 +412,7 @@ static int aggregate_chunk(nts_exchange *ex, int i, bool forward, const void *in
         }
       plans.emplace_back(plan_key(F, gt.bf16), pl);
     }
+    ex->last.plan_chunks |= 1u << i;
     if (gt.bf16)
       return run_plan_bf16(pl, in_rows, NTS_DTYPE_BF16, gt.ld, out, F, st);
     return run_plan(pl, in, F, out, F, 0, st);
@@ -720,6 +729,9 @@ int nts_exchange_reserve(nts_exchange *ex, uint64_t floats_per_buffer, int n_buf
     NTS_CUDA_OK(cudaFree(ex->window));
   ex->window = nullptr;
   ex->buf_floats = 0;
+  // every epoch buffer starts 256-byte aligned, like the first: the push kernel's vector width must not depend on
+  // the epoch's parity
+  floats_per_buffer = (floats_per_buffer + 63) & ~63ull;
   NTS_CUDA_OK(cudaMalloc(reinterpret_cast<void **>(&ex->window), floats_per_buffer * n_buffers * sizeof(float)));
   ex->buf_floats = floats_per_buffer;
   ex->n_buffers = n_buffers;
@@ -777,13 +789,26 @@ static int stage_bf16(nts_exchange *ex, const void *src, int dtype, uint32_t F, 
                       const void **rows) {
   const uint32_t n = ex->d.owned_vertices;
   if (dtype == NTS_DTYPE_BF16 && gt.ld == F && aligned_to(src, 16)) {
+    ex->last.staging = 2;
     *rows = src;
     return 0;
   }
+  ex->last.staging = 1;
   NTS_TRY(grow(&ex->stage16, &ex->stage16_cap, (size_t)(n ? n : 1) * (gt.ld / 2)));
   NTS_TRY(to_bf16_rows(src, dtype, F, ex->stage16, n, F, gt.ld, st));
   *rows = ex->stage16;
   return 0;
+}
+
+// The receive mode of a forward / backward call.  decide_mode's timing runs aggregate chunks too, so the plan record
+// starts here; a merged launch gathers every remote chunk that has edges through the merged plan.
+static void record_mode(nts_exchange *ex, const nts_exchange::Mode &m) {
+  ex->last.mode = m.mode;
+  ex->last.plan_chunks = 0;
+  if (m.mode == 2)
+    for (int i = 0; i < ex->P; i++)
+      if (i != ex->p && ex->chunks[i].edges && ex->need_count[i])
+        ex->last.plan_chunks |= 1u << i;
 }
 
 static int forward_impl(nts_exchange *ex, const void *x_in, int x_dtype, float *y, nts_vid_t F, void *stream,
@@ -795,6 +820,8 @@ static int forward_impl(nts_exchange *ex, const void *x_in, int x_dtype, float *
   NTS_ARG_CHECK(d.owned_vertices == 0 || (x && y), "null feature pointer");
   cudaStream_t st = as_stream(stream);
   const int P = ex->P, p = ex->p;
+  ex->last = {};
+  ex->last.kind = 1;
   NTS_ARG_CHECK(!bf16 || P > 1, "BF16 gathers on one partition run through nts_gather_plan_run_bf16_ex");
   if (P == 1)
     return nts_gather_by_dst_from_src(x, y, d.local_weight_forward, d.local_row_indices, d.local_column_offset,
@@ -812,6 +839,7 @@ static int forward_impl(nts_exchange *ex, const void *x_in, int x_dtype, float *
   const uint32_t epoch = ++ex->epoch;
   const size_t buf = (size_t)(epoch % ex->n_buffers) * ex->buf_floats;
   const uint32_t wait_epoch = epoch > (uint32_t)ex->n_buffers ? epoch - ex->n_buffers : 0u;
+  ex->last.epoch = (int)epoch, ex->last.buffer = (int)(epoch % ex->n_buffers);
   const bool tr = ex->trace && (int)ex->tev.size() >= 4 + 2 * (P - 1);
   NTS_CUDA_OK(cudaEventRecord(ex->ev_main, st)); // x is ready
   if (tr)
@@ -828,6 +856,7 @@ static int forward_impl(nts_exchange *ex, const void *x_in, int x_dtype, float *
   // one launch over all of them once everything has landed (merged); measured once per width, see decide_mode
   nts_exchange::Mode *mode = nullptr;
   NTS_TRY(decide_mode(ex, true, F, st, &mode, gt));
+  record_mode(ex, *mode);
   NTS_TRY(aggregate_chunk(ex, p, true, x, y, F, st, gt));
   if (tr)
     NTS_CUDA_OK(cudaEventRecord(ex->tev[3], st));
@@ -876,6 +905,8 @@ static int backward_impl(nts_exchange *ex, const float *g, float *dx, nts_vid_t 
   NTS_ARG_CHECK(d.owned_vertices == 0 || (g && dx), "null gradient pointer");
   cudaStream_t st = as_stream(stream);
   const int P = ex->P, p = ex->p;
+  ex->last = {};
+  ex->last.kind = 2;
   NTS_ARG_CHECK(!bf16 || P > 1, "BF16 gathers on one partition run through nts_gather_plan_run_bf16_ex");
   if (P == 1)
     return nts_gather_by_src_from_dst(g, dx, d.local_weight_backward, d.local_row_offset, d.local_column_indices,
@@ -890,11 +921,13 @@ static int backward_impl(nts_exchange *ex, const float *g, float *dx, nts_vid_t 
   const uint32_t epoch = ++ex->epoch;
   const size_t buf = (size_t)(epoch % ex->n_buffers) * ex->buf_floats;
   const uint32_t wait_epoch = epoch > (uint32_t)ex->n_buffers ? epoch - ex->n_buffers : 0u;
+  ex->last.epoch = (int)epoch, ex->last.buffer = (int)(epoch % ex->n_buffers);
   NTS_TRY(grow(&ex->bsend, &ex->bsend_cap, (size_t)(ex->recv_total ? ex->recv_total : 1) * F));
   if (ex->recv_total)
     NTS_CUDA_OK(cudaMemsetAsync(ex->bsend, 0, (size_t)ex->recv_total * F * sizeof(float), st));
   nts_exchange::Mode *mode = nullptr;
   NTS_TRY(decide_mode(ex, false, F, st, &mode, gt));
+  record_mode(ex, *mode);
   if (mode->mode == 2) {
     // ---- merged: ONE launch computes the partial gradients of the active sources of all remote chunks, then every
     // slice goes to its owner through the copy engines
@@ -950,6 +983,8 @@ static int fetch_impl(nts_exchange *ex, const float *x, float *mirror, nts_vid_t
   cudaStream_t st = as_stream(stream);
   const int P = ex->P, p = ex->p;
   const uint32_t own = d.local_need_count;
+  ex->last = {};
+  ex->last.kind = 3;
   NTS_ARG_CHECK(own == 0 || d.local_need, "exchange descriptor lacks local_need (rows of this partition it reads itself)");
   if (P == 1)
     return own ? nts_gather_rows(mirror, x, d.local_need, own, F, stream) : 0;
@@ -957,6 +992,7 @@ static int fetch_impl(nts_exchange *ex, const float *x, float *mirror, nts_vid_t
   const uint32_t epoch = ++ex->epoch;
   const size_t buf = (size_t)(epoch % ex->n_buffers) * ex->buf_floats;
   const uint32_t wait_epoch = epoch > (uint32_t)ex->n_buffers ? epoch - ex->n_buffers : 0u;
+  ex->last.epoch = (int)epoch, ex->last.buffer = (int)(epoch % ex->n_buffers);
   NTS_CUDA_OK(cudaEventRecord(ex->ev_main, st));
   NTS_CUDA_OK(cudaStreamWaitEvent(ex->comm, ex->ev_main, 0));
   NTS_TRY(push_my_rows(ex, x, F, buf, epoch, wait_epoch));
@@ -989,6 +1025,8 @@ static int return_impl(nts_exchange *ex, const float *gm, float *dx, nts_vid_t F
   cudaStream_t st = as_stream(stream);
   const int P = ex->P, p = ex->p;
   const uint32_t own = d.local_need_count;
+  ex->last = {};
+  ex->last.kind = 4;
   NTS_ARG_CHECK(own == 0 || d.local_need, "exchange descriptor lacks local_need");
   if (P == 1)
     return own ? nts_scatter_add_rows(dx, gm, d.local_need, own, F, stream) : 0;
@@ -997,6 +1035,7 @@ static int return_impl(nts_exchange *ex, const float *gm, float *dx, nts_vid_t F
   const size_t buf = (size_t)(epoch % ex->n_buffers) * ex->buf_floats;
   const size_t before = ex->recv_offs[p];
   const uint32_t wait_epoch = epoch > (uint32_t)ex->n_buffers ? epoch - ex->n_buffers : 0u;
+  ex->last.epoch = (int)epoch, ex->last.buffer = (int)(epoch % ex->n_buffers);
   NTS_CUDA_OK(cudaEventRecord(ex->ev_main, st));
   NTS_CUDA_OK(cudaStreamWaitEvent(ex->comm, ex->ev_main, 0));
   for (int s = 1; s < P; s++) {
@@ -1051,6 +1090,32 @@ int nts_exchange_last_timeline(nts_exchange *ex, float *ms, int capacity) {
     prev = ex->tev[5 + 2 * (s - 1)];
   }
   NTS_CUDA_OK(cudaEventElapsedTime(&ms[2 * P], ex->tev[0], prev));
+  return 0;
+}
+
+int nts_exchange_last_paths(const nts_exchange *ex, int *kind, int *epoch, int *buffer, int *mode,
+                            uint32_t *kernel_peers, uint32_t *dma_peers, int *push_vec, uint32_t *plan_chunks,
+                            int *bf16_staging) {
+  NTS_ARG_CHECK(ex != nullptr, "null engine");
+  const nts_exchange::Paths &r = ex->last;
+  if (kind)
+    *kind = r.kind;
+  if (epoch)
+    *epoch = r.epoch;
+  if (buffer)
+    *buffer = r.buffer;
+  if (mode)
+    *mode = r.mode;
+  if (kernel_peers)
+    *kernel_peers = r.kernel_peers;
+  if (dma_peers)
+    *dma_peers = r.dma_peers;
+  if (push_vec)
+    *push_vec = r.vec;
+  if (plan_chunks)
+    *plan_chunks = r.plan_chunks;
+  if (bf16_staging)
+    *bf16_staging = r.staging;
   return 0;
 }
 

@@ -56,6 +56,12 @@ def test_aggregate_launch_record_takes_null_outputs():
     assert all(v.value >= 0 for v in vals)
 
 
+def test_exchange_path_record_refuses_a_null_engine():
+    lib = _lib.load()
+    assert lib.nts_exchange_last_paths(None, *([None] * 9)) != 0
+    assert b"null engine" in lib.nts_last_error()
+
+
 def test_empty_chunks_are_a_no_op_before_any_pointer_is_looked_at():
     """A rank that owns no vertices (or a chunk without edges) hands the aggregation entries empty tensors, whose data
     pointers are NULL: the entries must return success without touching CUDA or complaining about the pointers."""
