@@ -103,6 +103,16 @@ int nts_segment_gather_sum_range(const float *input, float *output, const float 
                                  nts_vid_t n_rows, uint64_t edge_begin, uint64_t edge_end, nts_vid_t feature_size,
                                  void *stream);
 
+/* K1 on BF16 rows with FP32 accumulation: output[r, 0:F] += sum_e weight[e] * float(input[indices[e], 0:F]) (weight
+ * NULL: 1), F = feature_size.  `input` holds BF16 rows of stride input_ld values (input_ld % 8 == 0, >= F, 16-byte
+ * aligned; columns F..input_ld-1 are never added); `output` is FP32 [n_rows, F] contiguous.  Accumulates like
+ * nts_segment_gather_sum (rows cut by edge quanta finish with atomics); row addresses are 64-bit.  The layout
+ * conditions are checked first; n_rows == 0 or n_edges == 0 then launches nothing.  FP32 operands are rounded with
+ * nts_rows_to_bf16. */
+int nts_segment_gather_sum_bf16(const void *input, nts_vid_t input_ld, float *output, const float *weight,
+                                const nts_vid_t *indices, const nts_vid_t *offsets, nts_vid_t n_rows, uint64_t n_edges,
+                                nts_vid_t feature_size, void *stream);
+
 /* ---- preprocessed aggregation: nts_gather_plan --------------------------------------------------------------------
  * The arrays of one chunk direction (CSC: column_offset / row_indices / edge_weight_forward; CSR: row_offset /
  * column_indices / edge_weight_backward; core/GraphSegment.h:52-139) regrouped ONCE on the device for repeated
@@ -214,8 +224,9 @@ int nts_segment_gather_sum_heads(const float *input, float *output, const float 
  * re-association): variant 0 = auto, see DESIGN.md "kernel variants". */
 int nts_aggregate_set_variant(int variant, int edges_per_warp);
 int nts_aggregate_last_launch(int *grid, int *block, int *smem_bytes, int *variant);
-/* Template point of the last launch: floats (BF16 values for the BF16 fused GAT forward) per vector load, vector chunks
- * per lane, edges loaded before their FMAs (U), __launch_bounds__ minimum CTAs per SM, and column tiles. */
+/* Template point of the last launch: floats (BF16 values for the BF16 fused GAT forward and
+ * nts_segment_gather_sum_bf16) per vector load, vector chunks per lane, edges loaded before their FMAs (U),
+ * __launch_bounds__ minimum CTAs per SM, and column tiles.  Virtual warps show in nts_aggregate_last_launch's grid. */
 int nts_aggregate_last_shape(int *vec, int *k, int *u, int *min_blocks, int *tiles);
 uint64_t nts_kernel_launch_count(void); /* kernels launched by this library since load */
 
@@ -375,6 +386,15 @@ int nts_gather_rows(float *dst, const float *src, const nts_vid_t *rows, nts_vid
 int nts_gather_rows_sharded(float *dst, const float *const *shards, const nts_vid_t *shard_offsets, int n_shards,
                             nts_vid_t shard_pitch, const nts_vid_t *ids, nts_vid_t n, nts_vid_t feature_size,
                             void *stream);
+/* The same gather from BF16 shards: shard rows of shard_pitch BF16 values (shard_pitch % 8 == 0, >= feature_size; every
+ * shard 16-byte aligned), read 16 bytes at a time.  dst_dtype NTS_DTYPE_BF16: dst holds BF16 rows of stride dst_ld
+ * (dst_ld % 8 == 0, >= feature_size, dst 16-byte aligned) and gets a plain copy of columns [0, 8*ceil(F/8)) (the
+ * columns past feature_size get the shard's pad values, later columns are not written).  NTS_DTYPE_F32: dst is FP32
+ * [n, feature_size] contiguous (dst_ld == feature_size) and gets the rows widened exactly.  Ids as above; n == 0
+ * launches nothing. */
+int nts_gather_rows_sharded_bf16(void *dst, int dst_dtype, nts_vid_t dst_ld, const void *const *shards,
+                                 const nts_vid_t *shard_offsets, int n_shards, nts_vid_t shard_pitch,
+                                 const nts_vid_t *ids, nts_vid_t n, nts_vid_t feature_size, void *stream);
 /* dst[rows[k],:] += src[k,:]  (receiver-side add of partial gradients; rows must be unique) */
 int nts_scatter_add_rows(float *dst, const float *src, const nts_vid_t *rows, nts_vid_t n_rows,
                          nts_vid_t feature_size, void *stream);

@@ -97,6 +97,43 @@ __device__ __forceinline__ void red_add(float8v *p, float8v a) {
   red_add(&p->hi, a.hi);
 }
 
+// o[col .. col+7] (+)= a for the columns < Fo of a row of Fo floats (K1 on BF16 rows: the output's width need not be a
+// multiple of the 8-value chunk).  Whole chunks go as 16- or 8-byte vectors when Fo and the row allow them.
+__device__ __forceinline__ void flush_cols(float *o, uint32_t col, uint32_t Fo, const float8v &a, bool whole) {
+  const float v[8] = {a.lo.x, a.lo.y, a.lo.z, a.lo.w, a.hi.x, a.hi.y, a.hi.z, a.hi.w};
+  const uintptr_t align = reinterpret_cast<uintptr_t>(o);
+  if ((Fo & 3u) == 0 && (align & 15u) == 0) { // col and Fo multiples of 4: whole float4s
+#pragma unroll
+    for (int i = 0; i < 8; i += 4)
+      if (col + i < Fo) {
+        const float4 x = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
+        if (whole)
+          rmw_add(reinterpret_cast<float4 *>(o + col + i), x);
+        else
+          red_add(reinterpret_cast<float4 *>(o + col + i), x);
+      }
+  } else if ((Fo & 1u) == 0 && (align & 7u) == 0) {
+#pragma unroll
+    for (int i = 0; i < 8; i += 2)
+      if (col + i < Fo) {
+        const float2 x = make_float2(v[i], v[i + 1]);
+        if (whole)
+          rmw_add(reinterpret_cast<float2 *>(o + col + i), x);
+        else
+          red_add(reinterpret_cast<float2 *>(o + col + i), x);
+      }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; i++)
+      if (col + i < Fo) {
+        if (whole)
+          rmw_add(o + col + i, v[i]);
+        else
+          red_add(o + col + i, v[i]);
+      }
+  }
+}
+
 // largest r in [0, n_rows) with off[r] <= e  (requires off[0] <= e < off[n_rows])
 __device__ __forceinline__ uint32_t find_row(const uint32_t *__restrict__ off, uint32_t n_rows, uint32_t e) {
   uint32_t lo = 0, hi = n_rows; // invariant: off[lo] <= e < off[hi]
@@ -169,9 +206,11 @@ __device__ __forceinline__ float att_weight(float s, float d, float m, float inv
 // G    : virtual warps per warp (BULK only): rows of at most 16 vectors leave half of the lanes idle, so the warp is
 //        split into G independent groups of 32/G lanes, each with its own edge quantum and row state (the BULK
 //        variant has no warp-wide shuffles; all bookkeeping is per lane).  Used by the fused GAT layers (F = 64).
-// T    : gathered element type.  float, or __nv_bfloat16 for the fused GAT layer (HM == 2) with VEC = 8: one 16-byte
-//        load carries 8 BF16 values that are widened to FP32 in registers; F is then the BF16 row stride ld (a multiple
-//        of 8), which the FP32 output shares.
+// T    : gathered element type.  float, or __nv_bfloat16 with VEC = 8: one 16-byte load carries 8 BF16 values that are
+//        widened to FP32 in registers, and F is the BF16 row stride ld (a multiple of 8).  In the fused GAT layer
+//        (HM == 2) the FP32 output shares that stride.  In head mode 0 (K1 on BF16 rows, kNarrowOut) the output is
+//        [n_rows, Fo] contiguous with Fo <= ld carried in `heads` (unused by HM 0 otherwise): a lane's chunks cover
+//        ceil(Fo / 8) chunks of the row and its flush writes only columns < Fo.
 template <int VEC, int K, int U, bool BULK, int MINB = 1, int HM = 0, int G = 1, class T = float>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, MINB)
     segment_gather_sum_kernel(const T *__restrict__ in, float *__restrict__ out, const float *__restrict__ w,
@@ -181,7 +220,8 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MINB)
                               uint32_t tile_major, uint32_t heads, AttParams att, uint32_t e_begin, uint32_t out_mod) {
   static_assert(!(HM == 1 && BULK), "[E, H] weight matrices are not bulk-staged (indices of HM 0 / 2 are)");
   static_assert(G == 1 || (BULK && K == 1), "virtual warps need the shuffle-free variant and one chunk per lane");
-  static_assert(std::is_same<T, float>::value || (HM == 2 && VEC == 8), "BF16 rows: fused GAT layer, 8 per chunk");
+  static_assert(std::is_same<T, float>::value || (HM != 1 && VEC == 8), "BF16 rows: head mode 0 or 2, 8 per chunk");
+  constexpr bool kNarrowOut = !std::is_same<T, float>::value && HM == 0;
   using V = typename Vec<VEC>::type;
   using L = typename Ld<T, VEC>::type; // what a lane loads per chunk (FP32: V itself)
   constexpr uint32_t GS = 32 / G;
@@ -189,7 +229,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MINB)
   const uint32_t n_edges = (uint32_t)n_edges64;
   const uint32_t lane = threadIdx.x & (GS - 1);
   const uint32_t warp_in_block = threadIdx.x / GS;
-  const uint32_t nvec = F / VEC;
+  const uint32_t nvec = kNarrowOut ? (heads + VEC - 1) / VEC : F / VEC;
 
   // quantum / column tile owned by this warp.
   //   interleaved (tile_major = 0): consecutive warps = the column tiles of one quantum (they share index loads)
@@ -295,16 +335,25 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MINB)
   auto flush = [&](bool whole) {
     const uint32_t orow = out_mod ? row % out_mod : row;
     whole = whole && !out_mod;
-    V *o = reinterpret_cast<V *>(out + (size_t)orow * F) + c0;
+    if constexpr (kNarrowOut) {
 #pragma unroll
-    for (int k = 0; k < K; k++) {
-      if (act[k]) {
-        if (whole)
-          rmw_add(o + k * GS, acc[k]);
-        else
-          red_add(o + k * GS, acc[k]);
+      for (int k = 0; k < K; k++) {
+        if (act[k])
+          flush_cols(out + (size_t)orow * heads, (c0 + k * GS) * 8u, heads, acc[k], whole);
+        zero_vec(acc[k]);
       }
-      zero_vec(acc[k]);
+    } else {
+      V *o = reinterpret_cast<V *>(out + (size_t)orow * F) + c0;
+#pragma unroll
+      for (int k = 0; k < K; k++) {
+        if (act[k]) {
+          if (whole)
+            rmw_add(o + k * GS, acc[k]);
+          else
+            red_add(o + k * GS, acc[k]);
+        }
+        zero_vec(acc[k]);
+      }
     }
   };
   // move to the row containing edge ee (ee >= row_end on entry)
@@ -732,6 +781,113 @@ static int gat_forward_bf16(const __nv_bfloat16 *in, float *out, const uint32_t 
   return fail(-1, "no BF16 fused-GAT instantiation for this (chunks, U, virtual warps) point", __FILE__, __LINE__);
 }
 
+// ---- K1 on BF16 rows (head mode 0) -----------------------------------------------------------------------------------
+// out[r, :F] += sum_e w_e * float(in[idx[e], :F]) with BF16 rows of stride ld (ld % 8 == 0, ld >= F, 16-byte aligned)
+// and a contiguous FP32 output [n_rows, F].  Same edge quanta, staging variants and atomics as the FP32 K1.
+template <int K, int U, int MINB, int G>
+static int launch_k1_bf16(bool bulk, const LaunchShape &sh, const __nv_bfloat16 *in, float *out, const float *w,
+                          const uint32_t *idx, const uint32_t *off, uint32_t n_rows, uint64_t n_edges, uint32_t ld,
+                          uint32_t F, uint32_t Q, cudaStream_t st) {
+  constexpr uint32_t kVW = kWarpsPerBlock * G;
+  const uint64_t warps = (n_edges + Q - 1) / Q * sh.tiles;
+  const uint64_t blocks = (warps + kVW - 1) / kVW;
+  NTS_ARG_CHECK(blocks <= 0x7fffffffull, "aggregation grid too large");
+  g_last_grid = (int)blocks;
+  g_last_block = kWarpsPerBlock * 32;
+  g_last_variant = bulk ? 2 : 1;
+  g_last_vec = 8, g_last_k = K, g_last_u = U, g_last_minb = MINB, g_last_tiles = (int)sh.tiles;
+  if (bulk) {
+    const size_t smem = 16 + 2 * ((size_t)kVW * Q + 8) * 4;
+    auto kern = segment_gather_sum_kernel<8, K, U, true, MINB, 0, G, __nv_bfloat16>;
+    NTS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    g_last_smem = (int)smem;
+    kern<<<(unsigned)blocks, kWarpsPerBlock * 32, smem, st>>>(in, out, w, idx, off, nullptr, 0, n_rows, n_edges, ld, Q,
+                                                              sh.tiles, sh.tile_vecs, 0, F, kNoAtt, 0, 0);
+  } else {
+    if constexpr (G == 1) {
+      g_last_smem = 0;
+      segment_gather_sum_kernel<8, K, U, false, MINB, 0, 1, __nv_bfloat16><<<(unsigned)blocks, kWarpsPerBlock * 32, 0,
+                                                                              st>>>(
+          in, out, w, idx, off, nullptr, 0, n_rows, n_edges, ld, Q, sh.tiles, sh.tile_vecs, 0, F, kNoAtt, 0, 0);
+    } else {
+      return fail(-1, "virtual warps need the bulk-staged variant", __FILE__, __LINE__);
+    }
+  }
+  NTS_LAUNCH_CHECK();
+  return 0;
+}
+
+// Chunks of 8 values, K <= 4 per lane per column tile; rows of at most 16 chunks (F <= 128: F = 41 and 37 are 6 and 5
+// chunks, F = 128 is 16) split the warp into G = 2 virtual warps under the bulk-staged variant, F = 602 (76 chunks) is
+// K = 3.  (U, MINB, G) measured on sampled config B blocks (H100 SXM, 700 W, tools/sample_dtype_sweep.py): at F = 41
+// G = 4 / 2 / 1 took 43.4 / 36.2 / 30.7 us at (U 4, MINB 4) and G = 2 took 30.7 us at MINB 2 (a block's few edges
+// already shrink the quantum to 32, so G divides the grid); F = 602 U = 4 / 2: 73.5 / 75.4 us.  NTS_K1_BF16_TUNE="U,MINB,G"
+// is a measurement hook, whose G applies only to a one-chunk row under the bulk variant that it fits.
+static int segment_gather_sum_bf16(const __nv_bfloat16 *in, uint32_t ld, float *out, const float *w,
+                                   const uint32_t *idx, const uint32_t *off, uint32_t n_rows, uint64_t n_edges,
+                                   uint32_t F, cudaStream_t st) {
+  LaunchShape s;
+  s.vec = 8;
+  s.heads = 1;
+  s.tile_major = 0;
+  const uint32_t nvec = (F + 7) / 8;
+  const uint32_t chunks = (nvec + 31) / 32;
+  s.tiles = (chunks + 3) / 4;
+  s.tile_vecs = (nvec + s.tiles - 1) / s.tiles;
+  s.k = (int)((s.tile_vecs + 31) / 32);
+  s.tiles = (nvec + s.tile_vecs - 1) / s.tile_vecs;
+  int variant = g_variant == 0 ? 2 : g_variant;
+  // the bulk copies need 16-byte aligned index/weight arrays (cudaMalloc gives 256)
+  if (variant == 2 && !(aligned_to(idx, 16) && (!w || aligned_to(w, 16))))
+    variant = 1;
+  const bool bulk = variant == 2;
+  const bool narrow = bulk && s.k == 1 && s.tiles == 1;
+  s.g = narrow && nvec <= 16 ? 2 : 1;
+  s.u = s.k <= 3 ? 4 : 2;
+  s.minb = s.k == 4 ? 1 : 2;
+  if (const char *tune = getenv("NTS_K1_BF16_TUNE")) {
+    int tu = 0, tb = 0, tg = 0;
+    if (sscanf(tune, "%d,%d,%d", &tu, &tb, &tg) == 3) {
+      s.u = tu;
+      s.minb = tb;
+      if (narrow && tg >= 1 && (uint32_t)(32 / tg) >= nvec)
+        s.g = tg;
+    }
+  }
+  uint32_t Q = g_edges_per_warp > 0 ? (uint32_t)g_edges_per_warp : 512u / (uint32_t)s.g;
+  if (g_edges_per_warp <= 0) {
+    const uint64_t want_warps = (uint64_t)sm_count() * 64;
+    while (Q > 32 && ((n_edges + Q - 1) / Q) * s.tiles < want_warps)
+      Q >>= 1;
+  }
+  Q = (Q + 31u) & ~31u;
+  if (s.g > 1 && Q * s.g > 1024) // the CTA's staged index span must keep fitting shared memory
+    Q = (1024u / s.g) & ~31u;
+#define NTS_BF16_CASE(K_, U_, B_, G_)                                                                              \
+  if (s.k == K_ && s.u == U_ && s.minb == B_ && s.g == G_)                                                         \
+    return launch_k1_bf16<K_, U_, B_, G_>(bulk, s, in, out, w, idx, off, n_rows, n_edges, ld, F, Q, st);
+  // default points
+  NTS_BF16_CASE(1, 4, 2, 2)
+  NTS_BF16_CASE(1, 4, 2, 1)
+  NTS_BF16_CASE(2, 4, 2, 1)
+  NTS_BF16_CASE(3, 4, 2, 1)
+  NTS_BF16_CASE(4, 2, 1, 1)
+  // extra points reachable through NTS_K1_BF16_TUNE
+  NTS_BF16_CASE(1, 4, 4, 4)
+  NTS_BF16_CASE(1, 4, 4, 2)
+  NTS_BF16_CASE(1, 4, 4, 1)
+  NTS_BF16_CASE(1, 2, 4, 4)
+  NTS_BF16_CASE(1, 8, 2, 4)
+  NTS_BF16_CASE(1, 4, 2, 4)
+  NTS_BF16_CASE(1, 2, 4, 2)
+  NTS_BF16_CASE(1, 8, 2, 2)
+  NTS_BF16_CASE(3, 2, 2, 1)
+  NTS_BF16_CASE(3, 2, 1, 1)
+  NTS_BF16_CASE(3, 4, 1, 1)
+#undef NTS_BF16_CASE
+  return fail(-1, "no BF16 K1 instantiation for this (chunks, U, occupancy, virtual warps) point", __FILE__, __LINE__);
+}
+
 } // namespace nts
 
 extern "C" {
@@ -799,6 +955,20 @@ int nts_gat_fused_aggregate_forward_bf16(const void *mirror, float *output, cons
   nts::AttParams att = {src_score, dst_score, seg_max, seg_sum, negative_slope};
   return nts::gat_forward_bf16(static_cast<const __nv_bfloat16 *>(mirror), output, row_indices, column_offset,
                                mirror_index, batch_size, n_edges, ld, heads, att, nts::as_stream(stream));
+}
+
+int nts_segment_gather_sum_bf16(const void *input, nts_vid_t input_ld, float *output, const float *weight,
+                                const nts_vid_t *indices, const nts_vid_t *offsets, nts_vid_t n_rows, uint64_t n_edges,
+                                nts_vid_t feature_size, void *stream) {
+  NTS_ARG_CHECK(input_ld % 8 == 0 && input_ld >= feature_size,
+                "BF16 rows need a stride input_ld >= feature_size with input_ld % 8 == 0");
+  if (n_rows == 0 || n_edges == 0 || feature_size == 0)
+    return 0;
+  NTS_ARG_CHECK(input && output && indices && offsets, "null pointer passed to nts_segment_gather_sum_bf16");
+  NTS_ARG_CHECK(nts::aligned_to(input, 16), "nts_segment_gather_sum_bf16 needs a 16-byte aligned input");
+  NTS_ARG_CHECK(n_edges < 0xffffffffull, "chunk edge count must fit uint32 offsets");
+  return nts::segment_gather_sum_bf16(static_cast<const __nv_bfloat16 *>(input), input_ld, output, weight, indices,
+                                      offsets, n_rows, n_edges, feature_size, nts::as_stream(stream));
 }
 
 int nts_gather_by_dst_from_src(const float *input, float *output, const float *weight_forward,

@@ -199,6 +199,81 @@ static void launch_gather_rows_sharded(int svec, unsigned grid, cudaStream_t st,
     gather_rows_sharded_kernel<LANES, 1><<<grid, kThreads, 0, st>>>(dst, shards, offsets, n_shards, pitch, ids, n, F);
 }
 
+// The BF16 twin: shard rows of `pitch` BF16 values (pitch % 8 == 0), one 16-byte load per 8 values.  SVEC == 0 copies
+// them into BF16 rows of stride ld_out (ld_out % 8 == 0, dst 16-byte aligned): whole chunks, so the columns
+// [F, 8 ceil(F/8)) receive the shard's pad.  SVEC = 4 / 2 / 1 widens them into FP32 [n, F] with stores of SVEC floats.
+// Same shard staging and search as gather_rows_sharded_kernel; LANES lanes per row of ceil(F/8) chunks.
+template <int LANES, int SVEC>
+__global__ void __launch_bounds__(kThreads)
+    gather_rows_sharded_bf16_kernel(void *__restrict__ dst, uint32_t ld_out, const uint4 *const *__restrict__ shards,
+                                    const uint32_t *__restrict__ offsets, int n_shards, uint32_t pitch,
+                                    const uint32_t *__restrict__ ids, uint32_t n, uint32_t F) {
+  __shared__ uint32_t s_off[kMaxShards + 1];
+  __shared__ const uint4 *s_shard[kMaxShards];
+  for (int i = threadIdx.x; i <= n_shards; i += blockDim.x) {
+    s_off[i] = __ldg(offsets + i);
+    if (i < n_shards)
+      s_shard[i] = shards[i];
+  }
+  __syncthreads();
+  constexpr uint32_t kRowsPerBlock = kThreads / LANES;
+  const uint32_t sub = threadIdx.x & (LANES - 1);
+  const uint32_t nvec = (F + 7) / 8;
+  for (uint64_t k = (uint64_t)blockIdx.x * kRowsPerBlock + threadIdx.x / LANES; k < n;
+       k += (uint64_t)gridDim.x * kRowsPerBlock) {
+    const uint32_t id = __ldg(ids + k);
+    int lo = 0, hi = n_shards;
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (s_off[mid] <= id)
+        lo = mid;
+      else
+        hi = mid;
+    }
+    const uint4 *s = s_shard[lo] + (size_t)(id - s_off[lo]) * (pitch / 8);
+    for (uint32_t c0 = sub; c0 < nvec; c0 += kGatherUnroll * LANES) {
+      uint4 v[kGatherUnroll];
+#pragma unroll
+      for (int u = 0; u < kGatherUnroll; u++)
+        if (c0 + u * LANES < nvec)
+          v[u] = __ldg(s + c0 + u * LANES);
+#pragma unroll
+      for (int u = 0; u < kGatherUnroll; u++) {
+        const uint32_t c = c0 + u * LANES;
+        if (c < nvec) {
+          if constexpr (SVEC == 0) {
+            reinterpret_cast<uint4 *>(dst)[(size_t)k * (ld_out / 8) + c] = v[u];
+          } else {
+            float *d = reinterpret_cast<float *>(dst) + (size_t)k * F;
+            const float8v x = widen(v[u]);
+            store_vec4<SVEC>(d, 8 * c, x.lo, F);
+            if (8 * c + 4 < F)
+              store_vec4<SVEC>(d, 8 * c + 4, x.hi, F);
+          }
+        }
+      }
+    }
+  }
+}
+
+template <int LANES>
+static void launch_gather_rows_sharded_bf16(int svec, unsigned grid, cudaStream_t st, void *dst, uint32_t ld_out,
+                                            const uint4 *const *shards, const uint32_t *offsets, int n_shards,
+                                            uint32_t pitch, const uint32_t *ids, uint32_t n, uint32_t F) {
+  if (svec == 0)
+    gather_rows_sharded_bf16_kernel<LANES, 0><<<grid, kThreads, 0, st>>>(dst, ld_out, shards, offsets, n_shards, pitch,
+                                                                         ids, n, F);
+  else if (svec == 4)
+    gather_rows_sharded_bf16_kernel<LANES, 4><<<grid, kThreads, 0, st>>>(dst, ld_out, shards, offsets, n_shards, pitch,
+                                                                         ids, n, F);
+  else if (svec == 2)
+    gather_rows_sharded_bf16_kernel<LANES, 2><<<grid, kThreads, 0, st>>>(dst, ld_out, shards, offsets, n_shards, pitch,
+                                                                         ids, n, F);
+  else
+    gather_rows_sharded_bf16_kernel<LANES, 1><<<grid, kThreads, 0, st>>>(dst, ld_out, shards, offsets, n_shards, pitch,
+                                                                         ids, n, F);
+}
+
 // msg[e,:] (=|+=) x[dst(e),:] : destination row broadcast over its CSC segment
 template <int VEC, bool ACCUM>
 __global__ void __launch_bounds__(kThreads)
@@ -1020,6 +1095,42 @@ int nts_gather_rows_sharded(float *dst, const float *const *shards, const nts_vi
     launch_gather_rows_sharded<16>(svec, grid, st, dst, shards, shard_offsets, n_shards, shard_pitch, ids, n, F);
   else
     launch_gather_rows_sharded<32>(svec, grid, st, dst, shards, shard_offsets, n_shards, shard_pitch, ids, n, F);
+  NTS_LAUNCH_CHECK();
+  return 0;
+}
+
+int nts_gather_rows_sharded_bf16(void *dst, int dst_dtype, nts_vid_t dst_ld, const void *const *shards,
+                                 const nts_vid_t *shard_offsets, int n_shards, nts_vid_t shard_pitch,
+                                 const nts_vid_t *ids, nts_vid_t n, nts_vid_t feature_size, void *stream) {
+  NTS_ARG_CHECK(dst_dtype == NTS_DTYPE_BF16 || dst_dtype == NTS_DTYPE_F32,
+                "nts_gather_rows_sharded_bf16: dst_dtype must be NTS_DTYPE_BF16 or NTS_DTYPE_F32");
+  NTS_ARG_CHECK(shard_pitch % 8 == 0 && shard_pitch >= feature_size,
+                "nts_gather_rows_sharded_bf16: shard_pitch must be a multiple of 8 and at least feature_size");
+  NTS_ARG_CHECK(dst_dtype == NTS_DTYPE_F32 ? dst_ld == feature_size : (dst_ld % 8 == 0 && dst_ld >= feature_size),
+                "nts_gather_rows_sharded_bf16: dst_ld must be feature_size (FP32) or a multiple of 8 >= feature_size "
+                "(BF16)");
+  if (n == 0 || feature_size == 0)
+    return 0;
+  NTS_ARG_CHECK(dst && shards && shard_offsets && ids, "null pointer passed to nts_gather_rows_sharded_bf16");
+  NTS_ARG_CHECK(n_shards >= 1 && n_shards <= kMaxShards, "nts_gather_rows_sharded_bf16 needs 1..32 shards");
+  NTS_ARG_CHECK(dst_dtype == NTS_DTYPE_F32 || aligned_to(dst, 16),
+                "nts_gather_rows_sharded_bf16: BF16 rows need a 16-byte aligned dst");
+  const uint32_t F = feature_size, nvec = (F + 7) / 8;
+  const int svec = dst_dtype == NTS_DTYPE_BF16 ? 0 : pick_vec(F, dst, dst);
+  const int lanes = nvec <= 8 ? 8 : (nvec <= 16 ? 16 : 32);
+  const uint64_t rows_per_block = kThreads / lanes;
+  const uint64_t cap = (uint64_t)sm_count() * 16;
+  const unsigned grid = (unsigned)std::min<uint64_t>((n + rows_per_block - 1) / rows_per_block, cap);
+  cudaStream_t st = as_stream(stream);
+  const uint4 *const *sh = reinterpret_cast<const uint4 *const *>(shards);
+  if (lanes == 8)
+    launch_gather_rows_sharded_bf16<8>(svec, grid, st, dst, dst_ld, sh, shard_offsets, n_shards, shard_pitch, ids, n, F);
+  else if (lanes == 16)
+    launch_gather_rows_sharded_bf16<16>(svec, grid, st, dst, dst_ld, sh, shard_offsets, n_shards, shard_pitch, ids, n,
+                                        F);
+  else
+    launch_gather_rows_sharded_bf16<32>(svec, grid, st, dst, dst_ld, sh, shard_offsets, n_shards, shard_pitch, ids, n,
+                                        F);
   NTS_LAUNCH_CHECK();
   return 0;
 }

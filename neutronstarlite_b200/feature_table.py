@@ -1,12 +1,16 @@
-"""A [V, F] float32 feature table sharded by row ranges over the GPUs of one node, read by global row id from any rank.
+"""A [V, F] feature table sharded by row ranges over the GPUs of one node, read by global row id from any rank.
 
-`ShardedFeatureTable(local_rows, offsets, group)` is collective over the process group: rank r owns rows
-[offsets[r], offsets[r+1]) (any non-decreasing split of [0, V), empty shards allowed; the callers' default is
+`ShardedFeatureTable(local_rows, offsets, group, dtype=torch.float32)` is collective over the process group: rank r
+owns rows [offsets[r], offsets[r+1]) (any non-decreasing split of [0, V), empty shards allowed; the callers' default is
 graph.partition_offsets_from_out_degree, the reference's partitioner) and keeps them in one device buffer of its own
 at a pitch of 4*ceil(F/4) floats.  The ranks exchange CUDA-IPC handles of these buffers once, so that every rank maps
 every other rank's shard (peer memory, reached over NVLink between GPUs), and `gather(ids)` reads the rows of any ids
 with one launch of nts_gather_rows_sharded (include/nts_b200.h).  A torch caching-allocator tensor cannot be exported
 as it is (an IPC handle names the allocation's base, not the sub-block), hence the table's own buffer.
+
+dtype=torch.bfloat16 stores the rows rounded to BF16 (nts_rows_to_bf16, round to nearest even) at a pitch of
+8*ceil(F/8) values with zero pad columns: half the memory, and half the bytes per gathered row, local or remote.  Its
+gathers run nts_gather_rows_sharded_bf16 and return BF16 rows, or the same rows widened to float32 on request.
 
 Scope is one node: at most 32 ranks in one CUDA-IPC domain, as for the exchange engine (exchange.py).  With one rank
 (or no process group) the table is a single shard and `gather` is a local gather."""
@@ -31,15 +35,17 @@ def _group_rank_world(group):
 
 
 class ShardedFeatureTable:
-    """See the module docstring.  Attributes: rows (V), F, pitch, offsets ([world+1] numpy), rank, world, group,
-    device."""
+    """See the module docstring.  Attributes: rows (V), F, dtype, pitch (in elements of dtype), local_bytes (this
+    rank's shard buffer), offsets ([world+1] numpy), rank, world, group, device."""
 
-    def __init__(self, local_rows, offsets, group=None):
+    def __init__(self, local_rows, offsets, group=None, dtype=torch.float32):
         self.group = group
         self.rank, self.world = _group_rank_world(group)
         if self.world > MAX_SHARDS:
             raise _lib.NtsError("a sharded feature table spans at most %d ranks, the group has %d"
                                 % (MAX_SHARDS, self.world))
+        if dtype not in (torch.float32, torch.bfloat16):
+            raise _lib.NtsError("a feature table stores torch.float32 or torch.bfloat16 rows, not %s" % (dtype,))
         off = np.asarray(offsets, dtype=np.int64).reshape(-1)
         if off.size != self.world + 1 or off[0] != 0 or (np.diff(off) < 0).any() or off[-1] >= 2 ** 32:
             raise _lib.NtsError("offsets must be %d non-decreasing row ids starting at 0, got %s"
@@ -50,17 +56,23 @@ class ShardedFeatureTable:
         lo, hi = int(off[self.rank]), int(off[self.rank + 1])
         if x.shape[0] != hi - lo:
             raise _lib.NtsError("rank %d owns rows [%d, %d) but local_rows has %d rows" % (self.rank, lo, hi, x.shape[0]))
-        self.offsets, self.rows, self.F = off, int(off[-1]), int(x.shape[1])
-        self.pitch = (self.F + 3) // 4 * 4
+        self.offsets, self.rows, self.F, self.dtype = off, int(off[-1]), int(x.shape[1]), dtype
+        bf16 = dtype == torch.bfloat16
+        self.pitch = (self.F + 7) // 8 * 8 if bf16 else (self.F + 3) // 4 * 4
         self.device = x.device
         self._peers = []
         L = _lib.load()
         n = (hi - lo) * self.pitch
-        self._buf = L.nts_malloc_device(max(n, 4) * 4)
+        self.local_bytes = n * (2 if bf16 else 4)
+        self._buf = L.nts_malloc_device(max(self.local_bytes, 16))
         if not self._buf:
             raise _lib.NtsError("nts_malloc_device failed: " + L.nts_last_error().decode(errors="replace"))
         try:
-            if n:
+            if n and bf16:
+                x = x.contiguous()
+                _lib.call("nts_rows_to_bf16", x.data_ptr(), 0, self.F, self._buf, hi - lo, self.F, self.pitch,
+                          _stream())
+            elif n:
                 mine = torch.as_tensor(_DeviceArray(self._buf, n, "<f4"), device=self.device).view(hi - lo, self.pitch)
                 mine[:, self.F:].zero_()
                 mine[:, :self.F].copy_(x)
@@ -71,11 +83,14 @@ class ShardedFeatureTable:
                 h = C.create_string_buffer(64)
                 _lib.call("nts_ipc_get_handle", self._buf, h)
                 info = [None] * self.world
-                dist.all_gather_object(info, (bytes(h.raw), self.F), group=group)
-                widths = sorted(set(f for _, f in info))
+                dist.all_gather_object(info, (bytes(h.raw), self.F, str(dtype)), group=group)
+                widths = sorted(set(f for _, f, _ in info))
                 if len(widths) != 1:
                     raise _lib.NtsError("the ranks' local_rows have different widths: %s" % widths)
-                for j, (hj, _) in enumerate(info):
+                dtypes = sorted(set(d for _, _, d in info))
+                if len(dtypes) != 1:
+                    raise _lib.NtsError("the ranks' tables have different dtypes: %s" % dtypes)
+                for j, (hj, _, _) in enumerate(info):
                     if j == self.rank:
                         continue
                     p = L.nts_ipc_open_handle(hj)
@@ -89,9 +104,12 @@ class ShardedFeatureTable:
             self._release()
             raise
 
-    def gather(self, ids):
-        """Rows of the global ids `ids` (any integer tensor, numpy array or list; any order, repeats allowed) as a
-        [n, F] float32 tensor on this rank's device.  Ids outside [0, V) raise NtsError before any device work."""
+    def gather(self, ids, dtype=None):
+        """Rows of the global ids `ids` (any integer tensor, numpy array or list; any order, repeats allowed) as an
+        [n, F] tensor on this rank's device, of the table's dtype by default.  A BF16 table returns a [n, F] view of
+        [n, pitch] BF16 rows, or with dtype=torch.float32 the rows widened exactly; a float32 table refuses a BF16
+        output.  Ids outside [0, V) and a refused dtype raise NtsError before any device work."""
+        self._out_dtype(dtype)
         if torch.is_tensor(ids) and ids.is_cuda:
             if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
                 raise _lib.NtsError("ids must be an integer tensor, not %s" % ids.dtype)
@@ -104,18 +122,34 @@ class ShardedFeatureTable:
             if a.size and (a.min() < 0 or a.max() >= self.rows):
                 raise _lib.NtsError("row ids must be in [0, %d)" % self.rows)
             t = torch.from_numpy(a.astype(np.int32)).to(self.device)
-        return self._gather(t)
+        return self._gather(t, dtype)
 
-    def _gather(self, ids):
+    def _out_dtype(self, dtype):
+        dtype = self.dtype if dtype is None else dtype
+        if dtype not in (torch.float32, torch.bfloat16) or (dtype == torch.bfloat16 and self.dtype == torch.float32):
+            raise _lib.NtsError("a %s table gathers %s rows, not %s"
+                                % (self.dtype, "float32" if self.dtype == torch.float32 else "bfloat16 or float32",
+                                   dtype))
+        return dtype
+
+    def _gather(self, ids, dtype=None):
         """gather() without the range check, for ids known to be in [0, V): a contiguous int32 device tensor holding
         uint32 values (a sampled block's src)."""
         if self._buf is None:
             raise _lib.NtsError("the feature table is closed")
+        dtype = self._out_dtype(dtype)
         n = int(ids.numel())
-        out = torch.empty((n, self.F), dtype=torch.float32, device=self.device)
-        _lib.call("nts_gather_rows_sharded", out.data_ptr(), self._shards.data_ptr(), self._offsets.data_ptr(),
-                  self.world, self.pitch, ids.data_ptr() if n else None, n, self.F, _stream())
-        return out
+        idp = ids.data_ptr() if n else None
+        if self.dtype == torch.float32:
+            out = torch.empty((n, self.F), dtype=torch.float32, device=self.device)
+            _lib.call("nts_gather_rows_sharded", out.data_ptr(), self._shards.data_ptr(), self._offsets.data_ptr(),
+                      self.world, self.pitch, idp, n, self.F, _stream())
+            return out
+        ld = self.pitch if dtype == torch.bfloat16 else self.F
+        out = torch.empty((n, ld), dtype=dtype, device=self.device)
+        _lib.call("nts_gather_rows_sharded_bf16", out.data_ptr(), 1 if dtype == torch.bfloat16 else 0, ld,
+                  self._shards.data_ptr(), self._offsets.data_ptr(), self.world, self.pitch, idp, n, self.F, _stream())
+        return out[:, :self.F]
 
     def close(self):
         """Collective: synchronise this device, a barrier (no rank is still reading a peer's shard), then close the

@@ -368,29 +368,41 @@ class MiniBatchFuseOp(ntsGraphOp):
     table=True: X is the whole [V, F] feature table and the forward gathers by the block's global source ids
     (row_global), so the table rows of the block's sources are never copied out first; the table must have at least
     the graph's V rows (sampled_subgraph.vertices).  Such an op has no backward: it is the first graph op of the
-    model, which the tape never back-propagates."""
+    model, which the tape never back-propagates.
 
-    def __init__(self, sampled_subgraph, hop, table=False):
+    gather_dtype=torch.bfloat16: both directions gather BF16 rows with FP32 accumulation (nts_segment_gather_sum_bf16);
+    Y and dX stay float32.  A bfloat16 X (the table or local rows) is used as it is: rows of a pitch ld % 8 == 0
+    (ld >= F, e.g. a [:, :F] view of [n, ld] rows), 16-byte aligned.  A float32 X, and dY in the backward, are rounded
+    once into pitched scratch rows (nts_rows_to_bf16)."""
+
+    def __init__(self, sampled_subgraph, hop, table=False, gather_dtype=None):
         super().__init__(sampled_subgraph, None)
         self.block = sampled_subgraph.blocks[hop]
         self.hop, self.table = int(hop), bool(table)
+        self.gather_dtype = _check_gather_dtype(gather_dtype)
         self.vertices = getattr(sampled_subgraph, "vertices", None)
         if self.table and (self.block.row_global is None or self.vertices is None):
             raise _lib.NtsError("table=True needs the block's global source ids (row_global) and the graph's vertex "
                                 "count (SampledSubgraph.vertices)")
 
     def forward(self, f_input, f_input1=None):
-        x = _check_input(f_input, "input")
         b = self.block
+        if self.gather_dtype is None:
+            x = _check_input(f_input, "input")
+        else:
+            x = _check_bf16_operand(_check_gathered(f_input, "input", self.gather_dtype, pitched=True), "input")
         if self.table and x.shape[0] < self.vertices:
             raise _lib.NtsError("the feature table has %d rows, the sampled graph has %d vertices"
                                 % (x.shape[0], self.vertices))
         if not self.table and x.shape[0] != b.n_src:
             raise _lib.NtsError("input has %d rows, hop %d has %d sources" % (x.shape[0], self.hop, b.n_src))
         y = torch.zeros((b.n_dst, x.shape[1]), dtype=torch.float32, device=x.device)
-        with _timed("minibatch_fwd", x.shape[1], b.n_edges, b.n_dst):
-            return segment_gather_sum(y, x, b.weight, b.row_global if self.table else b.row_indices,
-                                      b.column_offset, 0, b.n_dst, b.n_edges)
+        idx = b.row_global if self.table else b.row_indices
+        if self.gather_dtype is None:
+            with _timed("minibatch_fwd", x.shape[1], b.n_edges, b.n_dst):
+                return segment_gather_sum(y, x, b.weight, idx, b.column_offset, 0, b.n_dst, b.n_edges)
+        return segment_gather_sum_bf16(y, _bf16_rows(x, "minibatch_bf16_round"), b.weight, idx, b.column_offset,
+                                       b.n_dst, b.n_edges, "minibatch_fwd_bf16")
 
     def backward(self, f_output_grad):
         if self.table:
@@ -400,8 +412,43 @@ class MiniBatchFuseOp(ntsGraphOp):
         if g.shape[0] != b.n_dst:
             raise _lib.NtsError("output_grad has %d rows, hop %d has %d destinations" % (g.shape[0], self.hop, b.n_dst))
         dx = torch.zeros((b.n_src, g.shape[1]), dtype=torch.float32, device=g.device)
-        with _timed("minibatch_bwd", g.shape[1], b.n_edges, b.n_src):
-            return segment_gather_sum(dx, g, b.weight_backward, b.column_indices, b.row_offset, 0, b.n_src, b.n_edges)
+        if self.gather_dtype is None:
+            with _timed("minibatch_bwd", g.shape[1], b.n_edges, b.n_src):
+                return segment_gather_sum(dx, g, b.weight_backward, b.column_indices, b.row_offset, 0, b.n_src,
+                                          b.n_edges)
+        return segment_gather_sum_bf16(dx, _bf16_rows(g, "minibatch_bf16_round"), b.weight_backward, b.column_indices,
+                                       b.row_offset, b.n_src, b.n_edges, "minibatch_bwd_bf16")
+
+
+def _check_bf16_operand(t, name):
+    """A bfloat16 operand of K1 on BF16 rows must already have its layout: row pitch % 8 == 0, 16-byte aligned."""
+    if t.dtype == torch.bfloat16 and (t.stride(0) % 8 != 0 or t.data_ptr() % 16 != 0):
+        raise _lib.NtsError("a bfloat16 %s needs rows of a pitch that is a multiple of 8 values (e.g. a [:, :F] view "
+                            "of [n, 8*ceil(F/8)] rows), 16-byte aligned; got pitch %d" % (name, t.stride(0)))
+    return t
+
+
+def _bf16_rows(t, tag):
+    """(rows, ld): a bfloat16 t as it is, a float32 t rounded once into [n, 8*ceil(F/8)] rows (nts_rows_to_bf16)."""
+    if t.dtype == torch.bfloat16:
+        return t, int(t.stride(0))
+    n, F = t.shape
+    ld = (F + 7) // 8 * 8
+    r = torch.empty((n, ld), dtype=torch.bfloat16, device=t.device)
+    with _timed(tag, F, 0, n):
+        _lib.call("nts_rows_to_bf16", _ptr(t), _DTYPE_CODE[torch.float32], int(t.stride(0)), _ptr(r), n, F, ld,
+                  _stream())
+    return r[:, :F], ld
+
+
+def segment_gather_sum_bf16(out, rows, weight, indices, offsets, n_rows, n_edges, tag="segment_gather_sum_bf16"):
+    """out[r,:F] += sum_e float(x[indices[e],:F]) * weight[e] for rows = (x, ld): BF16 rows of pitch ld
+    (nts_segment_gather_sum_bf16)."""
+    x, ld = rows
+    with _timed(tag, out.shape[1], n_edges, n_rows):
+        _lib.call("nts_segment_gather_sum_bf16", _ptr(x), ld, _ptr(out), _ptr(weight), _ptr(indices), _ptr(offsets),
+                  int(n_rows), int(n_edges), int(out.shape[1]), _stream())
+    return out
 
 
 class ForwardGPUfuseOp(ntsGraphOp):

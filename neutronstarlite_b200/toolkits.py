@@ -246,8 +246,8 @@ class GCNEagerImpl(GCNImpl):
         self.ctx.appendNNOp(self.X[-1], self.loss)
 
 
-def _minibatch_op(sampled_subgraph, active, hop, table=False):
-    return ops.MiniBatchFuseOp(sampled_subgraph, hop, table=table)
+def _minibatch_op(sampled_subgraph, active, hop, table=False, gather_dtype=None):
+    return ops.MiniBatchFuseOp(sampled_subgraph, hop, table=table, gather_dtype=gather_dtype)
 
 
 class _SampledRounds:
@@ -278,11 +278,12 @@ class _SampledRounds:
         self.table, self.features, self.device = features, None, features.device
         self.rank, self.world = features.rank, features.world
 
-    def _input_rows(self, src):
-        """Features of the sampled sources `src` (global ids of a block, from the sampler: in range)."""
+    def _input_rows(self, src, dtype=torch.float32):
+        """Features of the sampled sources `src` (global ids of a block, from the sampler: in range), as float32 rows,
+        or from a BF16 table with dtype=torch.bfloat16 as BF16 rows ([n, F] view of pitched rows)."""
         if self.table is None:
             return self.features.index_select(0, src.long())
-        return self.table._gather(src)
+        return self.table._gather(src, dtype)
 
     def _batches(self, ids):
         """The seeds this rank runs in each round of a pass over `ids` (None in a round without a batch for it); sets
@@ -377,14 +378,22 @@ class GCNSampleImpl(_SampledRounds):
     at least 32 edges on small blocks); such rows sum in scheduling order and may differ in the last bits between
     runs (DESIGN.md §3 K8).
 
-    features: the [V, F] tensor, or a feature_table.ShardedFeatureTable for data-parallel rounds over its ranks
-    (_SampledRounds); the first layer then gathers the deepest hop's distinct sources from the table once
-    (nts_gather_rows_sharded) and aggregates them on local ids with K1.  `partitioned_graph` is the whole graph as a
-    single partition on every rank."""
+    features: the [V, F] tensor, or a feature_table.ShardedFeatureTable (float32 or bfloat16) for data-parallel rounds
+    over its ranks (_SampledRounds); the first layer then gathers the deepest hop's distinct sources from the table
+    once (nts_gather_rows_sharded, _bf16) and aggregates them on local ids with K1.  `partitioned_graph` is the whole
+    graph as a single partition on every rank.
+
+    gather_dtype=torch.bfloat16: every aggregation gathers BF16 rows with FP32 accumulation (ops.MiniBatchFuseOp's
+    option, nts_segment_gather_sum_bf16); activations, weights and gradients stay float32.  Tensor features are then
+    stored once as pitched BF16 rows [V, 8*ceil(F/8)] (the caller's tensor is left alone), which the first layer reads
+    by global id; a BF16 table hands its rows over as BF16, a float32 table's gathered rows are rounded once.  With
+    FP32 gathers a BF16 table's rows are widened exactly.  The reproducibility condition above holds as it is."""
 
     def __init__(self, partitioned_graph, layers, features, labels, mask, fanout, batch_size, learn_rate=0.01,
-                 weight_decay=0.0001, decay_rate=0.97, decay_epoch=100, drop_rate=0.5, seed=0, sample_seed=0):
+                 weight_decay=0.0001, decay_rate=0.97, decay_epoch=100, drop_rate=0.5, seed=0, sample_seed=0,
+                 gather_dtype=None):
         self.layers = list(layers)
+        self.gather_dtype = ops._check_gather_dtype(gather_dtype)
         if len(fanout) != len(self.layers) - 1:
             raise _lib.NtsError("fanout needs one entry per layer (%d), got %d" % (len(self.layers) - 1, len(fanout)))
         self.batch_size = int(batch_size)
@@ -393,6 +402,9 @@ class GCNSampleImpl(_SampledRounds):
         from .sample import NeighborSampler
         self.sampler = NeighborSampler(partitioned_graph, fanout, self.batch_size)
         self._init_features(features, self.sampler.V)
+        self.features16 = None
+        if self.gather_dtype is not None and self.table is None:
+            self.features16 = ops._bf16_rows(self.features, "minibatch_bf16_round")[0]
         self.drop_rate = drop_rate
         self.sample_seed = int(sample_seed)
         self.step = 0
@@ -420,15 +432,20 @@ class GCNSampleImpl(_SampledRounds):
         self.subgraph = sg = self.sampler.sample(seeds, self.sample_seed, self.step)
         self.step += 1
         L = len(self.layers) - 1
-        x = self.features if self.table is None else self._input_rows(sg.blocks[L - 1].src)
+        if self.table is None:
+            x = self.features if self.features16 is None else self.features16
+        else:
+            bf16 = self.gather_dtype is not None and self.table.dtype == torch.bfloat16
+            x = self._input_rows(sg.blocks[L - 1].src, torch.bfloat16 if bf16 else torch.float32)
         for l in range(L):
             hop = L - 1 - l
             if l != 0 and training and self.drop_rate > 0:
                 dropped = torch.nn.functional.dropout(x, self.drop_rate, training=True)
                 self.ctx.appendNNOp(x, dropped)
                 x = dropped
-            y = self.ctx.runGraphOp(_minibatch_op, sg, None, x.contiguous(), hop=hop,
-                                    table=l == 0 and self.table is None)
+            # the first layer's rows are contiguous float32 or pitched BF16 rows, which contiguous() would unpitch
+            y = self.ctx.runGraphOp(_minibatch_op, sg, None, x if l == 0 else x.contiguous(), hop=hop,
+                                    table=l == 0 and self.table is None, gather_dtype=self.gather_dtype)
             if l == L - 1:
                 x = self.ctx.runVertexForward(lambda n, _l=l: self.P[_l].forward(n), y)
             else:
@@ -604,7 +621,8 @@ class GATSampleImpl(_SampledRounds):
     (DESIGN.md §3 K8).
 
     features: the [V, F] tensor, or a feature_table.ShardedFeatureTable for data-parallel rounds over its ranks
-    (_SampledRounds); the first layer then reads its sources' rows from the table (nts_gather_rows_sharded).
+    (_SampledRounds); the first layer then reads its sources' rows from the table (nts_gather_rows_sharded).  A
+    bfloat16 table's rows are widened exactly to float32 (nts_gather_rows_sharded_bf16), since they feed x W.
     `partitioned_graph` is the whole graph as a single partition on every rank."""
 
     def __init__(self, partitioned_graph, layers, features, labels, mask, fanout, batch_size, heads=8,
