@@ -679,6 +679,18 @@ nts_sampler *nts_sampler_create(const nts_vid_t *column_offset, const nts_vid_t 
 nts_sampler *nts_sampler_create_ex(const nts_vid_t *column_offset, const nts_vid_t *row_indices,
                                    const float *edge_weight, nts_vid_t n_vertices, uint64_t n_edges,
                                    nts_vid_t max_seeds, int hops, const int *fanout, uint32_t flags, void *stream);
+/* The same sampler over a CSC sharded by destination ranges: shard o holds destinations [shard_offsets[o],
+ * shard_offsets[o+1]) as column_offsets[o][local dst + 1] (local offsets), row_indices[o] (global source ids) and
+ * edge_weights[o], in the slot order of the whole-graph CSC, so the blocks equal nts_sampler_create_ex's on the
+ * concatenated shards bit for bit.  The shard arrays may be any device memory the stream's device can read, peer
+ * memory included.  column_offsets / row_indices / edge_weights are host arrays of n_shards device pointers and
+ * shard_offsets a host array of n_shards + 1 ids; all are copied at create.  1 <= n_shards <= 32; shard_offsets start
+ * at 0 and do not decrease; V = shard_offsets[n_shards]; empty shards may have null arrays; every shard has fewer than
+ * 2^32 edges.  Used with nts_sampler_sample / _hop_view / _hop_dst_pos / _bytes / _destroy. */
+nts_sampler *nts_sampler_create_sharded(const nts_vid_t *const *column_offsets, const nts_vid_t *const *row_indices,
+                                        const float *const *edge_weights, const nts_vid_t *shard_offsets,
+                                        int n_shards, nts_vid_t max_seeds, int hops, const int *fanout,
+                                        uint32_t flags, void *stream);
 int nts_sampler_sample(nts_sampler *sampler, const nts_vid_t *seeds, nts_vid_t n_seeds, uint64_t seed, uint64_t step,
                        void *stream);
 int nts_sampler_hop_view(const nts_sampler *sampler, int hop, nts_sample_hop_view *view);
@@ -694,6 +706,18 @@ int nts_sampler_destroy(nts_sampler *sampler);
 int nts_sample_transpose(const nts_vid_t *column_offset, const nts_vid_t *row_indices, const float *weight,
                          nts_vid_t n_dst, nts_vid_t n_src, uint64_t n_edges, nts_vid_t *row_offset,
                          nts_vid_t *column_indices, float *weight_backward, void *stream);
+
+/* One weighted CSC from a rank's n_chunks chunk CSCs over the same n_dst destinations (PartitionedGraph's chunks:
+ * column_offsets[o][n_dst+1], row_indices[o] and edge_weights[o] device arrays of chunk o): destination d's slots are
+ * chunk 0's, then chunk 1's, ..., each in its chunk's order, which for the reference's chunks is the slot order of the
+ * single-partition CSC.  Outputs: column_offset[n_dst+1], row_indices_out / edge_weight_out [n_edges], where n_edges
+ * (< 2^32) is the sum of the chunks' edges.  The pointer arrays are host arrays; 1 <= n_chunks <= 32; row / weight
+ * arrays of chunks without edges may be null.  Before any slot is copied the stream is synchronised once to check the
+ * scanned edge count against n_edges and that no chunk with edges has a null array: either is an error, and only
+ * column_offset has been written.  Temporary memory is stream-ordered. */
+int nts_merge_chunk_csc(const nts_vid_t *const *column_offsets, const nts_vid_t *const *row_indices,
+                        const float *const *edge_weights, int n_chunks, nts_vid_t n_dst, uint64_t n_edges,
+                        nts_vid_t *column_offset, nts_vid_t *row_indices_out, float *edge_weight_out, void *stream);
 
 /* ---- feature / label / mask tables (GNNDatum, core/ntsDataloador.hpp) ----------------------------------------------------
  * Text tables exactly as GNNDatum::readFeature_Label_Mask (:156-221) reads them - "id f0 .. fF-1", "id label",

@@ -230,6 +230,10 @@ SIGNATURES.update({
     "nts_sampler_bytes": (_u64, [_vp]),
     "nts_sampler_destroy": (_int, [_vp]),
     "nts_sample_transpose": (_int, [_vp, _vp, _vp, _u32, _u32, _u64, _vp, _vp, _vp, _vp]),
+    "nts_sampler_create_sharded": (_vp, [C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_u32), _int, _u32,
+                                         _int, C.POINTER(_int), _u32, _vp]),
+    "nts_merge_chunk_csc": (_int, [C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), _int, _u32, _u64, _vp, _vp, _vp,
+                                   _vp]),
 })
 
 _lib = None

@@ -19,6 +19,9 @@
 // key's markers after its edges.  One inclusive scan over 64-bit flags (head count in the high word, marker count in
 // the low word) gives each pair its local source id and each edge pair its transposed position (sorted position minus
 // the markers before it), so the transposed block is still stable by edge position.  Markers write dst_pos.
+//
+// nts_sampler_create_sharded: count and select read a destination's CSC from the shard that owns it (ShardTable);
+// the draws use the global destination id, so the blocks are those of the whole-graph sampler.
 #include <cub/cub.cuh>
 
 #include <vector>
@@ -34,6 +37,7 @@ constexpr int kMaxFanout = 64;
 constexpr int kMaxHops = 8;
 constexpr int kSelectWarps = 8;
 constexpr int kThreads = 256;
+constexpr int kMaxShards = 32;       // nts_sampler_create_sharded
 constexpr u32 kMarker = 0x80000000u;   // value bit of a destination marker pair (edge positions are < 2^31)
 
 __host__ __device__ __forceinline__ u64 splitmix64(u64 z) {
@@ -43,16 +47,69 @@ __host__ __device__ __forceinline__ u64 splitmix64(u64 z) {
   return z ^ (z >> 31);
 }
 
+// The CSC sharded by destination ranges (nts_sampler_create_sharded): shard o holds destinations [off[o], off[o+1])
+// with local column offsets; row ids are global.  The table lives in the sampler's device memory.  count_kernel and
+// select_kernel take it as a last parameter, unused (null) by their whole-graph instantiations, whose code is that of
+// the whole-graph kernels they were before the sharded twins existed.
+struct ShardTable {
+  u32 n;
+  u32 off[kMaxShards + 1];
+  const u32 *col[kMaxShards];
+  const u32 *row[kMaxShards];
+  const float *w[kMaxShards];
+};
+
+// The table staged in shared memory, once per block and before any thread of the block returns.
+__device__ __forceinline__ const ShardTable &stage_shards(const ShardTable *__restrict__ table) {
+  __shared__ ShardTable s;
+  const u32 n = table->n;
+  for (u32 i = threadIdx.x; i <= n; i += blockDim.x) {
+    s.off[i] = table->off[i];
+    if (i < n) {
+      s.col[i] = table->col[i];
+      s.row[i] = table->row[i];
+      s.w[i] = table->w[i];
+    }
+  }
+  if (threadIdx.x == 0) s.n = n;
+  __syncthreads();
+  return s;
+}
+
+// The owner of v < V is the last shard with off[o] <= v, so an empty shard (off[o] == off[o+1]) is never chosen; v's
+// in-edges are slots [base, base + deg) of the owner's row / w.
+__device__ __forceinline__ int shard_of(const ShardTable &t, u32 v, u32 &base, u32 &deg) {
+  int lo = 0, hi = (int)t.n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (t.off[mid] <= v) lo = mid; else hi = mid;
+  }
+  const u32 lv = v - t.off[lo];
+  base = t.col[lo][lv];
+  deg = t.col[lo][lv + 1] - base;
+  return lo;
+}
+
+template <bool kSharded>
 __global__ void count_kernel(const u32 *__restrict__ dst, u32 n_dst, const u32 *__restrict__ g_col, u32 V, u32 k,
                              u32 *__restrict__ cnt, u32 *__restrict__ bad, u32 *__restrict__ marker_keys,
-                             u32 *__restrict__ marker_vals) {
+                             u32 *__restrict__ marker_vals, const ShardTable *__restrict__ shards) {
+  const ShardTable *t = nullptr;
+  if constexpr (kSharded) t = &stage_shards(shards);
   const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (i > n_dst) return;
   u32 c = 0;
   if (i < n_dst) {
     const u32 v = dst[i];
     if (v < V) {
-      c = min(g_col[v + 1] - g_col[v], k);
+      u32 deg;
+      if constexpr (kSharded) {
+        u32 base;
+        shard_of(*t, v, base, deg);
+      } else {
+        deg = g_col[v + 1] - g_col[v];
+      }
+      c = min(deg, k);
     } else {
       atomicOr(bad, 1u);
     }
@@ -64,28 +121,39 @@ __global__ void count_kernel(const u32 *__restrict__ dst, u32 n_dst, const u32 *
   cnt[i] = c;   // cnt[n_dst] = 0: the exclusive scan's last element is the edge count
 }
 
+template <bool kSharded>
 __global__ void __launch_bounds__(kSelectWarps * 32)
 select_kernel(const u32 *__restrict__ dst, u32 n_dst, const u32 *__restrict__ g_col, const u32 *__restrict__ g_row,
               const float *__restrict__ g_w, u32 V, u32 k, u64 step_key, u32 hop, const u32 *__restrict__ col,
               u32 *__restrict__ row_global, float *__restrict__ weight, u32 *__restrict__ edge_dst,
-              u32 *__restrict__ keys, u32 *__restrict__ vals) {
+              u32 *__restrict__ keys, u32 *__restrict__ vals, const ShardTable *__restrict__ shards) {
   __shared__ u32 chosen[kSelectWarps][kMaxFanout];
+  const ShardTable *t = nullptr;
+  if constexpr (kSharded) t = &stage_shards(shards);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const u32 d = blockIdx.x * kSelectWarps + warp;
   if (d >= n_dst) return;   // warp-uniform
   const u32 v = dst[d];
   u32 base = 0, deg = 0;
+  const u32 *row = g_row;
+  const float *w = g_w;
   if (v < V) {
-    base = g_col[v];
-    deg = g_col[v + 1] - base;
+    if constexpr (kSharded) {
+      const int o = shard_of(*t, v, base, deg);
+      row = t->row[o];
+      w = t->w[o];
+    } else {
+      base = g_col[v];
+      deg = g_col[v + 1] - base;
+    }
   }
   const u32 e0 = col[d];
   const u64 p0 = (u64)d * k;
   auto emit = [&](u32 i, u32 slot) {
     const u32 e = e0 + i;
-    const u32 s = g_row[base + slot];
+    const u32 s = row[base + slot];
     row_global[e] = s;
-    weight[e] = g_w[base + slot];
+    weight[e] = w[base + slot];
     edge_dst[e] = d;
     keys[p0 + i] = s;
     vals[p0 + i] = e;
@@ -236,6 +304,44 @@ __global__ void permute_kernel(const u32 *__restrict__ svals, u64 n, const u32 *
   w_t[i] = weight[e];
 }
 
+// nts_merge_chunk_csc: a rank's chunk CSCs (same destinations, chunk o's sources before chunk o+1's) merged into
+// one CSC per destination in chunk order.  count: each destination's in-degree over the chunks; a scan; copy: a warp
+// per destination appends each chunk's slots.
+struct ChunkCscs {
+  int n;
+  const u32 *col[kMaxShards];
+  const u32 *row[kMaxShards];
+  const float *w[kMaxShards];
+};
+
+__global__ void merge_count_kernel(const ChunkCscs c, u32 n_dst, u32 *__restrict__ deg, u32 *__restrict__ bad) {
+  const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i > n_dst) return;
+  u32 n = 0;
+  if (i < n_dst)
+    for (int o = 0; o < c.n; ++o) {
+      const u32 d = c.col[o][i + 1] - c.col[o][i];
+      if (d && (!c.row[o] || !c.w[o])) atomicOr(bad, 1u);   // a chunk with edges passed without its arrays
+      n += d;
+    }
+  deg[i] = n;   // deg[n_dst] = 0: the exclusive scan's last element is the edge count
+}
+
+__global__ void merge_copy_kernel(const ChunkCscs c, u32 n_dst, const u32 *__restrict__ out_col,
+                                  u32 *__restrict__ out_row, float *__restrict__ out_w) {
+  const u32 d = blockIdx.x * (blockDim.x / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (d >= n_dst) return;
+  u32 e = out_col[d];
+  for (int o = 0; o < c.n; ++o) {
+    const u32 b = c.col[o][d], n = c.col[o][d + 1] - b;
+    for (u32 j = lane; j < n; j += 32) {
+      out_row[e + j] = c.row[o][b + j];
+      out_w[e + j] = c.w[o][b + j];
+    }
+    e += n;
+  }
+}
+
 inline unsigned blocks_for(u64 n, int threads = kThreads) { return (unsigned)((n + threads - 1) / threads); }
 
 inline int bits_for(u32 v) {
@@ -249,6 +355,7 @@ inline int bits_for(u32 v) {
 struct nts_sampler {
   const u32 *g_col = nullptr, *g_row = nullptr;
   const float *g_w = nullptr;
+  ShardTable *shards = nullptr;   // nts_sampler_create_sharded: the shard table in device memory, else null
   u32 V = 0;
   u32 max_seeds = 0;
   int hops = 0;
@@ -363,9 +470,14 @@ int sample_hop(nts_sampler *s, int h, u64 step_key, cudaStream_t st) {
   const bool inc = s->include_dst;
   const u64 n_pad = (u64)n_dst * k;
   const u64 n_sort = inc ? n_pad + n_dst : n_pad;   // include_dst: the marker pairs follow the edge pairs
-  count_kernel<<<blocks_for((u64)n_dst + 1), kThreads, 0, st>>>(H.dst, n_dst, s->g_col, s->V, k, s->cnt,
-                                                                  s->counts + 2, inc ? s->keys + n_pad : nullptr,
-                                                                  inc ? s->vals + n_pad : nullptr);
+  u32 *const mk = inc ? s->keys + n_pad : nullptr, *const mv = inc ? s->vals + n_pad : nullptr;
+  const unsigned count_grid = blocks_for((u64)n_dst + 1);
+  if (s->shards)
+    count_kernel<true><<<count_grid, kThreads, 0, st>>>(H.dst, n_dst, nullptr, s->V, k, s->cnt, s->counts + 2, mk, mv,
+                                                        s->shards);
+  else
+    count_kernel<false><<<count_grid, kThreads, 0, st>>>(H.dst, n_dst, s->g_col, s->V, k, s->cnt, s->counts + 2, mk,
+                                                         mv, nullptr);
   NTS_LAUNCH_CHECK();
   size_t need = 0;
   NTS_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, need, s->cnt, H.col, (int64_t)n_dst + 1, st));
@@ -373,9 +485,15 @@ int sample_hop(nts_sampler *s, int h, u64 step_key, cudaStream_t st) {
   NTS_CUDA_OK(cub::DeviceScan::ExclusiveSum(s->tmp, need, s->cnt, H.col, (int64_t)n_dst + 1, st));
   const u32 *skeys = s->keys, *svals = s->vals;
   if (n_dst > 0) {
-    select_kernel<<<(n_dst + kSelectWarps - 1) / kSelectWarps, kSelectWarps * 32, 0, st>>>(
-        H.dst, n_dst, s->g_col, s->g_row, s->g_w, s->V, k, step_key, (u32)h, H.col, H.row_global, H.weight,
-        H.edge_dst, s->keys, s->vals);
+    const unsigned grid = (n_dst + kSelectWarps - 1) / kSelectWarps;
+    if (s->shards)
+      select_kernel<true><<<grid, kSelectWarps * 32, 0, st>>>(H.dst, n_dst, nullptr, nullptr, nullptr, s->V, k,
+                                                              step_key, (u32)h, H.col, H.row_global, H.weight,
+                                                              H.edge_dst, s->keys, s->vals, s->shards);
+    else
+      select_kernel<false><<<grid, kSelectWarps * 32, 0, st>>>(H.dst, n_dst, s->g_col, s->g_row, s->g_w, s->V, k,
+                                                               step_key, (u32)h, H.col, H.row_global, H.weight,
+                                                               H.edge_dst, s->keys, s->vals, nullptr);
     NTS_LAUNCH_CHECK();
     cub::DoubleBuffer<u32> kd(s->keys, s->keys_alt), vd(s->vals, s->vals_alt);
     const int end_bit = bits_for(s->V);
@@ -422,27 +540,29 @@ nts_sampler *nts_sampler_create(const nts_vid_t *column_offset, const nts_vid_t 
                                0, stream);
 }
 
-nts_sampler *nts_sampler_create_ex(const nts_vid_t *column_offset, const nts_vid_t *row_indices,
-                                   const float *edge_weight, nts_vid_t n_vertices, uint64_t n_edges,
-                                   nts_vid_t max_seeds, int hops, const int *fanout, uint32_t flags, void *stream) {
-  auto bad = [](const char *msg) -> nts_sampler * {
-    nts::fail(-1, msg, __FILE__, __LINE__);
-    return nullptr;
-  };
-  if (hops < 1 || hops > kMaxHops) return bad("sampler hops must be in 1..8");
-  if (!fanout) return bad("sampler fanout is null");
+} // extern "C"
+
+namespace {
+
+nts_sampler *sampler_fail(const char *msg) {
+  nts::fail(-1, msg, __FILE__, __LINE__);
+  return nullptr;
+}
+
+// the argument checks both constructors share; null when the arguments are valid
+const char *sampler_args_error(int hops, const int *fanout) {
+  if (hops < 1 || hops > kMaxHops) return "sampler hops must be in 1..8";
+  if (!fanout) return "sampler fanout is null";
   for (int h = 0; h < hops; ++h)
-    if (fanout[h] < 1 || fanout[h] > kMaxFanout) return bad("sampler fanout must be in 1..64");
-  if (n_vertices == 0 || n_vertices >= (1u << 31)) return bad("sampler needs 1 <= V < 2^31");
-  if (n_edges >= (1ull << 32)) return bad("sampler needs fewer than 2^32 edges");
-  if (!column_offset || (n_edges && (!row_indices || !edge_weight))) return bad("null graph array passed to sampler");
-  if (flags & ~(uint32_t)NTS_SAMPLER_INCLUDE_DST) return bad("unknown sampler flag bits");
-  nts_sampler *s = new nts_sampler;
+    if (fanout[h] < 1 || fanout[h] > kMaxFanout) return "sampler fanout must be in 1..64";
+  return nullptr;
+}
+
+// a sampler over s's graph (set by the caller): parameters, then the scratch for max_seeds seeds
+nts_sampler *sampler_init(nts_sampler *s, u32 V, nts_vid_t max_seeds, int hops, const int *fanout, uint32_t flags,
+                          void *stream) {
   s->include_dst = (flags & NTS_SAMPLER_INCLUDE_DST) != 0;
-  s->g_col = column_offset;
-  s->g_row = row_indices;
-  s->g_w = edge_weight;
-  s->V = n_vertices;
+  s->V = V;
   s->max_seeds = max_seeds;
   s->hops = hops;
   for (int h = 0; h < hops; ++h) s->fanout[h] = (u32)fanout[h];
@@ -451,6 +571,64 @@ nts_sampler *nts_sampler_create_ex(const nts_vid_t *column_offset, const nts_vid
     return nullptr;
   }
   return s;
+}
+
+} // namespace
+
+extern "C" {
+
+nts_sampler *nts_sampler_create_ex(const nts_vid_t *column_offset, const nts_vid_t *row_indices,
+                                   const float *edge_weight, nts_vid_t n_vertices, uint64_t n_edges,
+                                   nts_vid_t max_seeds, int hops, const int *fanout, uint32_t flags, void *stream) {
+  if (const char *why = sampler_args_error(hops, fanout)) return sampler_fail(why);
+  if (n_vertices == 0 || n_vertices >= (1u << 31)) return sampler_fail("sampler needs 1 <= V < 2^31");
+  if (n_edges >= (1ull << 32)) return sampler_fail("sampler needs fewer than 2^32 edges");
+  if (!column_offset || (n_edges && (!row_indices || !edge_weight)))
+    return sampler_fail("null graph array passed to sampler");
+  if (flags & ~(uint32_t)NTS_SAMPLER_INCLUDE_DST) return sampler_fail("unknown sampler flag bits");
+  nts_sampler *s = new nts_sampler;
+  s->g_col = column_offset;
+  s->g_row = row_indices;
+  s->g_w = edge_weight;
+  return sampler_init(s, n_vertices, max_seeds, hops, fanout, flags, stream);
+}
+
+nts_sampler *nts_sampler_create_sharded(const nts_vid_t *const *column_offsets, const nts_vid_t *const *row_indices,
+                                        const float *const *edge_weights, const nts_vid_t *shard_offsets,
+                                        int n_shards, nts_vid_t max_seeds, int hops, const int *fanout,
+                                        uint32_t flags, void *stream) {
+  if (const char *why = sampler_args_error(hops, fanout)) return sampler_fail(why);
+  if (n_shards < 1 || n_shards > kMaxShards) return sampler_fail("sharded sampler needs 1..32 shards");
+  if (!column_offsets || !row_indices || !edge_weights || !shard_offsets)
+    return sampler_fail("null shard array passed to sampler");
+  if (shard_offsets[0] != 0) return sampler_fail("shard offsets must start at 0");
+  for (int o = 0; o < n_shards; ++o) {
+    if (shard_offsets[o + 1] < shard_offsets[o]) return sampler_fail("shard offsets must be non-decreasing");
+    if (shard_offsets[o + 1] > shard_offsets[o] && (!column_offsets[o] || !row_indices[o] || !edge_weights[o]))
+      return sampler_fail("null graph array of a non-empty shard passed to sampler");
+  }
+  const u32 V = shard_offsets[n_shards];
+  if (V == 0 || V >= (1u << 31)) return sampler_fail("sampler needs 1 <= V < 2^31");
+  if (flags & ~(uint32_t)NTS_SAMPLER_INCLUDE_DST) return sampler_fail("unknown sampler flag bits");
+  ShardTable t{};
+  t.n = (u32)n_shards;
+  for (int o = 0; o <= n_shards; ++o) t.off[o] = shard_offsets[o];
+  for (int o = 0; o < n_shards; ++o) {
+    t.col[o] = column_offsets[o];
+    t.row[o] = row_indices[o];
+    t.w[o] = edge_weights[o];
+  }
+  nts_sampler *s = new nts_sampler;
+  cudaStream_t st = nts::as_stream(stream);
+  cudaError_t e = cudaSuccess;
+  if (s->alloc(&s->shards, 1) != 0 ||
+      (e = cudaMemcpyAsync(s->shards, &t, sizeof(t), cudaMemcpyHostToDevice, st)) != cudaSuccess ||
+      (e = cudaStreamSynchronize(st)) != cudaSuccess) {   // t is on this stack frame
+    if (e != cudaSuccess) nts::fail((int)e, cudaGetErrorString(e), __FILE__, __LINE__);
+    delete s;
+    return nullptr;
+  }
+  return sampler_init(s, V, max_seeds, hops, fanout, flags, stream);
 }
 
 int nts_sampler_sample(nts_sampler *s, const nts_vid_t *seeds, nts_vid_t n_seeds, uint64_t seed, uint64_t step,
@@ -552,6 +730,60 @@ int nts_sample_transpose(const nts_vid_t *column_offset, const nts_vid_t *row_in
   } while (0);
   cudaError_t e = cudaFreeAsync(t, st);
   if (rc == 0 && e != cudaSuccess) rc = nts::fail((int)e, cudaGetErrorString(e), __FILE__, __LINE__);
+  return rc;
+}
+
+int nts_merge_chunk_csc(const nts_vid_t *const *column_offsets, const nts_vid_t *const *row_indices,
+                        const float *const *edge_weights, int n_chunks, nts_vid_t n_dst, uint64_t n_edges,
+                        nts_vid_t *column_offset, nts_vid_t *row_indices_out, float *edge_weight_out, void *stream) {
+  NTS_ARG_CHECK(n_chunks >= 1 && n_chunks <= kMaxShards, "nts_merge_chunk_csc needs 1..32 chunks");
+  NTS_ARG_CHECK(column_offsets && row_indices && edge_weights && column_offset, "null array passed to nts_merge_chunk_csc");
+  NTS_ARG_CHECK(n_edges < (1ull << 32), "nts_merge_chunk_csc needs fewer than 2^32 edges");
+  NTS_ARG_CHECK(n_edges == 0 || (row_indices_out && edge_weight_out), "null output passed to nts_merge_chunk_csc");
+  ChunkCscs c{};
+  c.n = n_chunks;
+  for (int o = 0; o < n_chunks; ++o) {
+    NTS_ARG_CHECK(column_offsets[o] != nullptr, "null chunk column_offset passed to nts_merge_chunk_csc");
+    c.col[o] = column_offsets[o];
+    c.row[o] = row_indices[o];
+    c.w[o] = edge_weights[o];
+  }
+  cudaStream_t st = nts::as_stream(stream);
+  size_t scan_bytes = 0;
+  NTS_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (const u32 *)nullptr, (u32 *)nullptr,
+                                            (int64_t)n_dst + 1, st));
+  const size_t deg_bytes = (((size_t)n_dst + 1) * sizeof(u32) + 255) / 256 * 256;
+  char *t = nullptr;
+  NTS_CUDA_OK(cudaMallocAsync(reinterpret_cast<void **>(&t), deg_bytes + 256 + scan_bytes, st));
+  u32 *deg = reinterpret_cast<u32 *>(t), *bad = reinterpret_cast<u32 *>(t + deg_bytes);
+  // the scanned edge count and the bad-array flag, read back before the copy writes n_edges slots
+  u32 check[2] = {0, 0};
+  cudaError_t e = cudaMemsetAsync(bad, 0, sizeof(u32), st);
+  if (e == cudaSuccess) {
+    merge_count_kernel<<<blocks_for((u64)n_dst + 1), kThreads, 0, st>>>(c, n_dst, deg, bad);
+    ::nts::count_launch();
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess)
+    e = cub::DeviceScan::ExclusiveSum(t + deg_bytes + 256, scan_bytes, deg, column_offset, (int64_t)n_dst + 1, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(check, column_offset + n_dst, sizeof(u32), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(check + 1, bad, sizeof(u32), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  int rc = 0;
+  if (e != cudaSuccess) {
+    rc = nts::fail((int)e, cudaGetErrorString(e), __FILE__, __LINE__);
+  } else if (check[1]) {
+    rc = nts::fail(-1, "nts_merge_chunk_csc: null row / weight array of a chunk with edges", __FILE__, __LINE__);
+  } else if (check[0] != n_edges) {
+    rc = nts::fail(-1, "nts_merge_chunk_csc: n_edges differs from the chunks' edge count", __FILE__, __LINE__);
+  } else if (n_dst) {
+    merge_copy_kernel<<<(n_dst + 7) / 8, 256, 0, st>>>(c, n_dst, column_offset, row_indices_out, edge_weight_out);
+    ::nts::count_launch();
+    e = cudaGetLastError();
+    if (e != cudaSuccess) rc = nts::fail((int)e, cudaGetErrorString(e), __FILE__, __LINE__);
+  }
+  e = cudaFreeAsync(t, st);   // stream-ordered: after the kernels that read it
+  if (rc == 0 && e != cudaSuccess) return nts::fail((int)e, cudaGetErrorString(e), __FILE__, __LINE__);
   return rc;
 }
 

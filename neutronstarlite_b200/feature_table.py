@@ -34,7 +34,74 @@ def _group_rank_world(group):
     return dist.get_rank(group), dist.get_world_size(group)
 
 
-class ShardedFeatureTable:
+class PeerShards:
+    """One device buffer per rank of a process group (nts_malloc_device: a CUDA-IPC handle names the whole
+    allocation), mapped by every other rank.  The lifecycle ShardedFeatureTable and topology.ShardedTopology share:
+    `_alloc` this rank's buffer, fill it, `_share` it (one handle exchange, every peer buffer opened), and `close()`.
+    Subclasses set group, rank and world first."""
+
+    _buf = None
+    _peers = ()
+
+    def _alloc(self, nbytes):
+        L = _lib.load()
+        self._peers = []
+        self._buf = L.nts_malloc_device(max(int(nbytes), 16))
+        if not self._buf:
+            raise _lib.NtsError("nts_malloc_device failed: " + L.nts_last_error().decode(errors="replace"))
+
+    def _share(self, meta):
+        """Collective: (ptrs, metas) - every rank's buffer address in this process, this rank's own first-hand, and
+        every rank's `meta` (any picklable value).  Call once the buffer is filled on the current stream."""
+        if self.world == 1:
+            return [self._buf], [meta]
+        # the fill is complete before any peer can map the buffer: every rank passes this point first
+        torch.cuda.current_stream(self.device).synchronize()
+        L = _lib.load()
+        h = C.create_string_buffer(64)
+        _lib.call("nts_ipc_get_handle", self._buf, h)
+        info = [None] * self.world
+        dist.all_gather_object(info, (bytes(h.raw), meta), group=self.group)
+        ptrs = [self._buf] * self.world
+        for j, (hj, _) in enumerate(info):
+            if j == self.rank:
+                continue
+            p = L.nts_ipc_open_handle(hj)
+            if not p:
+                raise _lib.NtsError("nts_ipc_open_handle failed: " + L.nts_last_error().decode(errors="replace"))
+            self._peers.append(p)
+            ptrs[j] = p
+        return ptrs, [m for _, m in info]
+
+    def close(self):
+        """Collective: synchronise this device, a barrier (no rank is still reading a peer's shard), then close the
+        peer mappings and free this rank's buffer."""
+        if self._buf is None:
+            return
+        torch.cuda.synchronize(self.device)
+        if self.world > 1:
+            dist.barrier(group=self.group)
+        self._release()
+
+    def _release(self):
+        L = _lib.load()
+        for p in self._peers:
+            L.nts_ipc_close_handle(p)
+        self._peers = []
+        if self._buf:
+            L.nts_free_device(self._buf)
+        self._buf = None
+
+    def __del__(self):
+        # without close() a peer may still read this rank's shard: free it only when there is no peer
+        try:
+            if getattr(self, "_buf", None) and self.world == 1:
+                self._release()
+        except Exception:
+            pass
+
+
+class ShardedFeatureTable(PeerShards):
     """See the module docstring.  Attributes: rows (V), F, dtype, pitch (in elements of dtype), local_bytes (this
     rank's shard buffer), offsets ([world+1] numpy), rank, world, group, device."""
 
@@ -60,13 +127,9 @@ class ShardedFeatureTable:
         bf16 = dtype == torch.bfloat16
         self.pitch = (self.F + 7) // 8 * 8 if bf16 else (self.F + 3) // 4 * 4
         self.device = x.device
-        self._peers = []
-        L = _lib.load()
         n = (hi - lo) * self.pitch
         self.local_bytes = n * (2 if bf16 else 4)
-        self._buf = L.nts_malloc_device(max(self.local_bytes, 16))
-        if not self._buf:
-            raise _lib.NtsError("nts_malloc_device failed: " + L.nts_last_error().decode(errors="replace"))
+        self._alloc(self.local_bytes)
         try:
             if n and bf16:
                 x = x.contiguous()
@@ -76,28 +139,13 @@ class ShardedFeatureTable:
                 mine = torch.as_tensor(_DeviceArray(self._buf, n, "<f4"), device=self.device).view(hi - lo, self.pitch)
                 mine[:, self.F:].zero_()
                 mine[:, :self.F].copy_(x)
-            ptrs = [self._buf] * self.world
-            if self.world > 1:
-                # the copy is complete before any peer can map the buffer: every rank passes this point first
-                torch.cuda.current_stream(self.device).synchronize()
-                h = C.create_string_buffer(64)
-                _lib.call("nts_ipc_get_handle", self._buf, h)
-                info = [None] * self.world
-                dist.all_gather_object(info, (bytes(h.raw), self.F, str(dtype)), group=group)
-                widths = sorted(set(f for _, f, _ in info))
-                if len(widths) != 1:
-                    raise _lib.NtsError("the ranks' local_rows have different widths: %s" % widths)
-                dtypes = sorted(set(d for _, _, d in info))
-                if len(dtypes) != 1:
-                    raise _lib.NtsError("the ranks' tables have different dtypes: %s" % dtypes)
-                for j, (hj, _, _) in enumerate(info):
-                    if j == self.rank:
-                        continue
-                    p = L.nts_ipc_open_handle(hj)
-                    if not p:
-                        raise _lib.NtsError("nts_ipc_open_handle failed: " + L.nts_last_error().decode(errors="replace"))
-                    self._peers.append(p)
-                    ptrs[j] = p
+            ptrs, info = self._share((self.F, str(dtype)))
+            widths = sorted(set(f for f, _ in info))
+            if len(widths) != 1:
+                raise _lib.NtsError("the ranks' local_rows have different widths: %s" % widths)
+            dtypes = sorted(set(d for _, d in info))
+            if len(dtypes) != 1:
+                raise _lib.NtsError("the ranks' tables have different dtypes: %s" % dtypes)
             self._shards = torch.tensor(ptrs, dtype=torch.int64).to(self.device)
             self._offsets = torch.from_numpy(off.astype(np.uint32).view(np.int32)).to(self.device)
         except Exception:
@@ -150,30 +198,3 @@ class ShardedFeatureTable:
         _lib.call("nts_gather_rows_sharded_bf16", out.data_ptr(), 1 if dtype == torch.bfloat16 else 0, ld,
                   self._shards.data_ptr(), self._offsets.data_ptr(), self.world, self.pitch, idp, n, self.F, _stream())
         return out[:, :self.F]
-
-    def close(self):
-        """Collective: synchronise this device, a barrier (no rank is still reading a peer's shard), then close the
-        peer mappings and free this rank's buffer."""
-        if self._buf is None:
-            return
-        torch.cuda.synchronize(self.device)
-        if self.world > 1:
-            dist.barrier(group=self.group)
-        self._release()
-
-    def _release(self):
-        L = _lib.load()
-        for p in self._peers:
-            L.nts_ipc_close_handle(p)
-        self._peers = []
-        if self._buf:
-            L.nts_free_device(self._buf)
-        self._buf = None
-
-    def __del__(self):
-        # without close() a peer may still read this rank's shard: free it only when there is no peer
-        try:
-            if getattr(self, "_buf", None) and self.world == 1:
-                self._release()
-        except Exception:
-            pass

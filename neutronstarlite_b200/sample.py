@@ -11,6 +11,10 @@ and the seeds: it does not depend on launch configuration, batch composition or 
 include its destinations, and records each destination's position among them in `SampledBlock.dst_pos`: the block
 layout of a layer whose destinations read their own previous-layer rows (a GAT layer's destination scores).
 
+`NeighborSampler(topology.ShardedTopology, ...)` samples the same way over a CSC sharded by destination ranges over the
+ranks of one node (nts_sampler_create_sharded): each destination's in-edges are read from its owner's shard, local or
+peer memory, and the blocks are those of the single-partition graph, bit for bit.
+
 `SampledSubgraph` holds the blocks of one sample as `SampledBlock`s (device tensors); `ops.MiniBatchFuseOp` and
 `ops.MiniBatchGATOp` aggregate over them."""
 from __future__ import annotations
@@ -133,9 +137,9 @@ def check_fanout(fanout):
 
 class NeighborSampler:
     """K8 on the CSC of a single-partition graph (chunk 0's column_offset_gpu / row_indices_gpu /
-    edge_weight_forward_gpu).  Device scratch for max_seeds seeds is allocated once, here.  `sample()` synchronises
-    the stream once per hop; the blocks it returns are views that the next `sample()` overwrites (clone() them to keep
-    them).
+    edge_weight_forward_gpu), or on a topology.ShardedTopology (the same blocks; the sampler keeps a reference to the
+    topology).  Device scratch for max_seeds seeds is allocated once, here.  `sample()` synchronises the stream once
+    per hop; the blocks it returns are views that the next `sample()` overwrites (clone() them to keep them).
 
     include_dst=True: every hop's sources include its destinations and each block carries dst_pos (module docstring);
     the edges are those of the default mode, bit for bit."""
@@ -143,27 +147,41 @@ class NeighborSampler:
     SAMPLER_INCLUDE_DST = 1   # NTS_SAMPLER_INCLUDE_DST of include/nts_b200.h
 
     def __init__(self, partitioned_graph, fanout, max_seeds, include_dst=False):
+        from .topology import ShardedTopology
         pg = partitioned_graph
-        if pg.partitions != 1:
-            raise _lib.NtsError("NeighborSampler needs a single-partition graph (partitions == 1), got %d"
-                                % pg.partitions)
+        sharded = isinstance(pg, ShardedTopology)
+        if not sharded and pg.partitions != 1:
+            raise _lib.NtsError("NeighborSampler needs a single-partition graph (partitions == 1) or a "
+                                "ShardedTopology, got %d partitions" % pg.partitions)
         self.fanout = check_fanout(fanout)
-        c = pg.graph_chunks[0]
-        if c.column_offset_gpu is None:
-            raise _lib.NtsError("the graph has no device arrays (generate_all(device=...))")
-        self.V = int(pg.global_vertices)
         self.max_seeds = int(max_seeds)
         self.include_dst = bool(include_dst)
-        self.device = c.column_offset_gpu.device
-        self._graph = (c.column_offset_gpu, c.row_indices_gpu, c.edge_weight_forward_gpu)
         L = _lib.load()
         ks = (C.c_int * len(self.fanout))(*self.fanout)
-        self.handle = L.nts_sampler_create_ex(c.column_offset_gpu.data_ptr(), c.row_indices_gpu.data_ptr(),
-                                              c.edge_weight_forward_gpu.data_ptr(), self.V, int(c.edge_size),
-                                              self.max_seeds, len(self.fanout), ks,
-                                              self.SAMPLER_INCLUDE_DST if self.include_dst else 0, _stream())
+        flags = self.SAMPLER_INCLUDE_DST if self.include_dst else 0
+        if sharded:
+            if pg._buf is None:
+                raise _lib.NtsError("the topology is closed")
+            self.V, self.device, self._graph = pg.vertices, pg.device, pg
+            n = len(pg.offsets) - 1
+            cols, rows, ws = ((C.c_void_p * n)(*a) for a in pg.shard_arrays)
+            offs = (C.c_uint32 * (n + 1))(*[int(o) for o in pg.offsets])
+            self.handle = L.nts_sampler_create_sharded(cols, rows, ws, offs, n, self.max_seeds, len(self.fanout), ks,
+                                                       flags, _stream())
+            what = "nts_sampler_create_sharded"
+        else:
+            c = pg.graph_chunks[0]
+            if c.column_offset_gpu is None:
+                raise _lib.NtsError("the graph has no device arrays (generate_all(device=...))")
+            self.V = int(pg.global_vertices)
+            self.device = c.column_offset_gpu.device
+            self._graph = (c.column_offset_gpu, c.row_indices_gpu, c.edge_weight_forward_gpu)
+            self.handle = L.nts_sampler_create_ex(c.column_offset_gpu.data_ptr(), c.row_indices_gpu.data_ptr(),
+                                                  c.edge_weight_forward_gpu.data_ptr(), self.V, int(c.edge_size),
+                                                  self.max_seeds, len(self.fanout), ks, flags, _stream())
+            what = "nts_sampler_create_ex"
         if not self.handle:
-            raise _lib.NtsError("nts_sampler_create_ex failed: " + L.nts_last_error().decode(errors="replace"))
+            raise _lib.NtsError(what + " failed: " + L.nts_last_error().decode(errors="replace"))
 
     def bytes(self):
         return int(_lib.load().nts_sampler_bytes(self.handle))

@@ -7,7 +7,8 @@
   * `GCNEagerImpl` <-> toolkits/GCN_EAGER_single.hpp / GCN_EAGER.hpp order (X.W first, aggregate the narrow result).
   * `GATImpl`    <-> the flow of toolkits/GAT_CPU_DIST_OPTM.hpp on the fused multi-head aggregation (K7).
   * `GCNSampleImpl` <-> toolkits/GCN_CPU_SAMPLE.hpp (neighbour-sampled mini-batch GCN) on the K8 sampler and
-                     ops.MiniBatchFuseOp, on one GPU or data-parallel over a feature_table.ShardedFeatureTable.
+                     ops.MiniBatchFuseOp, on one GPU or data-parallel over a feature_table.ShardedFeatureTable,
+                     with the topology whole on every rank or sharded (topology.ShardedTopology).
   * `GATSampleImpl` <-> GATImpl's layers on GCNSampleImpl's batch loop: neighbour-sampled mini-batch GAT on the K8
                      sampler (destination-inclusive blocks) and K7 through ops.MiniBatchGATOp, on one GPU or
                      data-parallel like GCNSampleImpl.
@@ -261,10 +262,20 @@ class _SampledRounds:
     SUM-reduced the gradients over the ranks in the same parameter order everywhere (the reference's semantics: the
     effective step grows with N).  A rank without a batch in the last round contributes zero gradients and still joins
     every collective.  Mean loss and accuracies are reduced over the ranks at the end of a pass, so every rank returns
-    the same numbers.  Topology, labels and mask are whole-graph on every rank (the reference's FullyRepGraph)."""
+    the same numbers.  Labels and mask are whole-graph on every rank.  The topology is either the whole graph as a
+    single partition on every rank (the reference's FullyRepGraph), or a topology.ShardedTopology, of which each rank
+    keeps only its own destinations' in-edges; the blocks, and so rounds, steps and collectives, are the same either
+    way.  A topology sharded over N > 1 ranks needs a ShardedFeatureTable over the same ranks (its offsets may
+    differ)."""
 
-    def _init_features(self, features, vertices):
+    def _init_features(self, features, vertices, topology):
         from .feature_table import ShardedFeatureTable
+        from .topology import ShardedTopology
+        if isinstance(topology, ShardedTopology) and topology.world > 1 and not (
+                isinstance(features, ShardedFeatureTable) and features.world == topology.world
+                and features.rank == topology.rank):
+            raise _lib.NtsError("a topology sharded over %d ranks needs a ShardedFeatureTable over the same ranks"
+                                % topology.world)
         if not isinstance(features, ShardedFeatureTable):
             self.table, self.rank, self.world = None, 0, 1
             self.features = ops._check_input(features.detach(), "features")
@@ -381,7 +392,8 @@ class GCNSampleImpl(_SampledRounds):
     features: the [V, F] tensor, or a feature_table.ShardedFeatureTable (float32 or bfloat16) for data-parallel rounds
     over its ranks (_SampledRounds); the first layer then gathers the deepest hop's distinct sources from the table
     once (nts_gather_rows_sharded, _bf16) and aggregates them on local ids with K1.  `partitioned_graph` is the whole
-    graph as a single partition on every rank.
+    graph as a single partition on every rank, or a topology.ShardedTopology (each rank keeps its own destinations'
+    in-edges; the same blocks), which over N > 1 ranks needs a ShardedFeatureTable over the same ranks.
 
     gather_dtype=torch.bfloat16: every aggregation gathers BF16 rows with FP32 accumulation (ops.MiniBatchFuseOp's
     option, nts_segment_gather_sum_bf16); activations, weights and gradients stay float32.  Tensor features are then
@@ -401,7 +413,7 @@ class GCNSampleImpl(_SampledRounds):
             raise _lib.NtsError("batch_size must be >= 1")
         from .sample import NeighborSampler
         self.sampler = NeighborSampler(partitioned_graph, fanout, self.batch_size)
-        self._init_features(features, self.sampler.V)
+        self._init_features(features, self.sampler.V, partitioned_graph)
         self.features16 = None
         if self.gather_dtype is not None and self.table is None:
             self.features16 = ops._bf16_rows(self.features, "minibatch_bf16_round")[0]
@@ -623,7 +635,8 @@ class GATSampleImpl(_SampledRounds):
     features: the [V, F] tensor, or a feature_table.ShardedFeatureTable for data-parallel rounds over its ranks
     (_SampledRounds); the first layer then reads its sources' rows from the table (nts_gather_rows_sharded).  A
     bfloat16 table's rows are widened exactly to float32 (nts_gather_rows_sharded_bf16), since they feed x W.
-    `partitioned_graph` is the whole graph as a single partition on every rank."""
+    `partitioned_graph` is the whole graph as a single partition on every rank, or a topology.ShardedTopology as in
+    GCNSampleImpl."""
 
     def __init__(self, partitioned_graph, layers, features, labels, mask, fanout, batch_size, heads=8,
                  learn_rate=0.01, weight_decay=0.0001, decay_rate=0.97, decay_epoch=100, seed=0, sample_seed=0,
@@ -643,7 +656,7 @@ class GATSampleImpl(_SampledRounds):
             _refuse_bf16_gat_layers(self.layers, self.heads)
         from .sample import NeighborSampler
         self.sampler = NeighborSampler(partitioned_graph, fanout, self.batch_size, include_dst=True)
-        self._init_features(features, self.sampler.V)
+        self._init_features(features, self.sampler.V, partitioned_graph)
         self.sample_seed = int(sample_seed)
         self.step = 0
         self.ctx = NtsContext()
