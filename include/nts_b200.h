@@ -395,6 +395,22 @@ int nts_gather_rows_sharded(float *dst, const float *const *shards, const nts_vi
 int nts_gather_rows_sharded_bf16(void *dst, int dst_dtype, nts_vid_t dst_ld, const void *const *shards,
                                  const nts_vid_t *shard_offsets, int n_shards, nts_vid_t shard_pitch,
                                  const nts_vid_t *ids, nts_vid_t n, nts_vid_t feature_size, void *stream);
+/* K9: the weighted gather-sum of K1 with its sources read by global id from a sharded table:
+ * output[r, :F] += sum_{e in [offsets[r], offsets[r+1])} w(e) * row(indices[e]) for r < n_rows (w = weight[e], or 1
+ * when weight is NULL), row(g) = row g - shard_offsets[o] of shards[o] for the shard o that owns g.  Shards as for
+ * nts_gather_rows_sharded (1..32 row ranges, empty ones allowed, each 16-byte aligned) with rows of shard_pitch values
+ * of shard_dtype: NTS_DTYPE_F32 (shard_pitch % 4 == 0) or NTS_DTYPE_BF16 (shard_pitch % 8 == 0, widened exactly,
+ * FP32 accumulation); shard_pitch >= F, and columns past F are never added.  `offsets` holds absolute edge positions
+ * (offsets[0] == edge_begin, offsets[n_rows] == edge_end), and indices / weight are addressed by absolute edge
+ * position, as for nts_segment_gather_sum_range; every index must lie in [shard_offsets[0], shard_offsets[n_shards])
+ * (not checked on the device).  `output` is FP32 [n_rows, F] contiguous, zeroed by the caller.  Work is split by
+ * edges; rows cut by an edge quantum finish with atomics.  n_rows == 0 or an empty edge range launches nothing and
+ * looks at no pointer; layout errors return an error and launch nothing. */
+int nts_segment_gather_sum_sharded(float *output, const void *const *shards, int shard_dtype,
+                                   const nts_vid_t *shard_offsets, int n_shards, nts_vid_t shard_pitch,
+                                   const float *weight, const nts_vid_t *indices, const nts_vid_t *offsets,
+                                   nts_vid_t n_rows, uint64_t edge_begin, uint64_t edge_end, nts_vid_t feature_size,
+                                   void *stream);
 /* dst[rows[k],:] += src[k,:]  (receiver-side add of partial gradients; rows must be unique) */
 int nts_scatter_add_rows(float *dst, const float *src, const nts_vid_t *rows, nts_vid_t n_rows,
                          nts_vid_t feature_size, void *stream);

@@ -172,6 +172,42 @@ class ShardedFeatureTable(PeerShards):
             t = torch.from_numpy(a.astype(np.int32)).to(self.device)
         return self._gather(t, dtype)
 
+    def aggregate(self, out, column_offset, row_indices, weight, edge_begin, edge_end):
+        """out[r, :] += sum over the edges e in [column_offset[r], column_offset[r+1]) of weight[e] * row
+        row_indices[e] of the table (nts_segment_gather_sum_sharded), for r < out.shape[0]: the gather-sum of a CSC
+        slice whose sources are read by global id from every rank's shard, local or peer memory.  BF16 rows are widened
+        exactly and summed in FP32.
+
+        out: float32 CUDA [n_rows, F] contiguous (zero it for a plain sum).  column_offset: int32 CUDA, at least n_rows
+        + 1 absolute edge positions from edge_begin to edge_end (a slice of a whole-graph CSC's offsets, or a shard's
+        local offsets from 0).  row_indices (int32, global ids in [0, V)) and weight (float32, or None for 1) are
+        indexed by absolute edge position.  Asynchronous on the current stream.  A closed table and operands of the
+        wrong kind raise NtsError before any device work."""
+        if self._buf is None:
+            raise _lib.NtsError("the feature table is closed")
+        for name, t, dt in (("out", out, torch.float32), ("column_offset", column_offset, torch.int32),
+                            ("row_indices", row_indices, torch.int32), ("weight", weight, torch.float32)):
+            if t is None and name == "weight":
+                continue
+            if not torch.is_tensor(t) or not t.is_cuda or t.dtype != dt or t.device != self.device \
+                    or not t.is_contiguous():
+                raise _lib.NtsError("%s must be a contiguous %s tensor on %s" % (name, dt, self.device))
+        n_rows = int(out.shape[0]) if out.dim() == 2 else -1
+        if n_rows < 0 or out.shape[1] != self.F:
+            raise _lib.NtsError("out must be [n_rows, %d], got %s" % (self.F, tuple(out.shape)))
+        eb, ee = int(edge_begin), int(edge_end)
+        if column_offset.numel() < n_rows + 1 or not 0 <= eb <= ee <= row_indices.numel() or \
+                (weight is not None and weight.numel() < ee):
+            raise _lib.NtsError("column_offset needs %d entries and [edge_begin, edge_end) = [%d, %d) must lie in the "
+                                "%d edges of row_indices and weight" % (n_rows + 1, eb, ee, row_indices.numel()))
+        if n_rows == 0 or eb == ee:
+            return out
+        _lib.call("nts_segment_gather_sum_sharded", out.data_ptr(), self._shards.data_ptr(),
+                  1 if self.dtype == torch.bfloat16 else 0, self._offsets.data_ptr(), self.world, self.pitch,
+                  None if weight is None else weight.data_ptr(), row_indices.data_ptr(), column_offset.data_ptr(),
+                  n_rows, eb, ee, self.F, _stream())
+        return out
+
     def _out_dtype(self, dtype):
         dtype = self.dtype if dtype is None else dtype
         if dtype not in (torch.float32, torch.bfloat16) or (dtype == torch.bfloat16 and self.dtype == torch.float32):

@@ -483,6 +483,104 @@ class GCNSampleImpl(_SampledRounds):
         self.Update()
         return loss.detach(), correct
 
+    def _own_csc(self):
+        """(lo, hi, own_offsets, parts): this rank's destinations [lo, hi), the ownership offsets the per-layer tables
+        are built on, and the in-edge CSC pieces that cover [lo, hi) in order, as (column offsets [n + 1] int32,
+        row_indices, weight, edge_begin, edge_end) - a ShardedTopology's shards held in this process (all of them
+        after split()), or the slice [lo, hi) of the replicated single-partition CSC."""
+        from .sample import _DeviceArray
+        from .topology import ShardedTopology
+        topo = self.sampler._graph
+        dev = self.device
+
+        def borrowed(ptr, n, typestr):
+            if n == 0:
+                return torch.empty(0, dtype=torch.float32 if typestr == "<f4" else torch.int32, device=dev)
+            return torch.as_tensor(_DeviceArray(ptr, n, typestr), device=dev)
+
+        if isinstance(topo, ShardedTopology):
+            if topo._buf is None:
+                raise _lib.NtsError("the topology is closed")
+            off = [int(o) for o in topo.offsets]
+            mine = range(len(off) - 1) if topo.world == 1 else [topo.rank]
+            parts = []
+            for o in mine:
+                col = borrowed(topo.shard_arrays[0][o], off[o + 1] - off[o] + 1, "<i4")
+                n_edges = int(col[-1])
+                parts.append((col, borrowed(topo.shard_arrays[1][o], n_edges, "<i4"),
+                              borrowed(topo.shard_arrays[2][o], n_edges, "<f4"), 0, n_edges))
+            lo, hi = off[mine[0]], off[mine[-1] + 1]
+            return lo, hi, (off if topo.world > 1 else [0, off[-1]]), parts
+        c_col, c_row, c_w = topo
+        own = [0, self.sampler.V] if self.table is None else [int(o) for o in self.table.offsets]
+        lo, hi = own[self.rank], own[self.rank + 1]
+        col = c_col[lo:hi + 1]
+        eb, ee = (int(e) & 0xFFFFFFFF for e in col[[0, -1]].tolist())
+        return lo, hi, own, [(col, c_row, c_w, eb, ee)]
+
+    @torch.no_grad()
+    def infer(self):
+        """Full-neighbour inference: collective over the ranks of the model's table.  Returns (lo, out), out the last
+        layer's [hi - lo, classes] float32 outputs (before log_softmax, as Forward returns them) for the destinations
+        [lo, hi) this rank owns: a ShardedTopology's, else the table's offsets, else [0, V).
+
+        Layer l aggregates with the expectation of the sampled aggregation of its hop h = L-1-l, which keeps
+        min(indeg(v), k_h) uniform in-edge slots of v:  X_{l+1} = relu(s ⊙ A (X_l W_l)), s_v = min(1, k_h / indeg(v))
+        (1 when indeg(v) = 0), no relu on the last layer, no dropout.  With every fanout >= the largest in-degree it is
+        the full-graph GCN.  A layer that narrows (F_out < F_in) computes H = X_own W_l on this rank first and
+        aggregates H, otherwise it aggregates X and applies W_l after (GCN here has no bias: A(XW) = (AX)W).  The
+        aggregated rows are read by global id from a ShardedFeatureTable (nts_segment_gather_sum_sharded): the
+        features table itself for a widening first layer, otherwise one built for the layer from this rank's rows,
+        storing float32 or, with gather_dtype=torch.bfloat16, BF16 rows.  Building such a table is the point after
+        which every rank's rows are readable by its peers, and its close() the point after which no peer reads them
+        any more; both are collective, and every table is closed before infer returns.  A rank without destinations
+        joins every collective.  Neither the sampler, the step counter, the tape nor any gradient is touched."""
+        from .feature_table import ShardedFeatureTable
+        lo, hi, own, parts = self._own_csc()
+        group = None if self.table is None else self.table.group
+        dtype = self.gather_dtype or torch.float32
+        L = len(self.layers) - 1
+        x = None
+        for l in range(L):
+            k = self.sampler.fanout[L - 1 - l]
+            W = self.P[l].W.detach()
+            narrows = self.layers[l + 1] < self.layers[l]
+            if l == 0 and (narrows or self.table is None):
+                x = self.features[lo:hi] if self.table is None else \
+                    self.table.gather(np.arange(lo, hi), torch.float32)
+            if narrows:
+                src = ShardedFeatureTable(x.mm(W), own, group, dtype=dtype)
+            elif l == 0 and self.table is not None:
+                src = self.table
+            else:
+                src = ShardedFeatureTable(x.contiguous(), own, group, dtype=dtype)
+            y = torch.zeros((hi - lo, src.F), dtype=torch.float32, device=self.device)
+            row0 = 0
+            scale = []
+            for col, rows, w, eb, ee in parts:
+                n = col.numel() - 1
+                src.aggregate(y[row0:row0 + n], col, rows, w, eb, ee)
+                c = col.long() & 0xFFFFFFFF
+                deg = (c[1:] - c[:-1]).double()
+                scale.append(torch.where(deg > k, k / deg.clamp_min(1), torch.ones_like(deg)))
+                row0 += n
+            if src is not self.table:
+                src.close()
+            y.mul_(torch.cat(scale).float().unsqueeze(1))
+            if not narrows:
+                y = y.mm(W)
+            x = torch.relu(y) if l < L - 1 else y
+        return lo, x
+
+    def evaluate_full(self, s):
+        """Accuracy over mask == s from infer(): each rank counts its own rows and the counts are summed over the
+        ranks, so every rank returns the same number."""
+        lo, out = self.infer()
+        ids = self.nids[s].to(self.device)
+        mine = ids[(ids >= lo) & (ids < lo + out.shape[0])]
+        correct = (out.index_select(0, mine - lo).argmax(1) == self.L_GT.index_select(0, mine)).sum()
+        return self._totals(correct)[0] / max(ids.numel(), 1)
+
 
 class GATImpl:
     """Multi-head GAT on the fused aggregation path - the flow of toolkits/GAT_CPU_DIST_OPTM.hpp:196-241 (per-vertex
