@@ -411,6 +411,31 @@ int nts_segment_gather_sum_sharded(float *output, const void *const *shards, int
                                    const float *weight, const nts_vid_t *indices, const nts_vid_t *offsets,
                                    nts_vid_t n_rows, uint64_t edge_begin, uint64_t edge_end, nts_vid_t feature_size,
                                    void *stream);
+/* K10: full-neighbour GAT attention over a sharded table, for the destinations r < n_rows of a CSC piece addressed as
+ * for K9 (offsets[0] == edge_begin, offsets[n_rows] == edge_end, indices by absolute edge position, global ids).  The
+ * sources' scores s[g, h] are FP32 rows of score_pitch values (score_pitch >= heads, % 4 == 0) in score_shards, which
+ * share the row shards' shard_offsets (1..32 ranges), so one shard search per edge serves both; dst_score is the
+ * local [n_rows, heads] d[r, h].  logit(e, h) = leaky_relu(s[indices[e], h] + d[r, h], negative_slope).
+ * nts_gat_softmax_stats_sharded writes seg_max[r, h] = max_e logit and seg_sum[r, h] = sum_e exp(logit - seg_max)
+ * ([n_rows, heads] FP32; empty segments get (0, 1)); heads must divide 32.  n_rows == 0 launches nothing and looks at
+ * no pointer; an empty edge range only writes (0, 1).
+ * nts_gat_aggregate_sharded adds output[r, h*D:(h+1)*D] += sum_e a(e, h) * row(indices[e])[h*D:(h+1)*D], with
+ * a = exp(logit - seg_max) / seg_sum and D = feature_size / heads, rows as for K9 (FP32, or BF16 widened exactly with
+ * FP32 accumulation).  Every 16-byte load must lie inside one head: with heads > 1, D % 4 == 0 (FP32) or D % 8 == 0
+ * (BF16).  output is FP32 [n_rows, feature_size] contiguous, zeroed by the caller.  n_rows == 0, an empty edge range
+ * or feature_size == 0 launches nothing and looks at no pointer.  For both, layout errors return an error and launch
+ * nothing, and edge positions must fit uint32. */
+int nts_gat_softmax_stats_sharded(float *seg_max, float *seg_sum, const void *const *score_shards,
+                                  const nts_vid_t *shard_offsets, int n_shards, nts_vid_t score_pitch,
+                                  const float *dst_score, const nts_vid_t *indices, const nts_vid_t *offsets,
+                                  nts_vid_t n_rows, uint64_t edge_begin, uint64_t edge_end, nts_vid_t heads,
+                                  float negative_slope, void *stream);
+int nts_gat_aggregate_sharded(float *output, const void *const *shards, int shard_dtype,
+                              const nts_vid_t *shard_offsets, int n_shards, nts_vid_t shard_pitch,
+                              const void *const *score_shards, nts_vid_t score_pitch, const float *dst_score,
+                              const float *seg_max, const float *seg_sum, const nts_vid_t *indices,
+                              const nts_vid_t *offsets, nts_vid_t n_rows, uint64_t edge_begin, uint64_t edge_end,
+                              nts_vid_t feature_size, nts_vid_t heads, float negative_slope, void *stream);
 /* dst[rows[k],:] += src[k,:]  (receiver-side add of partial gradients; rows must be unique) */
 int nts_scatter_add_rows(float *dst, const float *src, const nts_vid_t *rows, nts_vid_t n_rows,
                          nts_vid_t feature_size, void *stream);

@@ -52,6 +52,10 @@ SIGNATURES = {
     "nts_segment_gather_sum_bf16": (_int, [_vp, _u32, _vp, _vp, _vp, _vp, _u32, _u64, _u32, _vp]),
     "nts_segment_gather_sum_sharded": (_int, [_vp, _vp, _int, _vp, _int, _u32, _vp, _vp, _vp, _u32, _u64, _u64, _u32,
                                               _vp]),
+    "nts_gat_softmax_stats_sharded": (_int, [_vp, _vp, _vp, _vp, _int, _u32, _vp, _vp, _vp, _u32, _u64, _u64, _u32,
+                                             C.c_float, _vp]),
+    "nts_gat_aggregate_sharded": (_int, [_vp, _vp, _int, _vp, _int, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _u32,
+                                         _u64, _u64, _u32, _u32, C.c_float, _vp]),
     "nts_gather_plan_pick_slabs": (_int, [_u32, _u64, _u32, _u32, _u64]),
     "nts_gather_plan_create_hybrid": (_vp, [_vp, _vp, _vp, _vp, _u32, _u32, _u64, _u32, _int, _int, _int, _vp]),
     "nts_gather_plan_create_parts": (_vp, [_vp, _int, _u32, _u32, _int, _u32, _vp]),

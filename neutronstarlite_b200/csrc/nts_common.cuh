@@ -100,6 +100,18 @@ __device__ __forceinline__ float4 widen(uint2 u) {
 }
 __device__ __forceinline__ float8v widen(uint4 u) { return {widen(make_uint2(u.x, u.y)), widen(make_uint2(u.z, u.w))}; }
 
+// GAT attention logits (K7, K10): leaky_relu, and the segment maximum merged with one atomic
+__device__ __forceinline__ float leaky(float x, float slope) { return x > 0.f ? x : x * slope; }
+__device__ __forceinline__ void atomic_max_float(float *addr, float v) {
+  // IEEE-754 order trick: non-negative floats order like signed ints, negative floats inversely like unsigned ints;
+  // one `red` instead of a CAS loop (v + 0.f turns -0.0 into +0.0, NaN never reaches here)
+  v += 0.f;
+  if (v >= 0.f)
+    atomicMax(reinterpret_cast<int *>(addr), __float_as_int(v));
+  else
+    atomicMin(reinterpret_cast<unsigned int *>(addr), __float_as_uint(v));
+}
+
 // A plan of parts (checked by the caller) with its slab count, and with hubs_allowed (a single part) its hub counts
 // and schedule, chosen by timing candidates for width feature_size in run mode run_flags (0 or NTS_PLAN_OVERWRITE),
 // as FP32 gathers or, with bf16, as BF16 gathers of BF16 rows (nts_plan.cu)

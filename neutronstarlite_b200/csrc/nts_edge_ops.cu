@@ -492,7 +492,6 @@ __global__ void __launch_bounds__(kThreads)
 // ---- fully fused GAT layer (K7): attention logits are never materialised ------------------------------------------
 //   logit[e,h] = leaky_relu(s[slot(e),h] + d[dst(e),h]);  a = softmax over the destination segment
 // stats kernel: seg_max[d,h], seg_sum[d,h] (sum of exp(logit - max)); empty segments get (0, 1).
-__device__ __forceinline__ float leaky(float x, float slope) { return x > 0.f ? x : x * slope; }
 
 __global__ void __launch_bounds__(kThreads)
     gat_softmax_stats_kernel(float *__restrict__ seg_max, float *__restrict__ seg_sum, const float *__restrict__ s_att,
@@ -538,16 +537,6 @@ __global__ void __launch_bounds__(kThreads)
       }
     }
   }
-}
-
-__device__ __forceinline__ void atomic_max_float(float *addr, float v) {
-  // IEEE-754 order trick: non-negative floats order like signed ints, negative floats inversely like unsigned ints;
-  // one `red` instead of a CAS loop (v + 0.f turns -0.0 into +0.0, NaN never reaches here)
-  v += 0.f;
-  if (v >= 0.f)
-    atomicMax(reinterpret_cast<int *>(addr), __float_as_int(v));
-  else
-    atomicMin(reinterpret_cast<unsigned int *>(addr), __float_as_uint(v));
 }
 
 // Edge-balanced statistics (H divides 32): a warp owns a quantum of consecutive EDGES whatever rows they belong to,

@@ -34,6 +34,21 @@ def _group_rank_world(group):
     return dist.get_rank(group), dist.get_world_size(group)
 
 
+def gat_shape_error(F, heads, dtype=torch.float32):
+    """Why K10 (ShardedFeatureTable.gat_aggregate) refuses rows of width F in `heads` heads of dtype, or None: heads
+    must divide 32 (the statistics' lanes are (edge, head) pairs) and F, and with heads > 1 a head must be a whole
+    number of 16-byte loads (4 FP32 or 8 BF16 values)."""
+    if heads < 1 or 32 % heads:
+        return "%d heads: the head count must divide 32" % heads
+    if F % heads:
+        return "width %d is not a multiple of %d heads" % (F, heads)
+    vec = 8 if dtype == torch.bfloat16 else 4
+    if heads > 1 and (F // heads) % vec:
+        return "%d heads of width %d: with more than one head, a head must be a multiple of %d %s values" % (
+            heads, F // heads, vec, "BF16" if vec == 8 else "FP32")
+    return None
+
+
 class PeerShards:
     """One device buffer per rank of a process group (nts_malloc_device: a CUDA-IPC handle names the whole
     allocation), mapped by every other rank.  The lifecycle ShardedFeatureTable and topology.ShardedTopology share:
@@ -185,6 +200,18 @@ class ShardedFeatureTable(PeerShards):
         wrong kind raise NtsError before any device work."""
         if self._buf is None:
             raise _lib.NtsError("the feature table is closed")
+        if not self._check_csc(out, column_offset, row_indices, weight, edge_begin, edge_end):
+            return out
+        n_rows, eb, ee = int(out.shape[0]), int(edge_begin), int(edge_end)
+        _lib.call("nts_segment_gather_sum_sharded", out.data_ptr(), self._shards.data_ptr(),
+                  1 if self.dtype == torch.bfloat16 else 0, self._offsets.data_ptr(), self.world, self.pitch,
+                  None if weight is None else weight.data_ptr(), row_indices.data_ptr(), column_offset.data_ptr(),
+                  n_rows, eb, ee, self.F, _stream())
+        return out
+
+    def _check_csc(self, out, column_offset, row_indices, weight, edge_begin, edge_end):
+        """NtsError for operands of aggregate() / gat_aggregate() of the wrong kind; False when there is nothing to
+        add (no rows or no edges)."""
         for name, t, dt in (("out", out, torch.float32), ("column_offset", column_offset, torch.int32),
                             ("row_indices", row_indices, torch.int32), ("weight", weight, torch.float32)):
             if t is None and name == "weight":
@@ -200,12 +227,53 @@ class ShardedFeatureTable(PeerShards):
                 (weight is not None and weight.numel() < ee):
             raise _lib.NtsError("column_offset needs %d entries and [edge_begin, edge_end) = [%d, %d) must lie in the "
                                 "%d edges of row_indices and weight" % (n_rows + 1, eb, ee, row_indices.numel()))
-        if n_rows == 0 or eb == ee:
+        return n_rows > 0 and eb < ee
+
+    def gat_aggregate(self, out, scores, dst_score, column_offset, row_indices, edge_begin, edge_end, heads,
+                      negative_slope=0.2):
+        """Full-neighbour GAT attention over the table (K10: nts_gat_softmax_stats_sharded, then
+        nts_gat_aggregate_sharded), for the destinations r < out.shape[0] of a CSC slice given as for aggregate():
+
+            logit(e, h) = leaky_relu(s[src(e), h] + dst_score[r, h], negative_slope)
+            out[r, h*D:(h+1)*D] += sum_e softmax_e(logit(., h)) * row src(e)[h*D:(h+1)*D]      D = F / heads
+
+        over the edges e in [column_offset[r], column_offset[r+1]).  `scores` is a float32 ShardedFeatureTable of [V,
+        heads] source scores over the same group and offsets: a source's row and scores are read by global id, local
+        or peer memory, with one shard search per edge.  dst_score: float32 CUDA [n_rows, heads] contiguous.  BF16 rows
+        are widened exactly and summed in FP32; scores and statistics are FP32.  Allocates the [n_rows, heads]
+        statistics and runs both entries asynchronously on the current stream.  A closed table, a score table of
+        another kind, heads that do not divide 32 or split a 16-byte load (gat_shape_error), and the operand errors of
+        aggregate() raise NtsError before any device work."""
+        heads = int(heads)
+        if not isinstance(scores, ShardedFeatureTable) or scores.dtype != torch.float32 or scores.F != heads:
+            raise _lib.NtsError("scores must be a float32 ShardedFeatureTable of %d columns" % heads)
+        if self._buf is None or scores._buf is None:
+            raise _lib.NtsError("the feature table is closed")
+        why = gat_shape_error(self.F, heads, self.dtype)
+        if why is not None:
+            raise _lib.NtsError(why)
+        if scores.world != self.world or scores.rank != self.rank or scores.device != self.device or \
+                not np.array_equal(scores.offsets, self.offsets):
+            raise _lib.NtsError("scores must span the same ranks and offsets as the table")
+        n_rows = int(out.shape[0]) if torch.is_tensor(out) and out.dim() == 2 else -1
+        if not torch.is_tensor(dst_score) or dst_score.dim() != 2 or tuple(dst_score.shape) != (n_rows, heads) or \
+                not dst_score.is_cuda or dst_score.dtype != torch.float32 or dst_score.device != self.device or \
+                not dst_score.is_contiguous():
+            raise _lib.NtsError("dst_score must be a contiguous float32 [%d, %d] tensor on %s"
+                                % (max(n_rows, 0), heads, self.device))
+        if not self._check_csc(out, column_offset, row_indices, None, edge_begin, edge_end):
             return out
-        _lib.call("nts_segment_gather_sum_sharded", out.data_ptr(), self._shards.data_ptr(),
+        eb, ee = int(edge_begin), int(edge_end)
+        seg = torch.empty((2, n_rows, heads), dtype=torch.float32, device=self.device)
+        st = _stream()
+        _lib.call("nts_gat_softmax_stats_sharded", seg[0].data_ptr(), seg[1].data_ptr(), scores._shards.data_ptr(),
+                  self._offsets.data_ptr(), self.world, scores.pitch, dst_score.data_ptr(), row_indices.data_ptr(),
+                  column_offset.data_ptr(), n_rows, eb, ee, heads, float(negative_slope), st)
+        _lib.call("nts_gat_aggregate_sharded", out.data_ptr(), self._shards.data_ptr(),
                   1 if self.dtype == torch.bfloat16 else 0, self._offsets.data_ptr(), self.world, self.pitch,
-                  None if weight is None else weight.data_ptr(), row_indices.data_ptr(), column_offset.data_ptr(),
-                  n_rows, eb, ee, self.F, _stream())
+                  scores._shards.data_ptr(), scores.pitch, dst_score.data_ptr(), seg[0].data_ptr(),
+                  seg[1].data_ptr(), row_indices.data_ptr(), column_offset.data_ptr(), n_rows, eb, ee, self.F, heads,
+                  float(negative_slope), st)
         return out
 
     def _out_dtype(self, dtype):

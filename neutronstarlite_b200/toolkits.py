@@ -347,6 +347,50 @@ class _SampledRounds:
         self.ctx.train()
         return self._totals(correct)[0] / max(ids.numel(), 1)
 
+    def _own_csc(self):
+        """(lo, hi, own_offsets, parts): this rank's destinations [lo, hi), the ownership offsets the per-layer tables
+        are built on, and the in-edge CSC pieces that cover [lo, hi) in order, as (column offsets [n + 1] int32,
+        row_indices, weight, edge_begin, edge_end) - a ShardedTopology's shards held in this process (all of them
+        after split()), or the slice [lo, hi) of the replicated single-partition CSC."""
+        from .sample import _DeviceArray
+        from .topology import ShardedTopology
+        topo = self.sampler._graph
+        dev = self.device
+
+        def borrowed(ptr, n, typestr):
+            if n == 0:
+                return torch.empty(0, dtype=torch.float32 if typestr == "<f4" else torch.int32, device=dev)
+            return torch.as_tensor(_DeviceArray(ptr, n, typestr), device=dev)
+
+        if isinstance(topo, ShardedTopology):
+            if topo._buf is None:
+                raise _lib.NtsError("the topology is closed")
+            off = [int(o) for o in topo.offsets]
+            mine = range(len(off) - 1) if topo.world == 1 else [topo.rank]
+            parts = []
+            for o in mine:
+                col = borrowed(topo.shard_arrays[0][o], off[o + 1] - off[o] + 1, "<i4")
+                n_edges = int(col[-1])
+                parts.append((col, borrowed(topo.shard_arrays[1][o], n_edges, "<i4"),
+                              borrowed(topo.shard_arrays[2][o], n_edges, "<f4"), 0, n_edges))
+            lo, hi = off[mine[0]], off[mine[-1] + 1]
+            return lo, hi, (off if topo.world > 1 else [0, off[-1]]), parts
+        c_col, c_row, c_w = topo
+        own = [0, self.sampler.V] if self.table is None else [int(o) for o in self.table.offsets]
+        lo, hi = own[self.rank], own[self.rank + 1]
+        col = c_col[lo:hi + 1]
+        eb, ee = (int(e) & 0xFFFFFFFF for e in col[[0, -1]].tolist())
+        return lo, hi, own, [(col, c_row, c_w, eb, ee)]
+
+    def evaluate_full(self, s):
+        """Accuracy over mask == s from the model's infer(): each rank counts its own rows and the counts are summed
+        over the ranks, so every rank returns the same number."""
+        lo, out = self.infer()
+        ids = self.nids[s].to(self.device)
+        mine = ids[(ids >= lo) & (ids < lo + out.shape[0])]
+        correct = (out.index_select(0, mine - lo).argmax(1) == self.L_GT.index_select(0, mine)).sum()
+        return self._totals(correct)[0] / max(ids.numel(), 1)
+
     def run_epoch(self, test=True):
         """One pass over the train batches (one Adam step per round) and, with test=True, sampled validation and test
         forwards.  Returns (mean train loss, [train, val, test] accuracy) - val / test are None with test=False."""
@@ -483,41 +527,6 @@ class GCNSampleImpl(_SampledRounds):
         self.Update()
         return loss.detach(), correct
 
-    def _own_csc(self):
-        """(lo, hi, own_offsets, parts): this rank's destinations [lo, hi), the ownership offsets the per-layer tables
-        are built on, and the in-edge CSC pieces that cover [lo, hi) in order, as (column offsets [n + 1] int32,
-        row_indices, weight, edge_begin, edge_end) - a ShardedTopology's shards held in this process (all of them
-        after split()), or the slice [lo, hi) of the replicated single-partition CSC."""
-        from .sample import _DeviceArray
-        from .topology import ShardedTopology
-        topo = self.sampler._graph
-        dev = self.device
-
-        def borrowed(ptr, n, typestr):
-            if n == 0:
-                return torch.empty(0, dtype=torch.float32 if typestr == "<f4" else torch.int32, device=dev)
-            return torch.as_tensor(_DeviceArray(ptr, n, typestr), device=dev)
-
-        if isinstance(topo, ShardedTopology):
-            if topo._buf is None:
-                raise _lib.NtsError("the topology is closed")
-            off = [int(o) for o in topo.offsets]
-            mine = range(len(off) - 1) if topo.world == 1 else [topo.rank]
-            parts = []
-            for o in mine:
-                col = borrowed(topo.shard_arrays[0][o], off[o + 1] - off[o] + 1, "<i4")
-                n_edges = int(col[-1])
-                parts.append((col, borrowed(topo.shard_arrays[1][o], n_edges, "<i4"),
-                              borrowed(topo.shard_arrays[2][o], n_edges, "<f4"), 0, n_edges))
-            lo, hi = off[mine[0]], off[mine[-1] + 1]
-            return lo, hi, (off if topo.world > 1 else [0, off[-1]]), parts
-        c_col, c_row, c_w = topo
-        own = [0, self.sampler.V] if self.table is None else [int(o) for o in self.table.offsets]
-        lo, hi = own[self.rank], own[self.rank + 1]
-        col = c_col[lo:hi + 1]
-        eb, ee = (int(e) & 0xFFFFFFFF for e in col[[0, -1]].tolist())
-        return lo, hi, own, [(col, c_row, c_w, eb, ee)]
-
     @torch.no_grad()
     def infer(self):
         """Full-neighbour inference: collective over the ranks of the model's table.  Returns (lo, out), out the last
@@ -571,15 +580,6 @@ class GCNSampleImpl(_SampledRounds):
                 y = y.mm(W)
             x = torch.relu(y) if l < L - 1 else y
         return lo, x
-
-    def evaluate_full(self, s):
-        """Accuracy over mask == s from infer(): each rank counts its own rows and the counts are summed over the
-        ranks, so every rank returns the same number."""
-        lo, out = self.infer()
-        ids = self.nids[s].to(self.device)
-        mine = ids[(ids >= lo) & (ids < lo + out.shape[0])]
-        correct = (out.index_select(0, mine - lo).argmax(1) == self.L_GT.index_select(0, mine)).sum()
-        return self._totals(correct)[0] / max(ids.numel(), 1)
 
 
 class GATImpl:
@@ -809,6 +809,57 @@ class GATSampleImpl(_SampledRounds):
             else:
                 x = ctx.runVertexForward(lambda t: torch.relu(t), nbr)
         return x
+
+    @torch.no_grad()
+    def infer(self):
+        """Full-neighbour inference: collective over the ranks of the model's table.  Returns (lo, out), out the last
+        layer's [hi - lo, classes] float32 log-probabilities (as Forward returns them) for the destinations [lo, hi)
+        this rank owns: a ShardedTopology's, else the table's offsets, else [0, V).
+
+        Layer l attends over every in-edge slot of each destination (a multi-edge counts once per slot, as the sampler
+        counts it; edge weights are ignored, as in MiniBatchGATOp):  T = X_own W_l, s = <T, al_l>, d = <T, ar_l> per
+        head, a[e, h] = softmax over the in-edge slots e of v of leaky_relu(s[src(e), h] + d[v, h], 0.2), Y[v, h] =
+        sum_e a[e, h] T[src(e), h] (zero at in-degree 0), X_{l+1} = relu(Y), or log_softmax(Y) on the last layer; no
+        dropout.  With every fanout >= the largest in-degree the sampled layer keeps every slot, so this is exactly
+        Forward over all vertices and the full-graph GATImpl.  Unlike GCNSampleImpl.infer, there is no expectation to
+        scale by: the sampled layer renormalises its softmax over the kept slots, a ratio estimator of this full
+        softmax with no closed-form mean, and the full softmax is what it tends to as the fanouts grow.
+
+        Every layer builds two ShardedFeatureTables from this rank's rows, T (float32, or BF16 with
+        gather_dtype=torch.bfloat16; scores always come from the float32 T) and the float32 scores s, and aggregates
+        each in-edge piece of [lo, hi) with ShardedFeatureTable.gat_aggregate (K10).  Building the tables is the point
+        after which every rank's rows are readable by its peers, and their close() the point after which no peer
+        reads them any more; both are collective.  A rank without destinations joins every collective.  A layer shape
+        K10 refuses (feature_table.gat_shape_error) raises NtsError before the first collective, on every rank alike.
+        Neither the sampler, the step counter, the tape nor any gradient is touched."""
+        from .feature_table import ShardedFeatureTable, gat_shape_error
+        dtype = self.gather_dtype or torch.float32
+        for l, H in enumerate(self.heads):
+            why = gat_shape_error(self.layers[l + 1], H, dtype)
+            if why is not None:
+                raise _lib.NtsError("layer %d cannot run full-neighbour inference: %s" % (l, why))
+        lo, hi, own, parts = self._own_csc()
+        group = None if self.table is None else self.table.group
+        x = self.features[lo:hi] if self.table is None else self.table.gather(np.arange(lo, hi), torch.float32)
+        L = len(self.layers) - 1
+        for l in range(L):
+            H = self.heads[l]
+            D = self.layers[l + 1] // H
+            t = x.mm(self.P[l].W.detach())
+            s = (t.view(-1, H, D) * self.al[l].W.detach()).sum(-1).contiguous()
+            d = (t.view(-1, H, D) * self.ar[l].W.detach()).sum(-1).contiguous()
+            rows = ShardedFeatureTable(t, own, group, dtype=dtype)
+            scores = ShardedFeatureTable(s, own, group)
+            y = torch.zeros((hi - lo, H * D), dtype=torch.float32, device=self.device)
+            row0 = 0
+            for col, ids, _, eb, ee in parts:
+                n = col.numel() - 1
+                rows.gat_aggregate(y[row0:row0 + n], scores, d[row0:row0 + n], col, ids, eb, ee, H)
+                row0 += n
+            rows.close()
+            scores.close()
+            x = torch.relu(y) if l < L - 1 else y.log_softmax(1)
+        return lo, x
 
     def Loss(self, out, seeds_dev):
         self.loss = torch.nn.functional.nll_loss(out, self.L_GT.index_select(0, seeds_dev))
