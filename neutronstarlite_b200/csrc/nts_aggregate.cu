@@ -40,140 +40,6 @@ static int g_edges_per_warp = 0;   // 0 = auto
 static int g_last_grid = 0, g_last_block = 0, g_last_smem = 0, g_last_variant = 0;
 static int g_last_vec = 0, g_last_k = 0, g_last_u = 0, g_last_minb = 0, g_last_tiles = 0; // instantiation of the last launch
 
-// ---- small device helpers --------------------------------------------------------------------------------
-__device__ __forceinline__ void fma_vec(float &a, float w, float x) { a = fmaf(w, x, a); }
-__device__ __forceinline__ void fma_vec(float2 &a, float w, float2 x) {
-  a.x = fmaf(w, x.x, a.x);
-  a.y = fmaf(w, x.y, a.y);
-}
-__device__ __forceinline__ void fma_vec(float4 &a, float w, float4 x) {
-  a.x = fmaf(w, x.x, a.x);
-  a.y = fmaf(w, x.y, a.y);
-  a.z = fmaf(w, x.z, a.z);
-  a.w = fmaf(w, x.w, a.w);
-}
-__device__ __forceinline__ void fma_vec(float8v &a, float w, float8v x) {
-  fma_vec(a.lo, w, x.lo);
-  fma_vec(a.hi, w, x.hi);
-}
-__device__ __forceinline__ void zero_vec(float &a) { a = 0.f; }
-__device__ __forceinline__ void zero_vec(float2 &a) { a = make_float2(0.f, 0.f); }
-__device__ __forceinline__ void zero_vec(float4 &a) { a = make_float4(0.f, 0.f, 0.f, 0.f); }
-__device__ __forceinline__ void zero_vec(float8v &a) {
-  zero_vec(a.lo);
-  zero_vec(a.hi);
-}
-
-__device__ __forceinline__ void rmw_add(float *p, float a) { *p = *p + a; }
-__device__ __forceinline__ void rmw_add(float2 *p, float2 a) {
-  float2 o = *p;
-  o.x += a.x;
-  o.y += a.y;
-  *p = o;
-}
-__device__ __forceinline__ void rmw_add(float4 *p, float4 a) {
-  float4 o = *p;
-  o.x += a.x;
-  o.y += a.y;
-  o.z += a.z;
-  o.w += a.w;
-  *p = o;
-}
-__device__ __forceinline__ void rmw_add(float8v *p, float8v a) {
-  rmw_add(&p->lo, a.lo);
-  rmw_add(&p->hi, a.hi);
-}
-// no-return vector reductions (sm_90+): one L2 atomic transaction per 8/16 bytes
-__device__ __forceinline__ void red_add(float *p, float a) { atomicAdd(p, a); }
-__device__ __forceinline__ void red_add(float2 *p, float2 a) {
-  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a.x), "f"(a.y) : "memory");
-}
-__device__ __forceinline__ void red_add(float4 *p, float4 a) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a.x), "f"(a.y), "f"(a.z), "f"(a.w)
-               : "memory");
-}
-__device__ __forceinline__ void red_add(float8v *p, float8v a) {
-  red_add(&p->lo, a.lo);
-  red_add(&p->hi, a.hi);
-}
-
-// o[col .. col+7] (+)= a for the columns < Fo of a row of Fo floats (K1 on BF16 rows: the output's width need not be a
-// multiple of the 8-value chunk).  Whole chunks go as 16- or 8-byte vectors when Fo and the row allow them.
-__device__ __forceinline__ void flush_cols(float *o, uint32_t col, uint32_t Fo, const float8v &a, bool whole) {
-  const float v[8] = {a.lo.x, a.lo.y, a.lo.z, a.lo.w, a.hi.x, a.hi.y, a.hi.z, a.hi.w};
-  const uintptr_t align = reinterpret_cast<uintptr_t>(o);
-  if ((Fo & 3u) == 0 && (align & 15u) == 0) { // col and Fo multiples of 4: whole float4s
-#pragma unroll
-    for (int i = 0; i < 8; i += 4)
-      if (col + i < Fo) {
-        const float4 x = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-        if (whole)
-          rmw_add(reinterpret_cast<float4 *>(o + col + i), x);
-        else
-          red_add(reinterpret_cast<float4 *>(o + col + i), x);
-      }
-  } else if ((Fo & 1u) == 0 && (align & 7u) == 0) {
-#pragma unroll
-    for (int i = 0; i < 8; i += 2)
-      if (col + i < Fo) {
-        const float2 x = make_float2(v[i], v[i + 1]);
-        if (whole)
-          rmw_add(reinterpret_cast<float2 *>(o + col + i), x);
-        else
-          red_add(reinterpret_cast<float2 *>(o + col + i), x);
-      }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 8; i++)
-      if (col + i < Fo) {
-        if (whole)
-          rmw_add(o + col + i, v[i]);
-        else
-          red_add(o + col + i, v[i]);
-      }
-  }
-}
-
-// largest r in [0, n_rows) with off[r] <= e  (requires off[0] <= e < off[n_rows])
-__device__ __forceinline__ uint32_t find_row(const uint32_t *__restrict__ off, uint32_t n_rows, uint32_t e) {
-  uint32_t lo = 0, hi = n_rows; // invariant: off[lo] <= e < off[hi]
-  while (hi - lo > 1) {
-    uint32_t mid = lo + ((hi - lo) >> 1);
-    if (__ldg(off + mid) <= e)
-      lo = mid;
-    else
-      hi = mid;
-  }
-  return lo;
-}
-
-// mbarrier / bulk-copy PTX (variant 2)
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-  asm volatile("{\n\t"
-               ".reg .pred p;\n\t"
-               "WAIT_%=:\n\t"
-               "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-               "@p bra DONE_%=;\n\t"
-               "bra WAIT_%=;\n\t"
-               "DONE_%=:\n\t"
-               "}" ::"r"(smem_u32(bar)),
-               "r"(parity)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gmem_src, uint32_t bytes, uint64_t *bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(smem_dst)),
-               "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-
 constexpr int kWarpsPerBlock = 8;
 
 // Fused GAT attention (K7): instead of loading a per-edge weight, recompute it from per-vertex scores
@@ -187,9 +53,7 @@ struct AttParams {
   float slope;    // leaky_relu negative slope
 };
 __device__ __forceinline__ float att_weight(float s, float d, float m, float inv_z, float slope) {
-  float x = s + d;
-  x = x > 0.f ? x : x * slope;
-  return expf(x - m) * inv_z;
+  return expf(leaky(s + d, slope) - m) * inv_z;
 }
 
 // ---- the kernel --------------------------------------------------------------------------------------------
@@ -482,14 +346,7 @@ struct LaunchShape {
 static LaunchShape pick_shape(const float *in, const float *out, uint32_t F, uint32_t heads) {
   LaunchShape s;
   s.heads = heads ? heads : 1;
-  bool a16 = aligned_to(in, 16) && aligned_to(out, 16);
-  bool a8 = aligned_to(in, 8) && aligned_to(out, 8);
-  if (F % 4 == 0 && a16)
-    s.vec = 4;
-  else if (F % 2 == 0 && a8)
-    s.vec = 2;
-  else
-    s.vec = 1;
+  s.vec = pick_vec(F, in, out);
   if (heads > 1) // a head's columns must be a whole number of vectors
     while (s.vec > 1 && (F / heads) % s.vec != 0)
       s.vec >>= 1;

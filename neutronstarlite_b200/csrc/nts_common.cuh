@@ -51,6 +51,16 @@ inline cudaStream_t as_stream(void *s) { return reinterpret_cast<cudaStream_t>(s
 
 inline bool aligned_to(const void *p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 
+// The widest vector (4, 2 or 1 floats) that rows of F floats allow at every one of the pointers (a null one counts as
+// aligned).  The width for several pointers is the minimum of their single widths.
+template <class... P> inline int pick_vec(uint32_t F, const P *...p) {
+  if (F % 4 == 0 && (aligned_to(p, 16) && ...))
+    return 4;
+  if (F % 2 == 0 && (aligned_to(p, 8) && ...))
+    return 2;
+  return 1;
+}
+
 int sm_count();
 
 // Minimum of two timed run() calls after one warm-up call, with CUDA events on st (synchronises).  Returns run()'s
@@ -81,6 +91,62 @@ template <> struct Vec<2> { using type = float2; };
 template <> struct Vec<4> { using type = float4; };
 template <> struct Vec<8> { using type = float8v; };
 
+// Arithmetic on the Vec<VEC> types: a = 0, a += w * x, *p += a (plain read-modify-write) and *p += a as no-return
+// vector reductions (sm_90+: one L2 atomic transaction per 8 / 16 bytes)
+__device__ __forceinline__ void zero_vec(float &a) { a = 0.f; }
+__device__ __forceinline__ void zero_vec(float2 &a) { a = make_float2(0.f, 0.f); }
+__device__ __forceinline__ void zero_vec(float4 &a) { a = make_float4(0.f, 0.f, 0.f, 0.f); }
+__device__ __forceinline__ void zero_vec(float8v &a) {
+  zero_vec(a.lo);
+  zero_vec(a.hi);
+}
+__device__ __forceinline__ void fma_vec(float &a, float w, float x) { a = fmaf(w, x, a); }
+__device__ __forceinline__ void fma_vec(float2 &a, float w, float2 x) {
+  a.x = fmaf(w, x.x, a.x);
+  a.y = fmaf(w, x.y, a.y);
+}
+__device__ __forceinline__ void fma_vec(float4 &a, float w, float4 x) {
+  a.x = fmaf(w, x.x, a.x);
+  a.y = fmaf(w, x.y, a.y);
+  a.z = fmaf(w, x.z, a.z);
+  a.w = fmaf(w, x.w, a.w);
+}
+__device__ __forceinline__ void fma_vec(float8v &a, float w, float8v x) {
+  fma_vec(a.lo, w, x.lo);
+  fma_vec(a.hi, w, x.hi);
+}
+__device__ __forceinline__ void rmw_add(float *p, float a) { *p = *p + a; }
+__device__ __forceinline__ void rmw_add(float2 *p, float2 a) {
+  float2 o = *p;
+  o.x += a.x;
+  o.y += a.y;
+  *p = o;
+}
+__device__ __forceinline__ void rmw_add(float4 *p, float4 a) {
+  float4 o = *p;
+  o.x += a.x;
+  o.y += a.y;
+  o.z += a.z;
+  o.w += a.w;
+  *p = o;
+}
+__device__ __forceinline__ void rmw_add(float8v *p, float8v a) {
+  rmw_add(&p->lo, a.lo);
+  rmw_add(&p->hi, a.hi);
+}
+__device__ __forceinline__ void red_add(float *p, float a) { atomicAdd(p, a); }
+__device__ __forceinline__ void red_add(float2 *p, float2 a) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a.x), "f"(a.y) : "memory");
+}
+__device__ __forceinline__ void red_add(float4 *p, float4 a) {
+  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a.x), "f"(a.y), "f"(a.z), "f"(a.w)
+               : "memory");
+}
+__device__ __forceinline__ void red_add(float8v *p, float8v a) {
+  red_add(&p->lo, a.lo);
+  red_add(&p->hi, a.hi);
+}
+
 // What one lane loads for VEC values of a row of element type T, and widen(), which turns it into the FP32 vector
 // Vec<VEC>.  A BF16 value is the upper half of the FP32 with the same bits, so widening is exact (one shift or mask);
 // for FP32 rows both are the identity.
@@ -110,6 +176,149 @@ __device__ __forceinline__ void atomic_max_float(float *addr, float v) {
     atomicMax(reinterpret_cast<int *>(addr), __float_as_int(v));
   else
     atomicMin(reinterpret_cast<unsigned int *>(addr), __float_as_uint(v));
+}
+
+// Segment search: the largest r in [0, n_rows) with off[r] <= e  (requires off[0] <= e < off[n_rows])
+__device__ __forceinline__ uint32_t find_row(const uint32_t *__restrict__ off, uint32_t n_rows, uint32_t e) {
+  uint32_t lo = 0, hi = n_rows; // invariant: off[lo] <= e < off[hi]
+  while (hi - lo > 1) {
+    const uint32_t mid = lo + ((hi - lo) >> 1);
+    if (__ldg(off + mid) <= e)
+      lo = mid;
+    else
+      hi = mid;
+  }
+  return lo;
+}
+
+// Tables sharded by global row ranges: shard o holds the ids [off[o], off[o+1]) of up to kMaxShards shards.
+constexpr int kMaxShards = 32;
+
+// The table's n_shards + 1 offsets and n_shards shard pointers staged in shared memory by the whole block; also(i)
+// stages entry i of tables that share the offsets.
+template <class P, class Also>
+__device__ __forceinline__ void stage_shard_table(uint32_t *s_off, const P **s_shard, const uint32_t *__restrict__ off,
+                                             const P *const *__restrict__ shards, int n_shards, Also also) {
+  for (int i = threadIdx.x; i <= n_shards; i += blockDim.x) {
+    s_off[i] = __ldg(off + i);
+    if (i < n_shards) {
+      s_shard[i] = shards[i];
+      also(i);
+    }
+  }
+  __syncthreads();
+}
+template <class P>
+__device__ __forceinline__ void stage_shard_table(uint32_t *s_off, const P **s_shard, const uint32_t *__restrict__ off,
+                                             const P *const *__restrict__ shards, int n_shards) {
+  stage_shard_table(s_off, s_shard, off, shards, n_shards, [](int) {});
+}
+
+// The owner of id: the last shard o with s_off[o] <= id, so an empty shard (s_off[o] == s_off[o+1]) is never chosen
+__device__ __forceinline__ int find_shard(const uint32_t *s_off, int n_shards, uint32_t id) {
+  int lo = 0, hi = n_shards;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (s_off[mid] <= id)
+      lo = mid;
+    else
+      hi = mid;
+  }
+  return lo;
+}
+
+// mbarrier / bulk-copy (TMA, SASS UBLKCP) PTX: global -> shared copies whose completion is counted on an mbarrier
+__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+}
+__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
+  asm volatile("{\n\t"
+               ".reg .pred p;\n\t"
+               "WAIT_%=:\n\t"
+               "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+               "@p bra DONE_%=;\n\t"
+               "bra WAIT_%=;\n\t"
+               "DONE_%=:\n\t"
+               "}" ::"r"(smem_u32(bar)),
+               "r"(parity)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gmem_src, uint32_t bytes, uint64_t *bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                   smem_u32(smem_dst)),
+               "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+
+// The columns col .. col+3 (col < F) of a chunk that are < F, written into a row of an FP32 output of row stride F
+// with stores of VEC floats (the output's rows are 16-byte aligned only when F % 4 == 0).  store_chunk_checked also
+// checks the first column: the two forms compile differently unless the caller's own col < F check is visible.
+template <int VEC> __device__ __forceinline__ void store_chunk(float *o, uint32_t col, uint32_t F, float4 a) {
+  if constexpr (VEC == 4) {
+    *reinterpret_cast<float4 *>(o + col) = a;
+  } else if constexpr (VEC == 2) {
+    *reinterpret_cast<float2 *>(o + col) = make_float2(a.x, a.y);
+    if (col + 2 < F)
+      *reinterpret_cast<float2 *>(o + col + 2) = make_float2(a.z, a.w);
+  } else {
+    o[col] = a.x;
+    if (col + 1 < F)
+      o[col + 1] = a.y;
+    if (col + 2 < F)
+      o[col + 2] = a.z;
+    if (col + 3 < F)
+      o[col + 3] = a.w;
+  }
+}
+template <int VEC>
+__device__ __forceinline__ void store_chunk_checked(float *__restrict__ o, uint32_t col, uint32_t F, float4 a) {
+  if constexpr (VEC == 4) {
+    *reinterpret_cast<float4 *>(o + col) = a;
+  } else if constexpr (VEC == 2) {
+    float2 *p = reinterpret_cast<float2 *>(o + col);
+    p[0] = make_float2(a.x, a.y);
+    if (col + 2 < F)
+      p[1] = make_float2(a.z, a.w);
+  } else {
+    const float v[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+      if (col + i < F)
+        o[col + i] = v[i];
+  }
+}
+// *p += a: a plain read-modify-write when `whole` (the caller is the only writer), else a reduction
+template <class V> __device__ __forceinline__ void add_vec(V *p, V a, bool whole) {
+  if (whole)
+    rmw_add(p, a);
+  else
+    red_add(p, a);
+}
+// o[col .. col+7] (+)= a for the columns < Fo of a row of Fo floats (K1 on BF16 rows: the output's width need not be a
+// multiple of the 8-value chunk).  Whole chunks go as 16- or 8-byte vectors when Fo and the row allow them.
+__device__ __forceinline__ void flush_cols(float *o, uint32_t col, uint32_t Fo, const float8v &a, bool whole) {
+  const float v[8] = {a.lo.x, a.lo.y, a.lo.z, a.lo.w, a.hi.x, a.hi.y, a.hi.z, a.hi.w};
+  const uintptr_t align = reinterpret_cast<uintptr_t>(o);
+  if ((Fo & 3u) == 0 && (align & 15u) == 0) { // col and Fo multiples of 4: whole float4s
+#pragma unroll
+    for (int i = 0; i < 8; i += 4)
+      if (col + i < Fo)
+        add_vec(reinterpret_cast<float4 *>(o + col + i), make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]), whole);
+  } else if ((Fo & 1u) == 0 && (align & 7u) == 0) {
+#pragma unroll
+    for (int i = 0; i < 8; i += 2)
+      if (col + i < Fo)
+        add_vec(reinterpret_cast<float2 *>(o + col + i), make_float2(v[i], v[i + 1]), whole);
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; i++)
+      if (col + i < Fo)
+        add_vec(o + col + i, v[i], whole);
+  }
 }
 
 // A plan of parts (checked by the caller) with its slab count, and with hubs_allowed (a single part) its hub counts

@@ -17,18 +17,6 @@ constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 constexpr uint32_t kEdgeQuantum = 64; // consecutive edges per warp
 
-__device__ __forceinline__ uint32_t eo_find_row(const uint32_t *__restrict__ off, uint32_t n_rows, uint32_t e) {
-  uint32_t lo = 0, hi = n_rows;
-  while (hi - lo > 1) {
-    uint32_t mid = lo + ((hi - lo) >> 1);
-    if (__ldg(off + mid) <= e)
-      lo = mid;
-    else
-      hi = mid;
-  }
-  return lo;
-}
-
 // mirror slot of edge e: through the MirrorIndex table, or directly when the index array already holds slots
 __device__ __forceinline__ uint32_t slot_at(const uint32_t *__restrict__ row_idx,
                                             const uint32_t *__restrict__ mirror_index, size_t e) {
@@ -36,19 +24,6 @@ __device__ __forceinline__ uint32_t slot_at(const uint32_t *__restrict__ row_idx
   return mirror_index ? __ldg(mirror_index + id) : id;
 }
 
-template <int VEC> __device__ __forceinline__ void vec_red_add(typename Vec<VEC>::type *p, typename Vec<VEC>::type a);
-template <> __device__ __forceinline__ void vec_red_add<1>(float *p, float a) { atomicAdd(p, a); }
-template <> __device__ __forceinline__ void vec_red_add<2>(float2 *p, float2 a) {
-  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a.x), "f"(a.y) : "memory");
-}
-template <> __device__ __forceinline__ void vec_red_add<4>(float4 *p, float4 a) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a.x), "f"(a.y), "f"(a.z), "f"(a.w)
-               : "memory");
-}
-template <> __device__ __forceinline__ void vec_red_add<8>(float8v *p, float8v a) {
-  vec_red_add<4>(&p->lo, a.lo);
-  vec_red_add<4>(&p->hi, a.hi);
-}
 __device__ __forceinline__ float vec_dot(float a, float b) { return a * b; }
 __device__ __forceinline__ float vec_dot(float2 a, float2 b) { return fmaf(a.x, b.x, a.y * b.y); }
 __device__ __forceinline__ float vec_dot(float4 a, float4 b) {
@@ -61,13 +36,6 @@ __device__ __forceinline__ float vec_scale(float a, float s) { return a * s; }
 __device__ __forceinline__ float2 vec_scale(float2 a, float s) { return make_float2(a.x * s, a.y * s); }
 __device__ __forceinline__ float4 vec_scale(float4 a, float s) { return make_float4(a.x * s, a.y * s, a.z * s, a.w * s); }
 __device__ __forceinline__ float8v vec_scale(float8v a, float s) { return {vec_scale(a.lo, s), vec_scale(a.hi, s)}; }
-__device__ __forceinline__ void vec_zero(float &a) { a = 0.f; }
-__device__ __forceinline__ void vec_zero(float2 &a) { a = make_float2(0.f, 0.f); }
-__device__ __forceinline__ void vec_zero(float4 &a) { a = make_float4(0.f, 0.f, 0.f, 0.f); }
-__device__ __forceinline__ void vec_zero(float8v &a) {
-  vec_zero(a.lo);
-  vec_zero(a.hi);
-}
 __device__ __forceinline__ float vec_add(float a, float b) { return a + b; }
 __device__ __forceinline__ float2 vec_add(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ float4 vec_add(float4 a, float4 b) {
@@ -109,7 +77,7 @@ __global__ void __launch_bounds__(kThreads)
         if (MODE == 1)
           d[c] = vec_add(d[c], v);
         else
-          vec_red_add<VEC>(d + c, v);
+          red_add(d + c, v);
       }
     }
   }
@@ -122,27 +90,7 @@ __global__ void __launch_bounds__(kThreads)
 // reaching into its padding; stores are SVEC floats wide (dst is [n, F], so F's alignment decides).  A row takes
 // LANES lanes (a virtual warp of a warp for rows of at most 8 / 16 float4s, as in the planned kernel), and each lane
 // issues up to kGatherUnroll loads before it stores them.
-constexpr int kMaxShards = 32;
 constexpr int kGatherUnroll = 4;
-
-template <int SVEC> __device__ __forceinline__ void store_vec4(float *d, uint32_t col, float4 v, uint32_t F);
-template <> __device__ __forceinline__ void store_vec4<4>(float *d, uint32_t col, float4 v, uint32_t) {
-  *reinterpret_cast<float4 *>(d + col) = v;
-}
-template <> __device__ __forceinline__ void store_vec4<2>(float *d, uint32_t col, float4 v, uint32_t F) {
-  *reinterpret_cast<float2 *>(d + col) = make_float2(v.x, v.y);
-  if (col + 2 < F)
-    *reinterpret_cast<float2 *>(d + col + 2) = make_float2(v.z, v.w);
-}
-template <> __device__ __forceinline__ void store_vec4<1>(float *d, uint32_t col, float4 v, uint32_t F) {
-  d[col] = v.x;
-  if (col + 1 < F)
-    d[col + 1] = v.y;
-  if (col + 2 < F)
-    d[col + 2] = v.z;
-  if (col + 3 < F)
-    d[col + 3] = v.w;
-}
 
 template <int LANES, int SVEC>
 __global__ void __launch_bounds__(kThreads)
@@ -151,26 +99,14 @@ __global__ void __launch_bounds__(kThreads)
                                const uint32_t *__restrict__ ids, uint32_t n, uint32_t F) {
   __shared__ uint32_t s_off[kMaxShards + 1];
   __shared__ const float *s_shard[kMaxShards];
-  for (int i = threadIdx.x; i <= n_shards; i += blockDim.x) {
-    s_off[i] = __ldg(offsets + i);
-    if (i < n_shards)
-      s_shard[i] = shards[i];
-  }
-  __syncthreads();
+  stage_shard_table(s_off, s_shard, offsets, shards, n_shards);
   constexpr uint32_t kRowsPerBlock = kThreads / LANES;
   const uint32_t sub = threadIdx.x & (LANES - 1);
   const uint32_t nvec = (F + 3) / 4;
   for (uint64_t k = (uint64_t)blockIdx.x * kRowsPerBlock + threadIdx.x / LANES; k < n;
        k += (uint64_t)gridDim.x * kRowsPerBlock) {
     const uint32_t id = __ldg(ids + k);
-    int lo = 0, hi = n_shards;
-    while (hi - lo > 1) {
-      const int mid = (lo + hi) >> 1;
-      if (s_off[mid] <= id)
-        lo = mid;
-      else
-        hi = mid;
-    }
+    const int lo = find_shard(s_off, n_shards, id);
     const float4 *s = reinterpret_cast<const float4 *>(s_shard[lo] + (size_t)(id - s_off[lo]) * pitch);
     float *d = dst + (size_t)k * F;
     for (uint32_t c0 = sub; c0 < nvec; c0 += kGatherUnroll * LANES) {
@@ -182,7 +118,7 @@ __global__ void __launch_bounds__(kThreads)
 #pragma unroll
       for (int u = 0; u < kGatherUnroll; u++)
         if (c0 + u * LANES < nvec)
-          store_vec4<SVEC>(d, 4 * (c0 + u * LANES), v[u], F);
+          store_chunk<SVEC>(d, 4 * (c0 + u * LANES), F, v[u]);
     }
   }
 }
@@ -210,26 +146,14 @@ __global__ void __launch_bounds__(kThreads)
                                     const uint32_t *__restrict__ ids, uint32_t n, uint32_t F) {
   __shared__ uint32_t s_off[kMaxShards + 1];
   __shared__ const uint4 *s_shard[kMaxShards];
-  for (int i = threadIdx.x; i <= n_shards; i += blockDim.x) {
-    s_off[i] = __ldg(offsets + i);
-    if (i < n_shards)
-      s_shard[i] = shards[i];
-  }
-  __syncthreads();
+  stage_shard_table(s_off, s_shard, offsets, shards, n_shards);
   constexpr uint32_t kRowsPerBlock = kThreads / LANES;
   const uint32_t sub = threadIdx.x & (LANES - 1);
   const uint32_t nvec = (F + 7) / 8;
   for (uint64_t k = (uint64_t)blockIdx.x * kRowsPerBlock + threadIdx.x / LANES; k < n;
        k += (uint64_t)gridDim.x * kRowsPerBlock) {
     const uint32_t id = __ldg(ids + k);
-    int lo = 0, hi = n_shards;
-    while (hi - lo > 1) {
-      const int mid = (lo + hi) >> 1;
-      if (s_off[mid] <= id)
-        lo = mid;
-      else
-        hi = mid;
-    }
+    const int lo = find_shard(s_off, n_shards, id);
     const uint4 *s = s_shard[lo] + (size_t)(id - s_off[lo]) * (pitch / 8);
     for (uint32_t c0 = sub; c0 < nvec; c0 += kGatherUnroll * LANES) {
       uint4 v[kGatherUnroll];
@@ -246,9 +170,9 @@ __global__ void __launch_bounds__(kThreads)
           } else {
             float *d = reinterpret_cast<float *>(dst) + (size_t)k * F;
             const float8v x = widen(v[u]);
-            store_vec4<SVEC>(d, 8 * c, x.lo, F);
+            store_chunk<SVEC>(d, 8 * c, F, x.lo);
             if (8 * c + 4 < F)
-              store_vec4<SVEC>(d, 8 * c + 4, x.hi, F);
+              store_chunk<SVEC>(d, 8 * c + 4, F, x.hi);
           }
         }
       }
@@ -287,7 +211,7 @@ __global__ void __launch_bounds__(kThreads)
   for (uint64_t qw = (uint64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); qw * kEdgeQuantum < n_edges; qw += nwarps) {
   const uint32_t e0 = (uint32_t)(qw * kEdgeQuantum);
   const uint32_t e1 = (uint32_t)min((uint64_t)n_edges, (uint64_t)e0 + kEdgeQuantum);
-  uint32_t row = eo_find_row(off, n_rows, e0);
+  uint32_t row = find_row(off, n_rows, e0);
   uint32_t row_end = __ldg(off + row + 1);
   for (uint32_t e = e0; e < e1; e++) {
     while (e >= row_end) {
@@ -321,7 +245,7 @@ __global__ void __launch_bounds__(kThreads)
   for (uint32_t cbase = 0; cbase < nvec; cbase += 32) {
     const uint32_t c = cbase + lane;
     const bool act = c < nvec;
-    uint32_t row = eo_find_row(off, n_rows, e0);
+    uint32_t row = find_row(off, n_rows, e0);
     uint32_t row_end = __ldg(off + row + 1);
     bool inside = __ldg(off + row) >= e0;
     V acc;
@@ -333,7 +257,7 @@ __global__ void __launch_bounds__(kThreads)
           if (inside)
             *o = vec_add(*o, acc);
           else
-            vec_red_add<VEC>(o, acc);
+            red_add(o, acc);
         }
         memset(&acc, 0, sizeof(V));
         do {
@@ -350,7 +274,7 @@ __global__ void __launch_bounds__(kThreads)
       if (inside && row_end <= e1)
         *o = vec_add(*o, acc);
       else
-        vec_red_add<VEC>(o, acc);
+        red_add(o, acc);
     }
   }
   } // quantum loop
@@ -462,7 +386,7 @@ __global__ void __launch_bounds__(kThreads)
   for (uint64_t qw = (uint64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); qw * kEdgeQuantum < n_edges; qw += nwarps) {
     const uint32_t e0 = (uint32_t)(qw * kEdgeQuantum);
     const uint32_t e1 = (uint32_t)min((uint64_t)n_edges, (uint64_t)e0 + kEdgeQuantum);
-    uint32_t row = eo_find_row(off, n_rows, e0);
+    uint32_t row = find_row(off, n_rows, e0);
     uint32_t row_end = __ldg(off + row + 1);
     for (uint32_t e = e0; e < e1; e++) {
       while (e >= row_end) {
@@ -479,7 +403,7 @@ __global__ void __launch_bounds__(kThreads)
         for (uint32_t c = h * head_vecs + lane; c < (h + 1) * head_vecs; c += 32) {
           V gv = __ldg(gm + c);
           dot += vec_dot(__ldg(mm + c), gv);
-          vec_red_add<VEC>(dm + c, vec_scale(gv, ae));
+          red_add(dm + c, vec_scale(gv, ae));
         }
         dot = warp_sum(dot);
         if (lane == 0)
@@ -573,7 +497,7 @@ __global__ void __launch_bounds__(kThreads)
   for (uint64_t qw = (uint64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); qw * kQuantum < n_edges; qw += nwarps) {
     const uint32_t e0 = (uint32_t)(qw * kQuantum);
     const uint32_t e1 = (uint32_t)min((uint64_t)n_edges, (uint64_t)e0 + kQuantum);
-    uint32_t row = eo_find_row(off, n_rows, e0);
+    uint32_t row = find_row(off, n_rows, e0);
     uint32_t row_end = __ldg(off + row + 1);
     float dv, mx = 0.f, acc;
     auto load_row = [&]() {
@@ -661,7 +585,7 @@ __global__ void __launch_bounds__(kThreads)
   for (uint64_t qw = (uint64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); qw * kEdgeQuantum < n_edges; qw += nwarps) {
     const uint32_t e0 = (uint32_t)(qw * kEdgeQuantum);
     const uint32_t e1 = (uint32_t)min((uint64_t)n_edges, (uint64_t)e0 + kEdgeQuantum);
-    uint32_t row = eo_find_row(off, n_rows, e0);
+    uint32_t row = find_row(off, n_rows, e0);
     uint32_t row_end = __ldg(off + row + 1);
     float d_acc[KB], dv[KB], mv[KB], iz[KB], og[KB];
     auto load_row = [&]() {
@@ -732,7 +656,7 @@ __global__ void __launch_bounds__(kThreads)
             dot = vec_dot(m_cur[k], gv);
             pre = __ldg(s_att + (size_t)slot * H + hk[k]) + dv[k];
             a = expf(leaky(pre, slope) - mv[k]) * iz[k];
-            vec_red_add<VEC>(dm + c, vec_scale(gv, a));
+            red_add(dm + c, vec_scale(gv, a));
           }
           // per-head dot: lanes of one head are contiguous and head_vecs is a power of two
           for (uint32_t o = head_vecs >> 1; o > 0; o >>= 1)
@@ -774,7 +698,7 @@ __global__ void __launch_bounds__(kThreads)
     const uint32_t e0 = (uint32_t)(qw * kEdgeQuantum);
     const uint32_t e1 = (uint32_t)min((uint64_t)n_edges, (uint64_t)e0 + kEdgeQuantum);
     for (uint32_t h = 0; h < H; h++) { // one head at a time: the per-row accumulator is a single register
-      uint32_t row = eo_find_row(off, n_rows, e0);
+      uint32_t row = find_row(off, n_rows, e0);
       uint32_t row_end = __ldg(off + row + 1);
       float d_acc = 0.f;
       for (uint32_t e = e0; e < e1; e++) {
@@ -798,7 +722,7 @@ __global__ void __launch_bounds__(kThreads)
         for (uint32_t c = lane; c < head_vecs; c += 32) {
           V gv = __ldg(gm + c);
           dot += vec_dot(__ldg(mm + c), gv);
-          vec_red_add<VEC>(dm + c, vec_scale(gv, a));
+          red_add(dm + c, vec_scale(gv, a));
         }
         dot = warp_sum(dot);
         const float d_pre = a * (dot - __ldg(out_dot_g + rh)) * (pre > 0.f ? 1.f : slope);
@@ -864,7 +788,7 @@ __global__ void __launch_bounds__(kThreads)
   for (uint64_t qw = (uint64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); qw * kBwdQuantum < n_edges; qw += nwarps) {
     const uint32_t e0 = (uint32_t)(qw * kBwdQuantum);
     const uint32_t e1 = (uint32_t)min((uint64_t)n_edges, (uint64_t)e0 + kBwdQuantum);
-    uint32_t row = eo_find_row(off, n_rows, e0);
+    uint32_t row = find_row(off, n_rows, e0);
     uint32_t row_begin = __ldg(off + row), row_end = __ldg(off + row + 1);
     V yv[KB], mg[KB];
     float rs[KB], acc[KB];
@@ -878,7 +802,7 @@ __global__ void __launch_bounds__(kThreads)
           yv[k] = widen(__ldg(yr + lane + 32 * k));
         if constexpr (SRC_MAJOR) {
           rs[k] = __ldg(src_score + (size_t)row * H + hk[k]);
-          vec_zero(mg[k]);
+          zero_vec(mg[k]);
         } else {
           rp[k] = __ldg(dst_pack + (size_t)row * H + hk[k]);
         }
@@ -894,7 +818,7 @@ __global__ void __launch_bounds__(kThreads)
             if (whole)
               *o = vec_add(*o, mg[k]);
             else
-              vec_red_add<VEC>(o, mg[k]);
+              red_add(o, mg[k]);
           }
         }
         if (lead[k]) {
@@ -1011,16 +935,6 @@ __global__ void __launch_bounds__(kThreads)
 }
 
 // ---- launch helpers ----------------------------------------------------------------------------------------
-static int pick_vec(uint32_t F, const void *a, const void *b, const void *c = nullptr) {
-  bool a16 = aligned_to(a, 16) && aligned_to(b, 16) && (!c || aligned_to(c, 16));
-  bool a8 = aligned_to(a, 8) && aligned_to(b, 8) && (!c || aligned_to(c, 8));
-  if (F % 4 == 0 && a16)
-    return 4;
-  if (F % 2 == 0 && a8)
-    return 2;
-  return 1;
-}
-
 // persistent-style grid: enough CTAs to fill every SM several times over, work is grid-strided
 static unsigned stream_grid(uint64_t rows) {
   uint64_t blocks = (rows + kWarps - 1) / kWarps;
@@ -1072,7 +986,7 @@ int nts_gather_rows_sharded(float *dst, const float *const *shards, const nts_vi
   NTS_ARG_CHECK(shard_pitch % 4 == 0 && shard_pitch >= feature_size,
                 "nts_gather_rows_sharded: shard_pitch must be a multiple of 4 and at least feature_size");
   const uint32_t F = feature_size, nvec = (F + 3) / 4;
-  const int svec = pick_vec(F, dst, dst);
+  const int svec = pick_vec(F, dst);
   const int lanes = nvec <= 8 ? 8 : (nvec <= 16 ? 16 : 32);
   const uint64_t rows_per_block = kThreads / lanes;
   const uint64_t cap = (uint64_t)sm_count() * 16;
@@ -1105,7 +1019,7 @@ int nts_gather_rows_sharded_bf16(void *dst, int dst_dtype, nts_vid_t dst_ld, con
   NTS_ARG_CHECK(dst_dtype == NTS_DTYPE_F32 || aligned_to(dst, 16),
                 "nts_gather_rows_sharded_bf16: BF16 rows need a 16-byte aligned dst");
   const uint32_t F = feature_size, nvec = (F + 7) / 8;
-  const int svec = dst_dtype == NTS_DTYPE_BF16 ? 0 : pick_vec(F, dst, dst);
+  const int svec = dst_dtype == NTS_DTYPE_BF16 ? 0 : pick_vec(F, dst);
   const int lanes = nvec <= 8 ? 8 : (nvec <= 16 ? 16 : 32);
   const uint64_t rows_per_block = kThreads / lanes;
   const uint64_t cap = (uint64_t)sm_count() * 16;

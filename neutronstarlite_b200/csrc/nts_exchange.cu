@@ -278,16 +278,9 @@ static int check_wait_error(nts_exchange *ex, int rc) {
 }
 
 static int launch_push(nts_exchange *ex, const PushArgs &a, const float *src, uint32_t F, cudaStream_t st) {
-  int vec = 1;
-  bool a16 = aligned_to(src, 16), a8 = aligned_to(src, 8);
-  for (int k = 0; k < a.n; k++) {
-    a16 = a16 && aligned_to(a.t[k].dst, 16);
-    a8 = a8 && aligned_to(a.t[k].dst, 8);
-  }
-  if (F % 4 == 0 && a16)
-    vec = 4;
-  else if (F % 2 == 0 && a8)
-    vec = 2;
+  int vec = pick_vec(F, src);
+  for (int k = 0; k < a.n; k++)
+    vec = std::min(vec, pick_vec(F, a.t[k].dst));
   const int ctas = ex->push_ctas;
   ex->last.vec = vec;
   if (vec == 4)

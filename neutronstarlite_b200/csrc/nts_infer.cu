@@ -29,30 +29,12 @@ namespace nts {
 namespace {
 
 constexpr int kWarps = 8;
-constexpr int kMaxShards = 32;
 
+// a += w * (the 16-byte load v as FP32 values: 4 floats, or 8 BF16 values widened)
 __device__ __forceinline__ void acc_add(float4 &a, float w, uint4 v, float) {
-  a.x = fmaf(w, __uint_as_float(v.x), a.x);
-  a.y = fmaf(w, __uint_as_float(v.y), a.y);
-  a.z = fmaf(w, __uint_as_float(v.z), a.z);
-  a.w = fmaf(w, __uint_as_float(v.w), a.w);
+  fma_vec(a, w, make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w)));
 }
-__device__ __forceinline__ void acc_add(float8v &a, float w, uint4 v, __nv_bfloat16) {
-  const float8v x = widen(v);
-  a.lo.x = fmaf(w, x.lo.x, a.lo.x);
-  a.lo.y = fmaf(w, x.lo.y, a.lo.y);
-  a.lo.z = fmaf(w, x.lo.z, a.lo.z);
-  a.lo.w = fmaf(w, x.lo.w, a.lo.w);
-  a.hi.x = fmaf(w, x.hi.x, a.hi.x);
-  a.hi.y = fmaf(w, x.hi.y, a.hi.y);
-  a.hi.z = fmaf(w, x.hi.z, a.hi.z);
-  a.hi.w = fmaf(w, x.hi.w, a.hi.w);
-}
-__device__ __forceinline__ void acc_zero(float4 &a) { a = make_float4(0.f, 0.f, 0.f, 0.f); }
-__device__ __forceinline__ void acc_zero(float8v &a) {
-  acc_zero(a.lo);
-  acc_zero(a.hi);
-}
+__device__ __forceinline__ void acc_add(float8v &a, float w, uint4 v, __nv_bfloat16) { fma_vec(a, w, widen(v)); }
 
 __device__ __forceinline__ void add4(float *p, float4 a, bool whole) {
   if (whole) {
@@ -110,19 +92,6 @@ __device__ __forceinline__ void flush_acc(float *o, uint32_t col, uint32_t F, co
   flush4(o, col, F, a.lo, svec, whole);
   if (col + 4 < F)
     flush4(o, col + 4, F, a.hi, svec, whole);
-}
-
-// largest r in [0, n_rows) with off[r] <= e  (requires off[0] <= e < off[n_rows])
-__device__ __forceinline__ uint32_t find_row(const uint32_t *__restrict__ off, uint32_t n_rows, uint32_t e) {
-  uint32_t lo = 0, hi = n_rows;
-  while (hi - lo > 1) {
-    const uint32_t mid = lo + ((hi - lo) >> 1);
-    if (__ldg(off + mid) <= e)
-      lo = mid;
-    else
-      hi = mid;
-  }
-  return lo;
 }
 
 // Weight policies of the walk.  The lane that stages an edge turns (edge, shard, local row) into a Staged value that
@@ -213,14 +182,8 @@ __global__ void __launch_bounds__(kWarps * 32, MINB)
   W<K> wp{prm};
   __shared__ uint32_t s_off[kMaxShards + 1];
   __shared__ const unsigned char *s_shard[W<K>::kTables * kMaxShards]; // row shards, then the policy's
-  for (int i = threadIdx.x; i <= n_shards; i += blockDim.x) {
-    s_off[i] = __ldg(shard_off + i);
-    if (i < n_shards) {
-      s_shard[i] = shards[i];
-      wp.stage_table(s_shard + kMaxShards, i);
-    }
-  }
-  __syncthreads();
+  stage_shard_table(s_off, s_shard, shard_off, shards, n_shards,
+                    [&](int i) { wp.stage_table(s_shard + kMaxShards, i); });
 
   const uint32_t lane = threadIdx.x & (GS - 1);
   const unsigned gmask = G == 1 ? 0xffffffffu : (((1u << GS) - 1u) << ((threadIdx.x & 31u) & ~(GS - 1u)));
@@ -247,7 +210,7 @@ __global__ void __launch_bounds__(kWarps * 32, MINB)
   Acc acc[K];
 #pragma unroll
   for (int k = 0; k < K; k++)
-    acc_zero(acc[k]);
+    zero_vec(acc[k]);
 
   auto flush = [&](bool whole) {
     float *o = out + (size_t)row * F;
@@ -255,7 +218,7 @@ __global__ void __launch_bounds__(kWarps * 32, MINB)
     for (int k = 0; k < K; k++) {
       if (act[k])
         flush_acc(o, (c0 + k * GS) * VEC, F, acc[k], svec, whole);
-      acc_zero(acc[k]);
+      zero_vec(acc[k]);
     }
   };
   auto advance = [&](uint32_t ee) { // ee >= row_end: the current row ends inside the quantum
@@ -274,14 +237,7 @@ __global__ void __launch_bounds__(kWarps * 32, MINB)
     Staged my_w = W<K>::kIdle;
     if (lane < cnt) { // the edge's shard, once: binary search over the staged offsets
       const uint32_t id = __ldg(idx + e + lane);
-      int lo = 0, hi = n_shards;
-      while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (s_off[mid] <= id)
-          lo = mid;
-        else
-          hi = mid;
-      }
+      const int lo = find_shard(s_off, n_shards, id);
       my_row = reinterpret_cast<unsigned long long>(s_shard[lo]) + (unsigned long long)(id - s_off[lo]) * row_bytes;
       my_w = wp.stage(e, lane, s_shard + kMaxShards, lo, id - s_off[lo]);
     }
@@ -381,7 +337,7 @@ int dispatch(float *out, const void *const *shards, const uint32_t *shard_off, i
              uint32_t e_begin, uint32_t e_end, uint32_t F, cudaStream_t st, const char *who) {
   constexpr uint32_t VEC = 16 / sizeof(T);
   const Shape s = pick_shape((F + VEC - 1) / VEC);
-  const int svec = (F % 4 == 0 && aligned_to(out, 16)) ? 4 : ((F % 2 == 0 && aligned_to(out, 8)) ? 2 : 1);
+  const int svec = pick_vec(F, out);
   const uint32_t row_bytes = pitch * (uint32_t)sizeof(T);
 #define NTS_K9_CASE(K_, U_, G_, B_)                                                                                   \
   if (s.k == K_ && s.u == U_ && s.g == G_ && s.minb == B_)                                                          \
@@ -429,12 +385,7 @@ __global__ void __launch_bounds__(kWarps * 32)
   constexpr uint32_t kQuantum = 512;
   __shared__ uint32_t s_off[kMaxShards + 1];
   __shared__ const unsigned char *s_shard[kMaxShards];
-  for (int i = threadIdx.x; i <= n_shards; i += blockDim.x) {
-    s_off[i] = __ldg(shard_off + i);
-    if (i < n_shards)
-      s_shard[i] = score_shards[i];
-  }
-  __syncthreads();
+  stage_shard_table(s_off, s_shard, shard_off, score_shards, n_shards);
 
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t h = lane % H, el = lane / H;
@@ -462,14 +413,7 @@ __global__ void __launch_bounds__(kWarps * 32)
     };
     auto score = [&](uint32_t e) {
       const uint32_t id = __ldg(idx + e);
-      int lo = 0, hi = n_shards;
-      while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (s_off[mid] <= id)
-          lo = mid;
-        else
-          hi = mid;
-      }
+      const int lo = find_shard(s_off, n_shards, id);
       return __ldg(reinterpret_cast<const float *>(s_shard[lo] + (size_t)(id - s_off[lo]) * score_row_bytes) + h);
     };
     load_row();

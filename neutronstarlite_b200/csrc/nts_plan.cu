@@ -70,18 +70,6 @@ namespace nts {
 static int g_plan_u = 0, g_plan_minb = 0, g_plan_q = 0, g_plan_variant = 0; // measurement hooks (NTS_PLAN_TUNE="U,MINB[,Q]"), 0 = default
 
 // ---- plan construction kernels -----------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t plan_find_row(const uint32_t *__restrict__ off, uint32_t n_rows, uint32_t e) {
-  uint32_t lo = 0, hi = n_rows;
-  while (hi - lo > 1) {
-    uint32_t mid = lo + ((hi - lo) >> 1);
-    if (__ldg(off + mid) <= e)
-      lo = mid;
-    else
-      hi = mid;
-  }
-  return lo;
-}
-
 // The mapped (gathered) row of edge e of a part: index_add + (slot_of[idx[e]] or idx[e] - index_base)
 __device__ __forceinline__ uint32_t plan_gathered_row(const nts_plan_part &pt, uint32_t e) {
   const uint32_t id = __ldg(pt.indices + e);
@@ -102,7 +90,7 @@ __global__ void plan_keys_kernel(nts_plan_part pt, uint32_t e_off, uint32_t n_ro
                                  uint32_t lda_c, uint64_t dc_cells, uint32_t lda_r, KeyT *__restrict__ key,
                                  uint32_t *__restrict__ val) {
   for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < pt.n_edges; e += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t r = plan_find_row(pt.offsets, pt.n_rows, (uint32_t)e) + pt.row_add;
+    const uint32_t r = find_row(pt.offsets, pt.n_rows, (uint32_t)e) + pt.row_add;
     const uint32_t g = plan_gathered_row(pt, (uint32_t)e);
     uint32_t s = g / slab_rows;
     if (s >= slabs)
@@ -224,32 +212,6 @@ __global__ void bf16_rows_kernel(const S *__restrict__ src, uint32_t lds, uint4 
 }
 
 // ---- the aggregation kernel ----------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t p_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void p_mbar_init(uint64_t *bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(p_smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void p_mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(p_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void p_mbar_wait(uint64_t *bar, uint32_t parity) {
-  asm volatile("{\n\t"
-               ".reg .pred p;\n\t"
-               "WAIT_%=:\n\t"
-               "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-               "@p bra DONE_%=;\n\t"
-               "bra WAIT_%=;\n\t"
-               "DONE_%=:\n\t"
-               "}" ::"r"(p_smem_u32(bar)),
-               "r"(parity)
-               : "memory");
-}
-__device__ __forceinline__ void p_bulk_g2s(void *smem_dst, const void *gmem_src, uint32_t bytes, uint64_t *bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   p_smem_u32(smem_dst)),
-               "l"(gmem_src), "r"(bytes), "r"(p_smem_u32(bar))
-               : "memory");
-}
-
 constexpr int kPlanWarps = 8;
 
 // Output columns 4c .. 4c+3 of one accumulator chunk, OUTV floats per store (the output keeps the caller's row
@@ -292,25 +254,6 @@ __device__ __forceinline__ void flush_chunk(float *__restrict__ orow, uint32_t c
         else
           orow[col + i] += v[i];
       }
-  }
-}
-
-// flush_chunk's plain store: the chunk's columns (< F) are written without reading the output.
-template <int OUTV>
-__device__ __forceinline__ void store_chunk(float *__restrict__ orow, uint32_t col, uint32_t F, float4 a) {
-  if constexpr (OUTV == 4) {
-    *reinterpret_cast<float4 *>(orow + col) = a;
-  } else if constexpr (OUTV == 2) {
-    float2 *p = reinterpret_cast<float2 *>(orow + col);
-    p[0] = make_float2(a.x, a.y);
-    if (col + 2 < F)
-      p[1] = make_float2(a.z, a.w);
-  } else {
-    const float v[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-    for (int i = 0; i < 4; i++)
-      if (col + i < F)
-        orow[col + i] = v[i];
   }
 }
 
@@ -382,15 +325,15 @@ __device__ __forceinline__ void planned_gather_body(unsigned char *smem_raw, uin
       const uint32_t n_el = (uint32_t)(ce1 - cta_e_base);
       bulk_bytes = (n_el * 8u) & ~15u;      // whole 16-byte units through the bulk engine, a last odd element by a plain load
       if (threadIdx.x == 0) {
-        p_mbar_init(bar, 1);
+        mbar_init(bar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         if (n_el & 1u)
           s_pair[n_el - 1] = __ldg(pairs + cta_e_base + n_el - 1);
       }
       __syncthreads();
       if (threadIdx.x == 0 && bulk_bytes) {
-        p_mbar_expect_tx(bar, bulk_bytes);
-        p_bulk_g2s(s_pair, pairs + cta_e_base, bulk_bytes, bar);
+        mbar_expect_tx(bar, bulk_bytes);
+        bulk_g2s(s_pair, pairs + cta_e_base, bulk_bytes, bar);
       }
     }
   }
@@ -405,7 +348,7 @@ __device__ __forceinline__ void planned_gather_body(unsigned char *smem_raw, uin
   for (int k = 0; k < K; k++)
     act[k] = (k * GS + lane) < tile_vecs && (c0 + k * GS) < ldc;
 
-  uint32_t row = plan_find_row(off, n_rows, e0);
+  uint32_t row = find_row(off, n_rows, e0);
   uint32_t row_end = __ldg(off + row + 1);
   bool row_started_inside = __ldg(off + row) >= e0;
 
@@ -446,7 +389,7 @@ __device__ __forceinline__ void planned_gather_body(unsigned char *smem_raw, uin
   };
 
   if (bulk_bytes)
-    p_mbar_wait(bar, 0);
+    mbar_wait(bar, 0);
 
   const uint2 *sp = s_pair - cta_e_base;
   uint32_t e = e0;
@@ -551,13 +494,13 @@ __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
       ce1 = e_end;
     if (lane == 0)
       for (int s = 0; s < STAGES; s++)
-        p_mbar_init(sbar + s, 1);
+        mbar_init(sbar + s, 1);
     if (ce0 < ce1) {
       cta_e_base = (uint32_t)(ce0 & ~1ull);
       const uint32_t n_el = (uint32_t)(ce1 - cta_e_base);
       bulk_bytes = (n_el * 8u) & ~15u;
       if (threadIdx.x == 0) {
-        p_mbar_init(bar, 1);
+        mbar_init(bar, 1);
         if (n_el & 1u)
           s_pair[n_el - 1] = __ldg(pairs + cta_e_base + n_el - 1);
       }
@@ -565,8 +508,8 @@ __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
     if (threadIdx.x == 0 && bulk_bytes) {
-      p_mbar_expect_tx(bar, bulk_bytes);
-      p_bulk_g2s(s_pair, pairs + cta_e_base, bulk_bytes, bar);
+      mbar_expect_tx(bar, bulk_bytes);
+      bulk_g2s(s_pair, pairs + cta_e_base, bulk_bytes, bar);
     }
   }
   if (e0_64 >= e_end)
@@ -581,13 +524,13 @@ __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
   for (int k = 0; k < K; k++)
     act[k] = (k * 32 + lane) < my_vecs;
 
-  uint32_t row = plan_find_row(off, n_rows, e0);
+  uint32_t row = find_row(off, n_rows, e0);
   uint32_t row_end = __ldg(off + row + 1);
   bool row_started_inside = __ldg(off + row) >= e0;
   float4 acc[K];
 #pragma unroll
   for (int k = 0; k < K; k++)
-    acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+    zero_vec(acc[k]);
   auto flush = [&](bool whole) {
     float *orow = out + (size_t)row * F;
 #pragma unroll
@@ -599,7 +542,7 @@ __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
         else
           flush_chunk<OUTV, true>(orow, col, F, acc[k]);
       }
-      acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+      zero_vec(acc[k]);
     }
   };
   auto advance = [&](uint32_t ee) {
@@ -611,12 +554,12 @@ __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
     row_started_inside = true;
   };
   if (bulk_bytes)
-    p_mbar_wait(bar, 0);
+    mbar_wait(bar, 0);
   const uint2 *sp = s_pair - cta_e_base;
   auto issue = [&](uint32_t e, uint32_t stage) { // lane 0 only
     const uint32_t src_row = sp[e].x;
-    p_mbar_expect_tx(sbar + stage, row_bytes);
-    p_bulk_g2s(sbuf + (size_t)stage * tile_vecs, in + (size_t)src_row * ld4 + tile * tile_vecs, row_bytes, sbar + stage);
+    mbar_expect_tx(sbar + stage, row_bytes);
+    bulk_g2s(sbuf + (size_t)stage * tile_vecs, in + (size_t)src_row * ld4 + tile * tile_vecs, row_bytes, sbar + stage);
   };
   if (lane == 0)
     for (uint32_t s = 0; s < STAGES && e0 + s < e1; s++)
@@ -624,7 +567,7 @@ __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
   uint32_t stage = 0, parity = 0;
   for (uint32_t e = e0; e < e1; e++) {
     const float w = __uint_as_float(sp[e].y);
-    p_mbar_wait(sbar + stage, parity);
+    mbar_wait(sbar + stage, parity);
     const float4 *b = sbuf + (size_t)stage * tile_vecs + lane;
     float4 v[K];
 #pragma unroll
@@ -635,12 +578,8 @@ __global__ void __launch_bounds__(kPlanWarps * 32, MINB)
       advance(e);
 #pragma unroll
     for (int k = 0; k < K; k++)
-      if (act[k]) {
-        acc[k].x = fmaf(w, v[k].x, acc[k].x);
-        acc[k].y = fmaf(w, v[k].y, acc[k].y);
-        acc[k].z = fmaf(w, v[k].z, acc[k].z);
-        acc[k].w = fmaf(w, v[k].w, acc[k].w);
-      }
+      if (act[k])
+        fma_vec(acc[k], w, v[k]);
     __syncwarp(); // every lane has consumed the stage (its values are in registers and used): it may be overwritten
     if (lane == 0 && e + STAGES < e1)
       issue(e + STAGES, stage);
@@ -754,7 +693,7 @@ static int launch_planned_tma(nts_gather_plan *pl, const PlanShape &sh, const fl
 constexpr int kHubBM = 128, kHubBN = 128, kHubBK = 16, kHubThreads = 256;
 
 __device__ __forceinline__ void p_cp_async16(void *smem_dst, const void *gmem_src, bool full) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(p_smem_u32(smem_dst)), "l"(gmem_src),
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src),
                "r"(full ? 16 : 0)
                : "memory");
 }
@@ -874,7 +813,7 @@ __device__ __forceinline__ void hub_gemm_tile(HubSmem<TN, TB> &sm, uint32_t tile
       const float4 a = make_float4(acc[i][j * 4], acc[i][j * 4 + 1], acc[i][j * 4 + 2], acc[i][j * 4 + 3]);
       if (col < F) {
         if constexpr (STORE)
-          store_chunk<OUTV>(orow, col, F, a);
+          store_chunk_checked<OUTV>(orow, col, F, a);
         else
           flush_chunk<OUTV, SPLIT>(orow, col, F, a);
       }
@@ -1042,7 +981,7 @@ static int run_gather(nts_gather_plan *pl, const T *in, uint32_t ld, float *outp
   sh.tile_vecs = (ldc + sh.tiles - 1) / sh.tiles;
   sh.k = (int)((sh.tile_vecs + 31) / 32);
   sh.tiles = (ldc + sh.tile_vecs - 1) / sh.tile_vecs;
-  sh.outv = (F % 4 == 0 && aligned_to(output, 16)) ? 4 : ((F % 2 == 0 && aligned_to(output, 8)) ? 2 : 1);
+  sh.outv = pick_vec(F, output);
   const bool fused = pl->overlap && pl->hub_rows;
   NTS_ARG_CHECK(!fused || g_plan_variant == 0, "the fused slab launches use the register-staging gather (variant 0)");
   if (overwrite && !pl->hub_cols)

@@ -37,7 +37,7 @@ constexpr int kMaxFanout = 64;
 constexpr int kMaxHops = 8;
 constexpr int kSelectWarps = 8;
 constexpr int kThreads = 256;
-constexpr int kMaxShards = 32;       // nts_sampler_create_sharded
+using nts::kMaxShards;               // nts_sampler_create_sharded
 constexpr u32 kMarker = 0x80000000u;   // value bit of a destination marker pair (edge positions are < 2^31)
 
 __host__ __device__ __forceinline__ u64 splitmix64(u64 z) {
@@ -79,11 +79,7 @@ __device__ __forceinline__ const ShardTable &stage_shards(const ShardTable *__re
 // The owner of v < V is the last shard with off[o] <= v, so an empty shard (off[o] == off[o+1]) is never chosen; v's
 // in-edges are slots [base, base + deg) of the owner's row / w.
 __device__ __forceinline__ int shard_of(const ShardTable &t, u32 v, u32 &base, u32 &deg) {
-  int lo = 0, hi = (int)t.n;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (t.off[mid] <= v) lo = mid; else hi = mid;
-  }
+  const int lo = nts::find_shard(t.off, (int)t.n, v);
   const u32 lv = v - t.off[lo];
   base = t.col[lo][lv];
   deg = t.col[lo][lv + 1] - base;
