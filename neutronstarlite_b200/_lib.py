@@ -1,4 +1,5 @@
-"""ctypes binding of libnts_b200.so - the C ABI declared in include/nts_b200.h.
+"""ctypes binding of libnts_b200.so - the C ABI declared in include/nts_b200.h - and the plumbing every caller shares:
+status and handle checks, the current stream, borrowed device arrays and caller ids.
 
 There is no fallback: if the shared object is missing or a call fails, we raise.
 """
@@ -7,6 +8,9 @@ from __future__ import annotations
 import ctypes as C
 import os
 import re
+
+import numpy as np
+import torch
 
 PKG = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG)
@@ -273,13 +277,64 @@ def load():
     return lib
 
 
+def last_error():
+    """The text of the library's last failure on this thread."""
+    return load().nts_last_error().decode(errors="replace")
+
+
 def check(rc, what=""):
     if rc != 0:
-        msg = load().nts_last_error().decode(errors="replace")
-        raise NtsError("libnts_b200 %s failed (rc=%d): %s" % (what, rc, msg))
+        raise NtsError("libnts_b200 %s failed (rc=%d): %s" % (what, rc, last_error()))
 
 
 def call(name, *args):
     """Invoke an int-returning ABI function and raise on a non-zero status."""
     rc = getattr(load(), name)(*args)
     check(rc, name)
+
+
+def checked(handle, what):
+    """A handle or pointer an ABI function returned; NtsError with the library's reason when it is null."""
+    if not handle:
+        raise NtsError("%s failed: %s" % (what, last_error()))
+    return handle
+
+
+def stream(device=None):
+    """The current CUDA stream of `device` (default: the current device), as the ABI's stream argument."""
+    return torch.cuda.current_stream(device).cuda_stream
+
+
+class _DeviceArray:
+    """A borrowed 1-D device array for torch.as_tensor (the CUDA array interface; no copy, no stream sync)."""
+
+    def __init__(self, ptr, n, typestr):
+        self.__cuda_array_interface__ = {"shape": (int(n),), "typestr": typestr, "data": (int(ptr), False),
+                                         "version": 2, "strides": None}
+
+
+_TYPESTR = {torch.int32: "<i4", torch.float32: "<f4"}
+
+
+def borrowed(ptr, n, dtype, device):
+    """A tensor over n int32 or float32 values of device memory at ptr that the library owns (no copy); an empty tensor
+    when n == 0, whatever ptr is."""
+    if n == 0:
+        return torch.empty(0, dtype=dtype, device=device)
+    return torch.as_tensor(_DeviceArray(ptr, n, _TYPESTR[dtype]), device=device)
+
+
+def device_ids(ids, bound, device, name, what):
+    """Caller ids (an integer tensor, numpy array or list) as a contiguous int32 tensor on `device`.  Ids outside
+    [0, bound) raise NtsError ("<what> must be in [0, bound)") before any device work for host ids; device ids are
+    checked in the caller's dtype, since a cast first could wrap an int64 id >= 2^32 into range."""
+    if torch.is_tensor(ids) and ids.is_cuda:
+        if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
+            raise NtsError("%s must be an integer tensor, not %s" % (name, ids.dtype))
+        if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= bound):
+            raise NtsError("%s must be in [0, %d)" % (what, bound))
+        return ids.reshape(-1).to(device=device, dtype=torch.int32).contiguous()
+    a = np.asarray(ids.numpy() if torch.is_tensor(ids) else ids).reshape(-1).astype(np.int64)
+    if a.size and (a.min() < 0 or a.max() >= bound):
+        raise NtsError("%s must be in [0, %d)" % (what, bound))
+    return torch.from_numpy(a.astype(np.int32)).to(device)

@@ -241,12 +241,11 @@ class GpuExchange:
     def forward(self, x, gather_dtype=None):
         """gather_dtype=torch.bfloat16: BF16 gathers with FP32 accumulation (ops.GatherPlan.run's contract); x may be
         float32 or bfloat16, the rows travel as BF16 on both transports."""
-        pg, plan, P, p = self.pg, self.plan, self.P, self.p
+        pg, plan = self.pg, self.plan
         bf16 = ops._check_gather_dtype(gather_dtype) is not None
         F = x.shape[1]
         y = torch.zeros((pg.owned_vertices, F), dtype=torch.float32, device=x.device)
-        cur = torch.cuda.current_stream()
-        if P == 1:
+        if self.P == 1:
             return ops.gather_by_dst_from_src(pg.graph_chunks[0], y, x, gather_dtype=gather_dtype)
         if self._p2p is not None:
             return self._forward_p2p(x, y, bf16)
@@ -257,67 +256,59 @@ class GpuExchange:
         recv = self._buf("frecv", plan.recv_total, F)
         if plan.send_total:
             _lib.call("nts_gather_rows", _ptr(send), _ptr(x), _ptr(plan.send_rows_all), plan.send_total, F,
-                      cur.cuda_stream)
-        self.comm_stream.wait_stream(cur)
-        with torch.cuda.stream(self.comm_stream):
-            in_split = [plan.send_count[j] if j != p else 0 for j in range(P)]
-            out_split = [plan.need_count[i] if i != p else 0 for i in range(P)]
-            dist.all_to_all_single(recv, send, output_split_sizes=out_split, input_split_sizes=in_split,
-                                   group=self.group)
-        # local chunk overlaps with the transfer
-        ops.gather_by_dst_from_src(pg.graph_chunks[p], y, x)
-        cur.wait_stream(self.comm_stream)
-        recv.record_stream(cur)
+                      _lib.stream())
+        self._all_to_all(recv, send, True, lambda: ops.gather_by_dst_from_src(pg.graph_chunks[self.p], y, x))
         self._aggregate_remote(y, recv)
         return y
+
+    def _all_to_all(self, recv, send, forward, local):
+        """One all_to_all_single of the packed rows with every peer on the side stream, while local() (the local
+        chunk's aggregation) runs on the current stream; the current stream then waits for recv.  forward: send
+        holds the rows each peer needs of this rank and recv the rows this rank needs; backward the other way round,
+        with partial gradients."""
+        plan, P, p = self.plan, self.P, self.p
+        cur = torch.cuda.current_stream()
+        self.comm_stream.wait_stream(cur)
+        with torch.cuda.stream(self.comm_stream):
+            sends = [plan.send_count[j] if j != p else 0 for j in range(P)]
+            needs = [plan.need_count[i] if i != p else 0 for i in range(P)]
+            dist.all_to_all_single(recv, send, output_split_sizes=needs if forward else sends,
+                                   input_split_sizes=sends if forward else needs, group=self.group)
+        local()
+        cur.wait_stream(self.comm_stream)
+        recv.record_stream(cur)
 
     def _forward_nccl_bf16(self, x, y):
         """x converted to BF16 once; the packed rows travel as BF16 (half the bytes); the local chunk and the merged
         remote chunks gather BF16 rows."""
-        pg, plan, P, p = self.pg, self.plan, self.P, self.p
+        pg, plan = self.pg, self.plan
         F = x.shape[1]
-        cur = torch.cuda.current_stream()
         xb = x if x.dtype == torch.bfloat16 else x.to(torch.bfloat16)
         send = self._buf("fsend16", plan.send_total, F, torch.bfloat16)
         recv = self._buf("frecv16", plan.recv_total, F, torch.bfloat16)
         if plan.send_total:
             torch.index_select(xb, 0, plan.send_rows_all, out=send)
-        self.comm_stream.wait_stream(cur)
-        with torch.cuda.stream(self.comm_stream):
-            in_split = [plan.send_count[j] if j != p else 0 for j in range(P)]
-            out_split = [plan.need_count[i] if i != p else 0 for i in range(P)]
-            dist.all_to_all_single(recv, send, output_split_sizes=out_split, input_split_sizes=in_split,
-                                   group=self.group)
-        ops.gather_by_dst_from_src(pg.graph_chunks[p], y, xb, gather_dtype=torch.bfloat16)
-        cur.wait_stream(self.comm_stream)
-        recv.record_stream(cur)
+        self._all_to_all(recv, send, True, lambda: ops.gather_by_dst_from_src(pg.graph_chunks[self.p], y, xb,
+                                                                              gather_dtype=torch.bfloat16))
         if plan.remote_edges:
             self._merged_plan("fwd", F).run(recv, y, torch.bfloat16)
         return y
 
     def _backward_nccl_bf16(self, g, dx):
         """dY converted to BF16 once locally; partial gradients are computed, sent and added in FP32."""
-        pg, plan, P, p = self.pg, self.plan, self.P, self.p
+        pg, plan = self.pg, self.plan
         F = g.shape[1]
-        cur = torch.cuda.current_stream()
         gb = g.to(torch.bfloat16)
         send = self._buf("bsend", plan.recv_total, F)
         recv = self._buf("brecv", plan.send_total, F)
         send.zero_()
         if plan.remote_edges:
             self._merged_plan("bwd", F).run(gb, send, torch.bfloat16)
-        self.comm_stream.wait_stream(cur)
-        with torch.cuda.stream(self.comm_stream):
-            in_split = [plan.need_count[i] if i != p else 0 for i in range(P)]
-            out_split = [plan.send_count[j] if j != p else 0 for j in range(P)]
-            dist.all_to_all_single(recv, send, output_split_sizes=out_split, input_split_sizes=in_split,
-                                   group=self.group)
-        ops.gather_by_src_from_dst(pg.graph_chunks[p], dx, gb, gather_dtype=torch.bfloat16)
-        cur.wait_stream(self.comm_stream)
-        recv.record_stream(cur)
+        self._all_to_all(recv, send, False, lambda: ops.gather_by_src_from_dst(pg.graph_chunks[self.p], dx, gb,
+                                                                               gather_dtype=torch.bfloat16))
         if plan.send_total:
             _lib.call("nts_scatter_add_rows_atomic", _ptr(dx), _ptr(recv), _ptr(plan.send_rows_all), plan.send_total, F,
-                      cur.cuda_stream)
+                      _lib.stream())
         return dx
 
     def _aggregate_remote(self, y, staged):
@@ -325,14 +316,10 @@ class GpuExchange:
         plan = self.plan
         if not plan.remote_edges:
             return
-        ev = ops._timer.bracket("fwd", staged.shape[1], plan.remote_edges, self.pg.owned_vertices) if ops._timer else None
-        if ev:
-            ev[0].record()
-        _lib.call("nts_segment_gather_sum", _ptr(staged), _ptr(y), _ptr(plan.remote_w), _ptr(plan.remote_slots),
-                  _ptr(plan.remote_col_offset), 0, self.pg.owned_vertices, plan.remote_edges, staged.shape[1],
-                  torch.cuda.current_stream().cuda_stream)
-        if ev:
-            ev[1].record()
+        with ops._timed("fwd", staged.shape[1], plan.remote_edges, self.pg.owned_vertices):
+            _lib.call("nts_segment_gather_sum", _ptr(staged), _ptr(y), _ptr(plan.remote_w), _ptr(plan.remote_slots),
+                      _ptr(plan.remote_col_offset), 0, self.pg.owned_vertices, plan.remote_edges, staged.shape[1],
+                      _lib.stream())
 
     def _partial_remote(self, out_rows, g):
         """Partial gradients of the active sources of ALL remote chunks in one launch (merged compact CSR); the
@@ -340,14 +327,10 @@ class GpuExchange:
         plan = self.plan
         if not plan.remote_edges:
             return
-        ev = ops._timer.bracket("bwd", g.shape[1], plan.remote_edges, out_rows.shape[0]) if ops._timer else None
-        if ev:
-            ev[0].record()
-        _lib.call("nts_segment_gather_sum", _ptr(g), _ptr(out_rows), _ptr(plan.bwd_w), _ptr(plan.bwd_indices),
-                  _ptr(plan.bwd_offsets), self.pg.graph_chunks[self.p].dst_range[0], out_rows.shape[0],
-                  plan.remote_edges, g.shape[1], torch.cuda.current_stream().cuda_stream)
-        if ev:
-            ev[1].record()
+        with ops._timed("bwd", g.shape[1], plan.remote_edges, out_rows.shape[0]):
+            _lib.call("nts_segment_gather_sum", _ptr(g), _ptr(out_rows), _ptr(plan.bwd_w), _ptr(plan.bwd_indices),
+                      _ptr(plan.bwd_offsets), self.pg.graph_chunks[self.p].dst_range[0], out_rows.shape[0],
+                      plan.remote_edges, g.shape[1], _lib.stream())
 
     # ---- mirror fetch / return (DistGPUGetDepNbrOp, core/ntsDistGPUGraphOp.hpp:48-143) ----------------------------
     def fetch_mirrors(self, x):
@@ -358,16 +341,16 @@ class GpuExchange:
         feature matrix to the host, through MPI and back, core/ntsDistGPUGraphOp.hpp:56-98.)"""
         plan, P, p = self.plan, self.P, self.p
         F = x.shape[1]
-        cur = torch.cuda.current_stream()
+        st = _lib.stream()
         M = sum(plan.need_count)
         mirror = torch.zeros((M, F), dtype=torch.float32, device=x.device)
         if self._p2p is not None:   # the peer-memory engine: rows pushed into the receive windows, no NCCL
             self._p2p.reserve(F)
-            _lib.call("nts_exchange_fetch_mirrors", self._p2p.handle, _ptr(x), _ptr(mirror), F, cur.cuda_stream)
+            _lib.call("nts_exchange_fetch_mirrors", self._p2p.handle, _ptr(x), _ptr(mirror), F, st)
             return mirror
         if P == 1:
             if M:
-                _lib.call("nts_gather_rows", _ptr(mirror), _ptr(x), _ptr(plan.need[0]), M, F, cur.cuda_stream)
+                _lib.call("nts_gather_rows", _ptr(mirror), _ptr(x), _ptr(plan.need[0]), M, F, st)
             return mirror
         rows_out = [plan.send_rows[j] if j != p else plan.need[p] for j in range(P)]
         n_out = [int(r.numel()) for r in rows_out]
@@ -376,7 +359,7 @@ class GpuExchange:
         for j in range(P):
             if n_out[j]:
                 _lib.call("nts_gather_rows", _ptr(send[pos:pos + n_out[j]]), _ptr(x), _ptr(rows_out[j]), n_out[j], F,
-                          cur.cuda_stream)
+                          st)
             pos += n_out[j]
         dist.all_to_all_single(mirror, send, output_split_sizes=list(plan.need_count), input_split_sizes=n_out,
                                group=self.group)
@@ -387,17 +370,15 @@ class GpuExchange:
         what arrives from all partitions (one unique-row scatter-add per sender)."""
         pg, plan, P, p = self.pg, self.plan, self.P, self.p
         F = gm.shape[1]
-        cur = torch.cuda.current_stream()
+        st = _lib.stream()
         dx = torch.zeros((pg.owned_vertices, F), dtype=torch.float32, device=gm.device)
         if self._p2p is not None:
             self._p2p.reserve(F)
-            _lib.call("nts_exchange_return_mirror_grads", self._p2p.handle, _ptr(gm.contiguous()), _ptr(dx), F,
-                      cur.cuda_stream)
+            _lib.call("nts_exchange_return_mirror_grads", self._p2p.handle, _ptr(gm.contiguous()), _ptr(dx), F, st)
             return dx
         if P == 1:
             if gm.shape[0]:
-                _lib.call("nts_scatter_add_rows", _ptr(dx), _ptr(gm), _ptr(plan.need[0]), gm.shape[0], F,
-                          cur.cuda_stream)
+                _lib.call("nts_scatter_add_rows", _ptr(dx), _ptr(gm), _ptr(plan.need[0]), gm.shape[0], F, st)
             return dx
         rows_in = [plan.send_rows[j] if j != p else plan.need[p] for j in range(P)]
         n_in = [int(r.numel()) for r in rows_in]
@@ -408,18 +389,17 @@ class GpuExchange:
         for j in range(P):
             if n_in[j]:
                 _lib.call("nts_scatter_add_rows", _ptr(dx), _ptr(recv[pos:pos + n_in[j]]), _ptr(rows_in[j]), n_in[j],
-                          F, cur.cuda_stream)
+                          F, st)
             pos += n_in[j]
         return dx
 
     # ---- backward ----------------------------------------------------------------------------------------------
     def backward(self, g, gather_dtype=None):
-        pg, plan, P, p = self.pg, self.plan, self.P, self.p
+        pg, plan = self.pg, self.plan
         bf16 = ops._check_gather_dtype(gather_dtype) is not None
         F = g.shape[1]
         dx = torch.zeros((pg.owned_vertices, F), dtype=torch.float32, device=g.device)
-        cur = torch.cuda.current_stream()
-        if P == 1:
+        if self.P == 1:
             return ops.gather_by_src_from_dst(pg.graph_chunks[0], dx, g, gather_dtype=gather_dtype)
         if self._p2p is not None:
             return self._backward_p2p(g, dx, bf16)
@@ -430,45 +410,28 @@ class GpuExchange:
         recv = self._buf("brecv", plan.send_total, F)
         send.zero_()
         self._partial_remote(send, g)
-        self.comm_stream.wait_stream(cur)
-        with torch.cuda.stream(self.comm_stream):
-            in_split = [plan.need_count[i] if i != p else 0 for i in range(P)]
-            out_split = [plan.send_count[j] if j != p else 0 for j in range(P)]
-            dist.all_to_all_single(recv, send, output_split_sizes=out_split, input_split_sizes=in_split,
-                                   group=self.group)
-        ops.gather_by_src_from_dst(pg.graph_chunks[p], dx, g)   # local chunk overlaps with the transfer
-        cur.wait_stream(self.comm_stream)
-        recv.record_stream(cur)
+        self._all_to_all(recv, send, False, lambda: ops.gather_by_src_from_dst(pg.graph_chunks[self.p], dx, g))
         if plan.send_total:  # rows repeat across senders -> vector atomics, one launch
             _lib.call("nts_scatter_add_rows_atomic", _ptr(dx), _ptr(recv), _ptr(plan.send_rows_all), plan.send_total, F,
-                      cur.cuda_stream)
+                      _lib.stream())
         return dx
 
     # ---- peer-memory transport: the C++ engine (csrc/nts_exchange.cu) --------------------------------------------------
     def _forward_p2p(self, x, y, bf16=False):
         self._p2p.reserve(x.shape[1], bf16)
-        ev = ops._timer.bracket("fwd", x.shape[1], self.pg.owned_edges, self.pg.owned_vertices) if ops._timer else None
-        if ev:
-            ev[0].record()
-        if bf16:
-            _lib.call("nts_exchange_forward_bf16", self._p2p.handle, _ptr(x), ops._DTYPE_CODE[x.dtype], _ptr(y),
-                      x.shape[1], torch.cuda.current_stream().cuda_stream)
-        else:
-            _lib.call("nts_exchange_forward", self._p2p.handle, _ptr(x), _ptr(y), x.shape[1],
-                      torch.cuda.current_stream().cuda_stream)
-        if ev:
-            ev[1].record()
+        with ops._timed("fwd", x.shape[1], self.pg.owned_edges, self.pg.owned_vertices):
+            if bf16:
+                _lib.call("nts_exchange_forward_bf16", self._p2p.handle, _ptr(x), ops._DTYPE_CODE[x.dtype], _ptr(y),
+                          x.shape[1], _lib.stream())
+            else:
+                _lib.call("nts_exchange_forward", self._p2p.handle, _ptr(x), _ptr(y), x.shape[1], _lib.stream())
         return y
 
     def _backward_p2p(self, g, dx, bf16=False):
         self._p2p.reserve(g.shape[1], bf16)
-        ev = ops._timer.bracket("bwd", g.shape[1], self.pg.owned_edges, self.pg.owned_vertices) if ops._timer else None
-        if ev:
-            ev[0].record()
-        _lib.call("nts_exchange_backward_bf16" if bf16 else "nts_exchange_backward", self._p2p.handle, _ptr(g),
-                  _ptr(dx), g.shape[1], torch.cuda.current_stream().cuda_stream)
-        if ev:
-            ev[1].record()
+        with ops._timed("bwd", g.shape[1], self.pg.owned_edges, self.pg.owned_vertices):
+            _lib.call("nts_exchange_backward_bf16" if bf16 else "nts_exchange_backward", self._p2p.handle, _ptr(g),
+                      _ptr(dx), g.shape[1], _lib.stream())
         return dx
 
 
@@ -516,9 +479,7 @@ class _PeerWindows:
         d.fwd_push_offset = self._keep["fwd_off"]
         d.bwd_push_offset = self._keep["bwd_off"]
         d.local_need, d.local_need_count = _ptr(plan.need[p]), plan.need_count[p]
-        self.handle = L.nts_exchange_create(C.byref(d))
-        if not self.handle:
-            raise _lib.NtsError("nts_exchange_create failed: " + L.nts_last_error().decode())
+        self.handle = _lib.checked(L.nts_exchange_create(C.byref(d)), "nts_exchange_create")
 
     def _cpu_collective(self):
         return dist.get_backend(self.ex.group) != "nccl"

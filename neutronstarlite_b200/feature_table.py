@@ -23,7 +23,6 @@ import torch
 import torch.distributed as dist
 
 from . import _lib
-from .sample import _DeviceArray, _stream
 
 MAX_SHARDS = 32
 
@@ -61,9 +60,7 @@ class PeerShards:
     def _alloc(self, nbytes):
         L = _lib.load()
         self._peers = []
-        self._buf = L.nts_malloc_device(max(int(nbytes), 16))
-        if not self._buf:
-            raise _lib.NtsError("nts_malloc_device failed: " + L.nts_last_error().decode(errors="replace"))
+        self._buf = _lib.checked(L.nts_malloc_device(max(int(nbytes), 16)), "nts_malloc_device")
 
     def _share(self, meta):
         """Collective: (ptrs, metas) - every rank's buffer address in this process, this rank's own first-hand, and
@@ -81,9 +78,7 @@ class PeerShards:
         for j, (hj, _) in enumerate(info):
             if j == self.rank:
                 continue
-            p = L.nts_ipc_open_handle(hj)
-            if not p:
-                raise _lib.NtsError("nts_ipc_open_handle failed: " + L.nts_last_error().decode(errors="replace"))
+            p = _lib.checked(L.nts_ipc_open_handle(hj), "nts_ipc_open_handle")
             self._peers.append(p)
             ptrs[j] = p
         return ptrs, [m for _, m in info]
@@ -149,9 +144,9 @@ class ShardedFeatureTable(PeerShards):
             if n and bf16:
                 x = x.contiguous()
                 _lib.call("nts_rows_to_bf16", x.data_ptr(), 0, self.F, self._buf, hi - lo, self.F, self.pitch,
-                          _stream())
+                          _lib.stream())
             elif n:
-                mine = torch.as_tensor(_DeviceArray(self._buf, n, "<f4"), device=self.device).view(hi - lo, self.pitch)
+                mine = _lib.borrowed(self._buf, n, torch.float32, self.device).view(hi - lo, self.pitch)
                 mine[:, self.F:].zero_()
                 mine[:, :self.F].copy_(x)
             ptrs, info = self._share((self.F, str(dtype)))
@@ -173,18 +168,7 @@ class ShardedFeatureTable(PeerShards):
         [n, pitch] BF16 rows, or with dtype=torch.float32 the rows widened exactly; a float32 table refuses a BF16
         output.  Ids outside [0, V) and a refused dtype raise NtsError before any device work."""
         self._out_dtype(dtype)
-        if torch.is_tensor(ids) and ids.is_cuda:
-            if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
-                raise _lib.NtsError("ids must be an integer tensor, not %s" % ids.dtype)
-            # range check in the caller's dtype: a cast first could wrap an int64 id >= 2^32 into [0, V)
-            if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= self.rows):
-                raise _lib.NtsError("row ids must be in [0, %d)" % self.rows)
-            t = ids.reshape(-1).to(device=self.device, dtype=torch.int32).contiguous()
-        else:
-            a = np.asarray(ids.numpy() if torch.is_tensor(ids) else ids).reshape(-1).astype(np.int64)
-            if a.size and (a.min() < 0 or a.max() >= self.rows):
-                raise _lib.NtsError("row ids must be in [0, %d)" % self.rows)
-            t = torch.from_numpy(a.astype(np.int32)).to(self.device)
+        t = _lib.device_ids(ids, self.rows, self.device, "ids", "row ids")
         return self._gather(t, dtype)
 
     def aggregate(self, out, column_offset, row_indices, weight, edge_begin, edge_end):
@@ -206,7 +190,7 @@ class ShardedFeatureTable(PeerShards):
         _lib.call("nts_segment_gather_sum_sharded", out.data_ptr(), self._shards.data_ptr(),
                   1 if self.dtype == torch.bfloat16 else 0, self._offsets.data_ptr(), self.world, self.pitch,
                   None if weight is None else weight.data_ptr(), row_indices.data_ptr(), column_offset.data_ptr(),
-                  n_rows, eb, ee, self.F, _stream())
+                  n_rows, eb, ee, self.F, _lib.stream())
         return out
 
     def _check_csc(self, out, column_offset, row_indices, weight, edge_begin, edge_end):
@@ -265,7 +249,7 @@ class ShardedFeatureTable(PeerShards):
             return out
         eb, ee = int(edge_begin), int(edge_end)
         seg = torch.empty((2, n_rows, heads), dtype=torch.float32, device=self.device)
-        st = _stream()
+        st = _lib.stream()
         _lib.call("nts_gat_softmax_stats_sharded", seg[0].data_ptr(), seg[1].data_ptr(), scores._shards.data_ptr(),
                   self._offsets.data_ptr(), self.world, scores.pitch, dst_score.data_ptr(), row_indices.data_ptr(),
                   column_offset.data_ptr(), n_rows, eb, ee, heads, float(negative_slope), st)
@@ -295,10 +279,11 @@ class ShardedFeatureTable(PeerShards):
         if self.dtype == torch.float32:
             out = torch.empty((n, self.F), dtype=torch.float32, device=self.device)
             _lib.call("nts_gather_rows_sharded", out.data_ptr(), self._shards.data_ptr(), self._offsets.data_ptr(),
-                      self.world, self.pitch, idp, n, self.F, _stream())
+                      self.world, self.pitch, idp, n, self.F, _lib.stream())
             return out
         ld = self.pitch if dtype == torch.bfloat16 else self.F
         out = torch.empty((n, ld), dtype=dtype, device=self.device)
         _lib.call("nts_gather_rows_sharded_bf16", out.data_ptr(), 1 if dtype == torch.bfloat16 else 0, ld,
-                  self._shards.data_ptr(), self._offsets.data_ptr(), self.world, self.pitch, idp, n, self.F, _stream())
+                  self._shards.data_ptr(), self._offsets.data_ptr(), self.world, self.pitch, idp, n, self.F,
+                  _lib.stream())
         return out[:, :self.F]

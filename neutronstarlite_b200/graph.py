@@ -274,7 +274,7 @@ class PartitionedGraph:
         dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         po = None if partition_offset is None else np.ascontiguousarray(partition_offset, dtype=np.uint32)
         with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream(dev).cuda_stream
+            stream = _lib.stream(dev)
             h = _lib.load().nts_graph_build_from_file(os.fsencode(path), int(vertices), int(partitions),
                                                       int(partition_id), _ptr(po), int(block_edges),
                                                       _lib_flags(dist), stream)
@@ -303,7 +303,7 @@ class PartitionedGraph:
         po = None if partition_offset is None else np.ascontiguousarray(partition_offset, dtype=np.uint32)
         dtype = 0 if src.dtype == torch.int32 else 1   # NTS_INDEX_I32 / NTS_INDEX_I64
         with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream(dev).cuda_stream
+            stream = _lib.stream(dev)
             h = _lib.load().nts_graph_build_from_device(
                 src.data_ptr() or None, dst.data_ptr() or None, dtype, int(src.numel()), int(vertices),
                 int(partitions), int(partition_id), _ptr(po),

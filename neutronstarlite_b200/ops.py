@@ -15,10 +15,7 @@ import time as _time
 import torch
 
 from . import _lib
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
+from ._lib import stream as _stream
 
 
 def row_pitched(t):
@@ -27,12 +24,18 @@ def row_pitched(t):
     return t.dim() == 2 and (t.is_contiguous() or (t.stride(1) == 1 and t.stride(0) >= t.shape[1]))
 
 
-def _check_input(t, name="input", pitched=False):
-    """pitched=True: also accept row-pitched tensors (row_pitched), for operators that pass the row pitch on."""
+_F32 = (torch.float32,)
+_F32_BF16 = (torch.float32, torch.bfloat16)
+
+
+def _check_input(t, name="input", pitched=False, dtypes=_F32):
+    """A 2-D CUDA tensor of one of `dtypes` (the gathered operand of BF16 gathers may be bfloat16 as well:
+    _gathered_dtypes).  pitched=True: also accept row-pitched tensors (row_pitched), for operators that pass the row
+    pitch on."""
     if not t.is_cuda:
         raise _lib.NtsError("%s must be a CUDA tensor (libnts_b200 has no CPU fallback)" % name)
-    if t.dtype != torch.float32 or t.dim() != 2:
-        raise _lib.NtsError("%s must be a 2-D float32 tensor" % name)
+    if t.dtype not in dtypes or t.dim() != 2:
+        raise _lib.NtsError("%s must be a 2-D %s tensor" % (name, " or ".join(str(d)[len("torch."):] for d in dtypes)))
     if not (t.is_contiguous() or (pitched and row_pitched(t))):
         # the reference borrows packed_accessor storage (core/NtsScheduler.hpp:505-515): contiguous only
         raise _lib.NtsError("%s must be contiguous" % name + (" or row-pitched" if pitched else ""))
@@ -46,17 +49,9 @@ def _check_gather_dtype(gather_dtype):
     return gather_dtype
 
 
-def _check_gathered(t, name, gather_dtype, pitched=False):
-    """_check_input for a gathered operand: with BF16 gathers a bfloat16 tensor is accepted as well (used as is)."""
-    if gather_dtype is None or (t.is_cuda and t.dtype == torch.float32):
-        return _check_input(t, name, pitched)
-    if not t.is_cuda:
-        raise _lib.NtsError("%s must be a CUDA tensor (libnts_b200 has no CPU fallback)" % name)
-    if t.dtype != torch.bfloat16 or t.dim() != 2:
-        raise _lib.NtsError("%s must be a 2-D float32 or bfloat16 tensor" % name)
-    if not (t.is_contiguous() or (pitched and row_pitched(t))):
-        raise _lib.NtsError("%s must be contiguous" % name + (" or row-pitched" if pitched else ""))
-    return t
+def _gathered_dtypes(gather_dtype):
+    """The types a gathered operand may have: float32, and with BF16 gathers bfloat16 as well (used as is)."""
+    return _F32 if gather_dtype is None else _F32_BF16
 
 
 _DTYPE_CODE = {torch.float32: 0, torch.bfloat16: 1}   # NTS_DTYPE_F32 / NTS_DTYPE_BF16 of include/nts_b200.h
@@ -148,8 +143,7 @@ class GatherPlan:
                 int(gather_rows), int(tune_for), _DTYPE_CODE[gather_dtype or torch.float32],
                 0 if tune_accumulate else PLAN_OVERWRITE, _stream())
         self.build_s = _time.perf_counter() - t0      # create synchronises the stream
-        if not self.handle:
-            raise _lib.NtsError("gather plan construction failed: " + L.nts_last_error().decode(errors="replace"))
+        _lib.checked(self.handle, "gather plan construction")
         self.slabs = int(L.nts_gather_plan_slabs(self.handle))
         hc, hr = C.c_int(0), C.c_int(0)
         _lib.call("nts_gather_plan_hubs", self.handle, C.byref(hc), C.byref(hr))
@@ -224,6 +218,16 @@ def set_plan_mode(mode, slabs=0):
     _plan_mode, _plan_slabs = mode, int(slabs)
 
 
+def _chunk_direction(chunk, direction):
+    """(offsets, indices, weight, index base, output rows, gathered rows) of one chunk direction: the CSC for "fwd"
+    (Y = A X), the CSR for "bwd" (dX = A^T dY)."""
+    if direction == "fwd":
+        return (chunk.column_offset_gpu, chunk.row_indices_gpu, chunk.edge_weight_forward_gpu, chunk.src_range[0],
+                chunk.batch_size_forward, chunk.batch_size_backward)
+    return (chunk.row_offset_gpu, chunk.column_indices_gpu, chunk.edge_weight_backward_gpu, chunk.dst_range[0],
+            chunk.batch_size_backward, chunk.batch_size_forward)
+
+
 def _chunk_plan(chunk, direction, F, gather_dtype=None):
     """The GatherPlan of one chunk direction for feature width F, or None when the plain kernel should run.
     BF16 gathers exist only in nts_gather_plan: with gather_dtype=torch.bfloat16 every chunk gets a plan, whatever its
@@ -231,10 +235,6 @@ def _chunk_plan(chunk, direction, F, gather_dtype=None):
     ForwardSingleGPUfuseOp runs them in."""
     if gather_dtype is None and (_plan_mode == "off" or (_plan_mode == "auto" and chunk.edge_size < PLAN_MIN_EDGES)):
         return None
-    if direction == "fwd":
-        n_rows, gather_rows = chunk.batch_size_forward, chunk.batch_size_backward
-    else:
-        n_rows, gather_rows = chunk.batch_size_backward, chunk.batch_size_forward
     plans = chunk.__dict__.setdefault("_gather_plans", {})      # (direction, slabs[, hub cols, hub rows]) -> plan
     tuned = chunk.__dict__.setdefault("_gather_plan_for", {})   # (direction, F[, "bf16"]) -> plan picked by measurement
     key = (direction, _plan_slabs) if _plan_slabs else (direction, "F", int(F))
@@ -242,14 +242,9 @@ def _chunk_plan(chunk, direction, F, gather_dtype=None):
         key += ("bf16",)
     plan = plans.get(key) if _plan_slabs else tuned.get(key)
     if plan is None:
-        if direction == "fwd":
-            plan = GatherPlan(chunk.column_offset_gpu, chunk.row_indices_gpu, chunk.edge_weight_forward_gpu,
-                              chunk.src_range[0], n_rows, chunk.edge_size, gather_rows, _plan_slabs, tune_for=int(F),
-                              gather_dtype=gather_dtype, tune_accumulate=False)
-        else:
-            plan = GatherPlan(chunk.row_offset_gpu, chunk.column_indices_gpu, chunk.edge_weight_backward_gpu,
-                              chunk.dst_range[0], n_rows, chunk.edge_size, gather_rows, _plan_slabs, tune_for=int(F),
-                              gather_dtype=gather_dtype, tune_accumulate=False)
+        offsets, indices, weight, index_base, n_rows, gather_rows = _chunk_direction(chunk, direction)
+        plan = GatherPlan(offsets, indices, weight, index_base, n_rows, chunk.edge_size, gather_rows, _plan_slabs,
+                          tune_for=int(F), gather_dtype=gather_dtype, tune_accumulate=False)
         share = (direction,) + plan.key()
         if share in plans:     # another width already settled on these slab and hub counts: share the arrays
             plan = plans[share]
@@ -274,45 +269,34 @@ def _plain_operands(out, x, accumulate):
     return x.contiguous()
 
 
+def _gather_chunk(direction, chunk, out, x, with_weight, gather_dtype, accumulate):
+    """One chunk direction (_chunk_direction) through its plan, or the plain kernel on the reference layout."""
+    plan = _bf16_plan(chunk, direction, x.shape[1], with_weight, gather_dtype)
+    offsets, indices, weight, _, n_rows, _ = _chunk_direction(chunk, direction)
+    with _timed(direction, x.shape[1], chunk.edge_size, n_rows):
+        if plan is not None:
+            return plan.run(x, out, gather_dtype, accumulate)
+        x = _plain_operands(out, x, accumulate)
+        # the plain entries take the CSC as (row_indices, column_offset) and the CSR as (row_offset, column_indices)
+        entry, a, b = (("nts_gather_by_dst_from_src", indices, offsets) if direction == "fwd" else
+                       ("nts_gather_by_src_from_dst", offsets, indices))
+        _lib.call(entry, _ptr(x), _ptr(out), _ptr(weight), _ptr(a), _ptr(b), chunk.src_range[0], chunk.src_range[1],
+                  chunk.dst_range[0], chunk.dst_range[1], chunk.edge_size, n_rows, int(x.shape[1]),
+                  1 if with_weight else 0, _stream())
+    return out
+
+
 def gather_by_dst_from_src(chunk, out, x, with_weight=True, gather_dtype=None, accumulate=True):
     """NtsScheduler::GatherByDstFromSrc (core/NtsScheduler.hpp:151-191) on one chunk: out += A x, or out = A x with
     accumulate=False.  x may be row-pitched (GatherPlan.run).  gather_dtype=torch.bfloat16: x (float32 or bfloat16)
     is gathered as BF16 rows with FP32 accumulation (GatherPlan.run)."""
-    plan = _bf16_plan(chunk, "fwd", x.shape[1], with_weight, gather_dtype)
-    ev = _timer.bracket("fwd", x.shape[1], chunk.edge_size, chunk.batch_size_forward) if _timer else None
-    if ev:
-        ev[0].record()
-    if plan is not None:
-        plan.run(x, out, gather_dtype, accumulate)
-    else:
-        x = _plain_operands(out, x, accumulate)
-        _lib.call("nts_gather_by_dst_from_src", _ptr(x), _ptr(out), _ptr(chunk.edge_weight_forward_gpu),
-                  _ptr(chunk.row_indices_gpu), _ptr(chunk.column_offset_gpu), chunk.src_range[0], chunk.src_range[1],
-                  chunk.dst_range[0], chunk.dst_range[1], chunk.edge_size, chunk.batch_size_forward,
-                  int(x.shape[1]), 1 if with_weight else 0, _stream())
-    if ev:
-        ev[1].record()
-    return out
+    return _gather_chunk("fwd", chunk, out, x, with_weight, gather_dtype, accumulate)
 
 
 def gather_by_src_from_dst(chunk, out, grad, with_weight=True, gather_dtype=None, accumulate=True):
     """NtsScheduler::GatherBySrcFromDst (core/NtsScheduler.hpp:257-293) on one chunk (accumulate and gather_dtype as
     in gather_by_dst_from_src: the gathered output gradient is rounded to BF16, dX accumulates in FP32)."""
-    plan = _bf16_plan(chunk, "bwd", grad.shape[1], with_weight, gather_dtype)
-    ev = _timer.bracket("bwd", grad.shape[1], chunk.edge_size, chunk.batch_size_backward) if _timer else None
-    if ev:
-        ev[0].record()
-    if plan is not None:
-        plan.run(grad, out, gather_dtype, accumulate)
-    else:
-        grad = _plain_operands(out, grad, accumulate)
-        _lib.call("nts_gather_by_src_from_dst", _ptr(grad), _ptr(out), _ptr(chunk.edge_weight_backward_gpu),
-                  _ptr(chunk.row_offset_gpu), _ptr(chunk.column_indices_gpu), chunk.src_range[0], chunk.src_range[1],
-                  chunk.dst_range[0], chunk.dst_range[1], chunk.edge_size, chunk.batch_size_backward,
-                  int(grad.shape[1]), 1 if with_weight else 0, _stream())
-    if ev:
-        ev[1].record()
-    return out
+    return _gather_chunk("bwd", chunk, out, grad, with_weight, gather_dtype, accumulate)
 
 
 class ntsGraphOp:
@@ -348,7 +332,7 @@ class ForwardSingleGPUfuseOp(ntsGraphOp):
         self.gather_dtype = _check_gather_dtype(gather_dtype)
 
     def forward(self, f_input, f_input1=None):
-        x = _check_gathered(f_input, "input", self.gather_dtype, pitched=True)
+        x = _check_input(f_input, "input", True, _gathered_dtypes(self.gather_dtype))
         c = self.partitioned_graph_.graph_chunks[0]
         y = torch.empty((c.batch_size_forward, x.shape[1]), dtype=torch.float32, device=x.device)
         return gather_by_dst_from_src(c, y, x, gather_dtype=self.gather_dtype, accumulate=False)
@@ -390,7 +374,7 @@ class MiniBatchFuseOp(ntsGraphOp):
         if self.gather_dtype is None:
             x = _check_input(f_input, "input")
         else:
-            x = _check_bf16_operand(_check_gathered(f_input, "input", self.gather_dtype, pitched=True), "input")
+            x = _check_bf16_operand(_check_input(f_input, "input", True, _F32_BF16), "input")
         if self.table and x.shape[0] < self.vertices:
             raise _lib.NtsError("the feature table has %d rows, the sampled graph has %d vertices"
                                 % (x.shape[0], self.vertices))
@@ -398,11 +382,7 @@ class MiniBatchFuseOp(ntsGraphOp):
             raise _lib.NtsError("input has %d rows, hop %d has %d sources" % (x.shape[0], self.hop, b.n_src))
         y = torch.zeros((b.n_dst, x.shape[1]), dtype=torch.float32, device=x.device)
         idx = b.row_global if self.table else b.row_indices
-        if self.gather_dtype is None:
-            with _timed("minibatch_fwd", x.shape[1], b.n_edges, b.n_dst):
-                return segment_gather_sum(y, x, b.weight, idx, b.column_offset, 0, b.n_dst, b.n_edges)
-        return segment_gather_sum_bf16(y, _bf16_rows(x, "minibatch_bf16_round"), b.weight, idx, b.column_offset,
-                                       b.n_dst, b.n_edges, "minibatch_fwd_bf16")
+        return self._k1(y, x, b.weight, idx, b.column_offset, b.n_dst, "minibatch_fwd")
 
     def backward(self, f_output_grad):
         if self.table:
@@ -412,12 +392,17 @@ class MiniBatchFuseOp(ntsGraphOp):
         if g.shape[0] != b.n_dst:
             raise _lib.NtsError("output_grad has %d rows, hop %d has %d destinations" % (g.shape[0], self.hop, b.n_dst))
         dx = torch.zeros((b.n_src, g.shape[1]), dtype=torch.float32, device=g.device)
+        return self._k1(dx, g, b.weight_backward, b.column_indices, b.row_offset, b.n_src, "minibatch_bwd")
+
+    def _k1(self, out, x, weight, indices, offsets, n_rows, tag):
+        """out += the block's gather-sum of x (K1 on FP32 rows, or on BF16 rows under tag + "_bf16")."""
+        n_edges = self.block.n_edges
         if self.gather_dtype is None:
-            with _timed("minibatch_bwd", g.shape[1], b.n_edges, b.n_src):
-                return segment_gather_sum(dx, g, b.weight_backward, b.column_indices, b.row_offset, 0, b.n_src,
-                                          b.n_edges)
-        return segment_gather_sum_bf16(dx, _bf16_rows(g, "minibatch_bf16_round"), b.weight_backward, b.column_indices,
-                                       b.row_offset, b.n_src, b.n_edges, "minibatch_bwd_bf16")
+            with _timed(tag, x.shape[1], n_edges, n_rows):
+                return segment_gather_sum(out, x, weight, indices, offsets, 0, n_rows, n_edges)
+        r = _bf16_rows(x, "minibatch_bf16_round")
+        return segment_gather_sum_bf16(out, (r, int(r.stride(0))), weight, indices, offsets, n_rows, n_edges,
+                                       tag + "_bf16")
 
 
 def _check_bf16_operand(t, name):
@@ -428,17 +413,18 @@ def _check_bf16_operand(t, name):
     return t
 
 
-def _bf16_rows(t, tag):
-    """(rows, ld): a bfloat16 t as it is, a float32 t rounded once into [n, 8*ceil(F/8)] rows (nts_rows_to_bf16)."""
+def _bf16_rows(t, tag, ld=None):
+    """A bfloat16 t as it is; a float32 t (of unit column stride) rounded once into [n, ld] BF16 rows (by default
+    ld = 8*ceil(F/8)), the columns past F zero."""
     if t.dtype == torch.bfloat16:
-        return t, int(t.stride(0))
+        return t
     n, F = t.shape
-    ld = (F + 7) // 8 * 8
+    ld = (F + 7) // 8 * 8 if ld is None else int(ld)
     r = torch.empty((n, ld), dtype=torch.bfloat16, device=t.device)
     with _timed(tag, F, 0, n):
         _lib.call("nts_rows_to_bf16", _ptr(t), _DTYPE_CODE[torch.float32], int(t.stride(0)), _ptr(r), n, F, ld,
                   _stream())
-    return r[:, :F], ld
+    return r
 
 
 def segment_gather_sum_bf16(out, rows, weight, indices, offsets, n_rows, n_edges, tag="segment_gather_sum_bf16"):
@@ -465,7 +451,7 @@ class ForwardGPUfuseOp(ntsGraphOp):
         self.exchange = exchange
 
     def forward(self, f_input, f_input1=None):
-        x = _check_gathered(f_input, "input", self.gather_dtype)
+        x = _check_input(f_input, "input", dtypes=_gathered_dtypes(self.gather_dtype))
         if self.gather_dtype is None:
             return self.exchange.forward(x)
         return self.exchange.forward(x, gather_dtype=self.gather_dtype)
@@ -634,7 +620,8 @@ class _FusedGAT:
     (column_offset[d] <= e < column_offset[d+1]) reads row slots[e] of the gathered matrix, which has n_src rows; the
     two-pass backward lists the out-edges of every row in (slot_row_offset, slot_column_indices), edges of a row in
     edge order.  forward(x, s, d) runs the statistics and the aggregation and keeps what the backward needs;
-    backward_two_pass(g, slot_row_offset, slot_column_indices) returns (dx, ds, dd)."""
+    backward_two_pass(g, slot_row_offset, slot_column_indices) and backward_one_pass(g, row_indices, mirror_index)
+    return (dx, ds, dd)."""
 
     def __init__(self, column_offset, slots, n_dst, n_src, n_edges, slope, gather_dtype):
         self.column_offset, self.slots = column_offset, slots
@@ -643,102 +630,82 @@ class _FusedGAT:
         self.saved = None
 
     def forward(self, x, s, d):
-        H = int(s.shape[1])
+        H, F = int(s.shape[1]), int(x.shape[1])
         seg_max = torch.empty((self.n_dst, H), dtype=torch.float32, device=x.device)
         seg_sum = torch.empty_like(seg_max)
-        with _timed("gat_stats", x.shape[1], self.n_edges, self.n_dst):
+        with _timed("gat_stats", F, self.n_edges, self.n_dst):
             _lib.call("nts_gat_softmax_stats", _ptr(seg_max), _ptr(seg_sum), _ptr(s), _ptr(d), _ptr(self.slots),
                       _ptr(self.column_offset), 0, self.n_dst, H, self.slope, _stream())
-        F = int(x.shape[1])
-        if self.gather_dtype is not None:
-            return self._forward_bf16(x, s, d, seg_max, seg_sum, H, F)
-        xk, Fk = x, F
-        if H == 1 and F % 4 != 0:
+        if self.gather_dtype is None:
             # odd single-head width (the 41-wide output layer of config D): gather from a copy padded to a multiple
             # of 4 columns so that the kernel uses 16-byte loads and packed virtual warps instead of 4-byte gathers
             # (11.9 -> ~4 ms per call on config D); the zero columns are dropped again below
-            Fk = (F + 3) // 4 * 4
-            xk = torch.nn.functional.pad(x, (0, Fk - F))
-        out = torch.zeros((self.n_dst, Fk), dtype=torch.float32, device=x.device)
+            ld = (F + 3) // 4 * 4 if H == 1 else F
+            rows = x if ld == F else torch.nn.functional.pad(x, (0, ld - F))
+            entry, widths = "nts_gat_fused_aggregate_forward", (ld,)
+        else:
+            # rows of ld = ceil(F/8)*8 BF16 values: 16-byte chunks of 8, and for the 41-wide layer this replaces the
+            # padded FP32 copy of the FP32 path; out shares the row stride and loses its zero pad columns below
+            ld = (F + 7) // 8 * 8
+            rows = self._to_bf16_rows(x, ld)
+            entry, widths = "nts_gat_fused_aggregate_forward_bf16", (F, ld)
+        out = torch.zeros((self.n_dst, ld), dtype=torch.float32, device=x.device)
         with _timed("gat_fwd", F, self.n_edges, self.n_dst):
-            _lib.call("nts_gat_fused_aggregate_forward", _ptr(xk), _ptr(out), _ptr(s), _ptr(d), _ptr(seg_max),
-                      _ptr(seg_sum), _ptr(self.slots), _ptr(self.column_offset), 0,
-                      self.n_dst, self.n_edges, Fk, H, self.slope, _stream())
-        if Fk != F:
+            _lib.call(entry, _ptr(rows), _ptr(out), _ptr(s), _ptr(d), _ptr(seg_max), _ptr(seg_sum), _ptr(self.slots),
+                      _ptr(self.column_offset), 0, self.n_dst, self.n_edges, *widths, H, self.slope, _stream())
+        if ld != F:
             out = out[:, :F].contiguous()
-        self.saved = (x, s, d, seg_max, seg_sum, out)
+        # what the backward gathers: x, or m~ = bf16(x) (the FP32 input is then not kept)
+        self.saved = (x if self.gather_dtype is None else rows, s, d, seg_max, seg_sum, out)
         return out
 
     @staticmethod
     def _to_bf16_rows(t, ld):
-        """bf16(t) as rows of ld values, the columns past t's width zero (nts_rows_to_bf16)."""
-        n, F = t.shape
-        r = torch.empty((n, ld), dtype=torch.bfloat16, device=t.device)
-        with _timed("gat_bf16_round", F, 0, n):
-            _lib.call("nts_rows_to_bf16", _ptr(t), _DTYPE_CODE[torch.float32], F, _ptr(r), n, F, ld, _stream())
-        return r
+        """bf16(t) as rows of ld values, the columns past t's width zero: K7's one rounding of its gathered operand."""
+        return _bf16_rows(t, "gat_bf16_round", ld)
 
-    def _forward_bf16(self, x, s, d, seg_max, seg_sum, H, F):
-        # rows of ld = ceil(F/8)*8 BF16 values: 16-byte chunks of 8, and for the 41-wide layer this replaces the
-        # padded FP32 copy of the FP32 path; out shares the row stride and loses its zero pad columns below
-        ld = (F + 7) // 8 * 8
-        mt = self._to_bf16_rows(x, ld)
-        out = torch.zeros((self.n_dst, ld), dtype=torch.float32, device=x.device)
-        with _timed("gat_fwd", F, self.n_edges, self.n_dst):
-            _lib.call("nts_gat_fused_aggregate_forward_bf16", _ptr(mt), _ptr(out), _ptr(s), _ptr(d), _ptr(seg_max),
-                      _ptr(seg_sum), _ptr(self.slots), _ptr(self.column_offset), 0, self.n_dst, self.n_edges,
-                      F, ld, H, self.slope, _stream())
-        if ld != F:
-            out = out[:, :F].contiguous()
-        self.saved = (mt, s, d, seg_max, seg_sum, out)   # m~ is what the backward gathers: the FP32 input is not kept
-        return out
-
-    def _backward_bf16(self, g, slot_off, slot_dst):
-        mt, s, d, seg_max, seg_sum, out = self.saved
-        H = int(s.shape[1])
-        M, ld = mt.shape
-        F = int(out.shape[1])
-        gt = self._to_bf16_rows(g, ld)
-        # <out, g~>, not <out, g>: the passes rely on sum_e a <m~, g~> == <out, g~>; mixing g and g~ would bias the
-        # score gradients by about 2^-8
-        out_dot_g = (out.detach() * gt[:, :F].float()).view(-1, H, F // H).sum(-1).contiguous()
-        dm = torch.zeros((M, ld), dtype=torch.float32, device=g.device)
-        ds = torch.zeros_like(s)
-        dd = torch.zeros_like(d)
-        pack = torch.empty((self.n_dst, H, 4), dtype=torch.float32, device=g.device)
-        with _timed("gat_bwd", F, 2 * self.n_edges, self.n_dst):
-            _lib.call("nts_gat_fused_aggregate_backward_two_pass_bf16", _ptr(dm), _ptr(ds), _ptr(dd), _ptr(pack),
-                      _ptr(mt), _ptr(s), _ptr(d), _ptr(seg_max), _ptr(seg_sum), _ptr(out_dot_g), _ptr(gt),
-                      _ptr(self.slots), _ptr(self.column_offset), 0, _ptr(slot_off), _ptr(slot_dst),
-                      self.n_dst, M, F, ld, H, self.slope, _stream())
-        if ld != F:
-            dm = dm[:, :F].contiguous()
-        return dm, ds, dd
-
-    def out_dot_grad(self, g):
-        """<out[d,h], g[d,h]> of the FP32 layer: sum_e a[e,h] <x[slot(e),h], g[d,h]>, so the softmax backward needs
-        no edge pass."""
-        x, s, _, _, _, out = self.saved
-        H = int(s.shape[1])
-        return (out.detach() * g).view(-1, H, x.shape[1] // H).sum(-1).contiguous()
+    def _grads(self, g):
+        """(out_dot_g, dm, ds, dd) for the gathered output gradient g (float32, or BF16 rows g~ = bf16(grad_out)):
+        out_dot_g[d, h] = <out[d,h], g[d,h]> = sum_e a[e,h] <x[slot(e),h], g[d,h]>, so the softmax backward needs no
+        edge pass, and zeroed gradients, dm as wide as the gathered rows."""
+        rows, s, d, _, _, out = self.saved
+        H, F = int(s.shape[1]), int(out.shape[1])
+        o = out.detach()
+        # <out, g~>, not <out, g>: the BF16 passes rely on sum_e a <m~, g~> == <out, g~>; mixing g and g~ would bias
+        # the score gradients by about 2^-8
+        out_dot_g = (o * (g if g.dtype == torch.float32 else g[:, :F].float())).view(-1, H, F // H).sum(-1).contiguous()
+        if rows.dtype == torch.float32:
+            dm = torch.zeros_like(rows)
+        else:
+            dm = torch.zeros(rows.shape, dtype=torch.float32, device=g.device)
+        return out_dot_g, dm, torch.zeros_like(s), torch.zeros_like(d)
 
     def backward_two_pass(self, g, slot_off, slot_dst):
         """No per-edge atomics: a destination-major and a source-major pass, each with register accumulators."""
-        if self.gather_dtype is not None:
-            return self._backward_bf16(g, slot_off, slot_dst)
+        rows, s, d, seg_max, seg_sum, out = self.saved
+        H, F = int(s.shape[1]), int(out.shape[1])
+        if self.gather_dtype is None:
+            gk, entry, widths = g, "nts_gat_fused_aggregate_backward_two_pass", (F,)
+        else:
+            gk = self._to_bf16_rows(g, rows.shape[1])
+            entry, widths = "nts_gat_fused_aggregate_backward_two_pass_bf16", (F, int(rows.shape[1]))
+        out_dot_g, dm, ds, dd = self._grads(gk)
+        pack = torch.empty((self.n_dst, H, 4), dtype=torch.float32, device=g.device)
+        with _timed("gat_bwd", F, 2 * self.n_edges, self.n_dst):
+            _lib.call(entry, _ptr(dm), _ptr(ds), _ptr(dd), _ptr(pack), _ptr(rows), _ptr(s), _ptr(d), _ptr(seg_max),
+                      _ptr(seg_sum), _ptr(out_dot_g), _ptr(gk), _ptr(self.slots), _ptr(self.column_offset), 0,
+                      _ptr(slot_off), _ptr(slot_dst), self.n_dst, rows.shape[0], *widths, H, self.slope, _stream())
+        if dm.shape[1] != F:
+            dm = dm[:, :F].contiguous()
+        return dm, ds, dd
+
+    def backward_one_pass(self, g, row_indices, mirror_index):
+        """The FP32 backward with per-edge atomics, on the CSC's row_indices and their mirror slots."""
         x, s, d, seg_max, seg_sum, out = self.saved
-        H = int(s.shape[1])
-        out_dot_g = self.out_dot_grad(g)
-        dm = torch.zeros_like(x)
-        ds = torch.zeros_like(s)
-        dd = torch.zeros_like(d)
-        pack = torch.empty((self.n_dst, H, 4), dtype=torch.float32, device=x.device)
-        with _timed("gat_bwd", x.shape[1], 2 * self.n_edges, self.n_dst):
-            _lib.call("nts_gat_fused_aggregate_backward_two_pass", _ptr(dm), _ptr(ds), _ptr(dd), _ptr(pack),
-                      _ptr(x), _ptr(s), _ptr(d), _ptr(seg_max), _ptr(seg_sum), _ptr(out_dot_g), _ptr(g),
-                      _ptr(self.slots), _ptr(self.column_offset), 0,
-                      _ptr(slot_off), _ptr(slot_dst), self.n_dst, x.shape[0], x.shape[1], H, self.slope,
-                      _stream())
+        out_dot_g, dm, ds, dd = self._grads(g)
+        _lib.call("nts_gat_fused_aggregate_backward", _ptr(dm), _ptr(ds), _ptr(dd), _ptr(x), _ptr(s), _ptr(d),
+                  _ptr(seg_max), _ptr(seg_sum), _ptr(out_dot_g), _ptr(g), _ptr(row_indices), _ptr(self.column_offset),
+                  _ptr(mirror_index), self.n_dst, x.shape[1], int(s.shape[1]), self.slope, _stream())
         return dm, ds, dd
 
 
@@ -815,17 +782,7 @@ class DistGPUFusedGATOp(_EdgeOp):
         g = _check_input(f_output_grad, "output_grad")
         if self.two_pass_backward:
             return self._k7.backward_two_pass(g, *self.slot_csr(pg))
-        x, s, d, seg_max, seg_sum, out = self._k7.saved
-        H = int(s.shape[1])
-        out_dot_g = self._k7.out_dot_grad(g)
-        dm = torch.zeros_like(x)
-        ds = torch.zeros_like(s)
-        dd = torch.zeros_like(d)
-        _lib.call("nts_gat_fused_aggregate_backward", _ptr(dm), _ptr(ds), _ptr(dd), _ptr(x), _ptr(s), _ptr(d),
-                  _ptr(seg_max), _ptr(seg_sum), _ptr(out_dot_g), _ptr(g), _ptr(pg.row_indices_gpu),
-                  _ptr(pg.column_offset_gpu), _ptr(pg.mirror_index_gpu), pg.owned_vertices, x.shape[1], H,
-                  self.slope, _stream())
-        return dm, ds, dd
+        return self._k7.backward_one_pass(g, pg.row_indices_gpu, pg.mirror_index_gpu)
 
 
 # the refusal of nts_gat_fused_aggregate_forward_bf16 (check_gat_bf16_layout) for a head width D % 8 != 0
@@ -845,7 +802,7 @@ def gat_bf16_shape_error(feature_size, heads):
     for name, n_ptrs in (("nts_gat_fused_aggregate_forward_bf16", 9),
                          ("nts_gat_fused_aggregate_backward_two_pass_bf16", 16)):
         if getattr(lib, name)(*([None] * n_ptrs), 0, 0, F, ld, H, 0.2, None) != 0:
-            return "%s: %s" % (name, lib.nts_last_error().decode(errors="replace"))
+            return "%s: %s" % (name, _lib.last_error())
     return None
 
 

@@ -30,18 +30,6 @@ MAX_FANOUT = 64
 MAX_HOPS = 8
 
 
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-class _DeviceArray:
-    """A borrowed 1-D device array for torch.as_tensor (the CUDA array interface; no copy, no stream sync)."""
-
-    def __init__(self, ptr, n, typestr):
-        self.__cuda_array_interface__ = {"shape": (int(n),), "typestr": typestr, "data": (int(ptr), False),
-                                         "version": 2, "strides": None}
-
-
 class SampledBlock:
     """One hop of a sample (the reference's sampled_sgs[hop]).
 
@@ -121,7 +109,7 @@ def transpose(column_offset, row_indices, weight, n_dst, n_src):
             raise _lib.NtsError("block arrays must be contiguous CUDA tensors")
     _lib.call("nts_sample_transpose", column_offset.data_ptr(), row_indices.data_ptr(), weight.data_ptr(),
               int(n_dst), int(n_src), n_edges, row_offset.data_ptr(), column_indices.data_ptr(),
-              weight_backward.data_ptr(), _stream())
+              weight_backward.data_ptr(), _lib.stream())
     return row_offset, column_indices, weight_backward
 
 
@@ -166,9 +154,9 @@ class NeighborSampler:
             n = len(pg.offsets) - 1
             cols, rows, ws = ((C.c_void_p * n)(*a) for a in pg.shard_arrays)
             offs = (C.c_uint32 * (n + 1))(*[int(o) for o in pg.offsets])
-            self.handle = L.nts_sampler_create_sharded(cols, rows, ws, offs, n, self.max_seeds, len(self.fanout), ks,
-                                                       flags, _stream())
-            what = "nts_sampler_create_sharded"
+            self.handle = _lib.checked(L.nts_sampler_create_sharded(cols, rows, ws, offs, n, self.max_seeds,
+                                                                    len(self.fanout), ks, flags, _lib.stream()),
+                                       "nts_sampler_create_sharded")
         else:
             c = pg.graph_chunks[0]
             if c.column_offset_gpu is None:
@@ -176,12 +164,12 @@ class NeighborSampler:
             self.V = int(pg.global_vertices)
             self.device = c.column_offset_gpu.device
             self._graph = (c.column_offset_gpu, c.row_indices_gpu, c.edge_weight_forward_gpu)
-            self.handle = L.nts_sampler_create_ex(c.column_offset_gpu.data_ptr(), c.row_indices_gpu.data_ptr(),
-                                                  c.edge_weight_forward_gpu.data_ptr(), self.V, int(c.edge_size),
-                                                  self.max_seeds, len(self.fanout), ks, flags, _stream())
-            what = "nts_sampler_create_ex"
-        if not self.handle:
-            raise _lib.NtsError(what + " failed: " + L.nts_last_error().decode(errors="replace"))
+            self.handle = _lib.checked(L.nts_sampler_create_ex(c.column_offset_gpu.data_ptr(),
+                                                               c.row_indices_gpu.data_ptr(),
+                                                               c.edge_weight_forward_gpu.data_ptr(), self.V,
+                                                               int(c.edge_size), self.max_seeds, len(self.fanout), ks,
+                                                               flags, _lib.stream()),
+                                       "nts_sampler_create_ex")
 
     def bytes(self):
         return int(_lib.load().nts_sampler_bytes(self.handle))
@@ -189,18 +177,7 @@ class NeighborSampler:
     def _seeds(self, seeds):
         """Seeds as a contiguous int32 device tensor; ids are checked against V before any device work when they
         are given on the host (numpy, list, CPU tensor)."""
-        if torch.is_tensor(seeds) and seeds.is_cuda:
-            if seeds.dtype.is_floating_point or seeds.dtype.is_complex or seeds.dtype == torch.bool:
-                raise _lib.NtsError("seeds must be an integer tensor, not %s" % seeds.dtype)
-            # range check in the caller's dtype: a cast first could wrap an int64 id >= 2^32 into [0, V)
-            if seeds.numel() and (int(seeds.min()) < 0 or int(seeds.max()) >= self.V):
-                raise _lib.NtsError("seed vertex ids must be in [0, %d)" % self.V)
-            t = seeds.reshape(-1).to(torch.int32).contiguous()
-        else:
-            a = np.asarray(seeds.numpy() if torch.is_tensor(seeds) else seeds).reshape(-1).astype(np.int64)
-            if a.size and (a.min() < 0 or a.max() >= self.V):
-                raise _lib.NtsError("seed vertex ids must be in [0, %d)" % self.V)
-            t = torch.from_numpy(a.astype(np.int32)).to(self.device)
+        t = _lib.device_ids(seeds, self.V, self.device, "seeds", "seed vertex ids")
         if t.numel() > self.max_seeds:
             raise _lib.NtsError("%d seeds, the sampler was created for at most %d" % (t.numel(), self.max_seeds))
         return t
@@ -209,17 +186,15 @@ class NeighborSampler:
         """The SampledSubgraph of `seeds` for (seed, step)."""
         s = self._seeds(seeds)
         _lib.call("nts_sampler_sample", self.handle, s.data_ptr() if s.numel() else None, int(s.numel()),
-                  int(seed) & 0xFFFFFFFFFFFFFFFF, int(step) & 0xFFFFFFFFFFFFFFFF, _stream())
+                  int(seed) & 0xFFFFFFFFFFFFFFFF, int(step) & 0xFFFFFFFFFFFFFFFF, _lib.stream())
         return SampledSubgraph([self._view(h) for h in range(len(self.fanout))], owner=self, vertices=self.V)
 
     def _view(self, hop):
         v = _lib.SampleHopView()
         _lib.call("nts_sampler_hop_view", self.handle, int(hop), C.byref(v))
 
-        def arr(ptr, n, typestr="<i4"):
-            if n == 0:
-                return torch.empty(0, dtype=torch.int32 if typestr == "<i4" else torch.float32, device=self.device)
-            return torch.as_tensor(_DeviceArray(ptr, n, typestr), device=self.device)
+        def arr(ptr, n, dtype=torch.int32):
+            return _lib.borrowed(ptr, n, dtype, self.device)
 
         nd, ns, ne = int(v.n_dst), int(v.n_src), int(v.n_edges)
         dst_pos = None
@@ -228,8 +203,8 @@ class NeighborSampler:
             _lib.call("nts_sampler_hop_dst_pos", self.handle, int(hop), C.byref(p))
             dst_pos = arr(p.value, nd)
         return SampledBlock(arr(v.dst, nd), arr(v.column_offset, nd + 1), arr(v.row_indices, ne),
-                            arr(v.weight, ne, "<f4"), arr(v.src, ns), arr(v.row_offset, ns + 1),
-                            arr(v.column_indices, ne), arr(v.weight_backward, ne, "<f4"), arr(v.row_global, ne),
+                            arr(v.weight, ne, torch.float32), arr(v.src, ns), arr(v.row_offset, ns + 1),
+                            arr(v.column_indices, ne), arr(v.weight_backward, ne, torch.float32), arr(v.row_global, ne),
                             dst_pos)
 
     def __del__(self):

@@ -80,11 +80,9 @@ class Parameter:
         used by the CPU tests (same arithmetic, pinned to the reference's golden vectors in tests/test_adam.py)."""
         with torch.no_grad():
             if self.W.is_cuda:
-                from . import _lib
                 _lib.call("nts_adam_update", self.W.data_ptr(), self.M.data_ptr(), self.V.data_ptr(),
                           self.W_gradient.data_ptr(), self.W.numel(), float(self.weight_decay), float(self.beta1),
-                          float(self.beta2), float(self.alpha), float(self.epsilon),
-                          torch.cuda.current_stream().cuda_stream)
+                          float(self.beta2), float(self.alpha), float(self.epsilon), _lib.stream())
                 return
             one = np.float32(1)
             W_g = self.W * float(self.weight_decay) + self.W_gradient
@@ -96,7 +94,52 @@ class Parameter:
         self.W.grad = None
 
 
-class GCNImpl:
+def _parameters(shapes, seed, device, learn_rate, weight_decay, decay=None):
+    """One Parameter per (w, h) of `shapes`, in order: the generator seeded with `seed` draws them and rank 0's values
+    are broadcast in that order.  decay = (decay_rate, decay_epoch) for Parameter.set_decay; None keeps Adam's
+    defaults (no decay)."""
+    gen = torch.Generator().manual_seed(seed)
+    params = []
+    for w, h in shapes:
+        p = Parameter(w, h, learn_rate, 0.9, 0.999, 1e-9, weight_decay, device=device, generator=gen)
+        p.init_parameter()
+        if decay is not None:
+            p.set_decay(*decay)
+        params.append(p)
+    return params
+
+
+def _update(params, zero_fill_missing):
+    """all_reduce_to_gradient, Adam and next() for every parameter.  A parameter without a gradient is skipped, or with
+    zero_fill_missing reduced and stepped as zeros (data-parallel rounds: the collectives are then the same on every
+    rank)."""
+    for p in params:
+        g = p.W.grad
+        if g is None:
+            if not zero_fill_missing:
+                continue
+            g = torch.zeros_like(p.W)
+        p.all_reduce_to_gradient(g)
+        p.learn_with_decay_Adam()
+        p.next()
+
+
+class _FullGraph:
+    """The loss and update of the full-graph models."""
+
+    def Loss(self):
+        """GCN.hpp:198-207: nll_loss over the local train rows (mean)."""
+        a = self.X[-1]
+        self.loss = torch.nn.functional.nll_loss(a.index_select(0, self.train_rows),
+                                                 self.L_GT.index_select(0, self.train_rows))
+        self.ctx.appendNNOp(a, self.loss)
+
+    def Update(self):
+        """GCN.hpp:209-215."""
+        _update(self.params(), False)
+
+
+class GCNImpl(_FullGraph):
     """toolkits/GCN.hpp:33-354.  `layers` = LAYERS of the cfg, e.g. [602, 128, 41].
 
     gather_dtype=torch.bfloat16: every aggregation gathers its operand as BF16 rows with FP32 accumulation (the
@@ -116,14 +159,8 @@ class GCNImpl:
         self.device = features.device
         self.drop_rate = drop_rate
         self.ctx = NtsContext()
-        gen = torch.Generator().manual_seed(seed)
-        self.P = []
-        for i in range(len(self.layers) - 1):
-            p = Parameter(self.layers[i], self.layers[i + 1], learn_rate, 0.9, 0.999, 1e-9, weight_decay,
-                          device=self.device, generator=gen)
-            p.init_parameter()
-            p.set_decay(decay_rate, decay_epoch)
-            self.P.append(p)
+        self.P = _parameters(zip(self.layers, self.layers[1:]), seed, self.device, learn_rate, weight_decay,
+                             (decay_rate, decay_epoch))
         self.L_GT = labels.to(self.device)
         self.MASK = mask.to(self.device)
         self.train_rows = (self.MASK == 0).nonzero().view(-1)
@@ -150,6 +187,9 @@ class GCNImpl:
         self.loss = None
         self.epoch = 0
 
+    def params(self):
+        return self.P
+
     def vertexForward(self, a, x, layer):
         """GCN.hpp:183-196."""
         if layer < len(self.layers) - 2:
@@ -170,20 +210,6 @@ class GCNImpl:
                 x_i = x_i.contiguous()
             y_i = self.ctx.runGraphOp(self.op_class, self.pg, None, x_i, **self.op_kwargs)
             self.X[i + 1] = self.ctx.runVertexForward(lambda n, v, _l=i: self.vertexForward(n, v, _l), y_i, x_i)
-
-    def Loss(self):
-        """GCN.hpp:198-207: nll_loss over the local train rows (mean)."""
-        a = self.X[-1]
-        self.loss = torch.nn.functional.nll_loss(a.index_select(0, self.train_rows),
-                                                 self.L_GT.index_select(0, self.train_rows))
-        self.ctx.appendNNOp(a, self.loss)
-
-    def Update(self):
-        """GCN.hpp:209-215."""
-        for p in self.P:
-            p.all_reduce_to_gradient(p.W.grad)
-            p.learn_with_decay_Adam()
-            p.next()
 
     def Test(self, s):
         """GCN.hpp:150-181: accuracy over mask == s, summed over ranks."""
@@ -268,6 +294,31 @@ class _SampledRounds:
     way.  A topology sharded over N > 1 ranks needs a ShardedFeatureTable over the same ranks (its offsets may
     differ)."""
 
+    def _init_rounds(self, partitioned_graph, layers, features, labels, mask, fanout, batch_size, sample_seed,
+                     gather_dtype, include_dst, log_softmax_in_loss, retain_tape):
+        """The set-up both models share.  What differs is passed in: include_dst for the sampler, log_softmax_in_loss
+        (Forward returns logits, not log-probabilities) and retain_tape (self_backward's retain_graph)."""
+        self.layers = list(layers)
+        self.gather_dtype = ops._check_gather_dtype(gather_dtype)
+        if len(fanout) != len(self.layers) - 1:
+            raise _lib.NtsError("fanout needs one entry per layer (%d), got %d" % (len(self.layers) - 1, len(fanout)))
+        self.batch_size = int(batch_size)
+        if self.batch_size < 1:
+            raise _lib.NtsError("batch_size must be >= 1")
+        from .sample import NeighborSampler
+        self.sampler = NeighborSampler(partitioned_graph, fanout, self.batch_size, include_dst=include_dst)
+        self._init_features(features, self.sampler.V, partitioned_graph)
+        self.sample_seed = int(sample_seed)
+        self.step = 0
+        self.ctx = NtsContext()
+        self.L_GT = labels.to(self.device)
+        mask = torch.as_tensor(mask).cpu()
+        self.nids = [(mask == s).nonzero().view(-1) for s in (0, 1, 2)]    # train / val / test ids, ascending
+        self.subgraph = None
+        self.loss = None
+        self.epoch = 0
+        self._log_softmax_in_loss, self._retain_tape = log_softmax_in_loss, retain_tape
+
     def _init_features(self, features, vertices, topology):
         from .feature_table import ShardedFeatureTable
         from .topology import ShardedTopology
@@ -324,15 +375,28 @@ class _SampledRounds:
         """all_reduce_to_gradient, Adam and next() for every parameter.  At world 1 a parameter without a gradient is
         skipped; data-parallel, every rank reduces and steps every parameter (a missing gradient counts as zeros), so
         that the collectives are the same on every rank."""
+        _update(self.params(), self.world > 1)
+
+    def Loss(self, out, seeds_dev):
+        """GCN_CPU_SAMPLE.hpp:187-195: nll_loss over the batch's seeds, after log_softmax where Forward returns
+        logits."""
+        self.loss = torch.nn.functional.nll_loss(out.log_softmax(1) if self._log_softmax_in_loss else out,
+                                                 self.L_GT.index_select(0, seeds_dev))
+        self.ctx.appendNNOp(out, self.loss)
+        return self.loss
+
+    def train_step(self, seeds):
+        """One batch: zero the gradients, sample, forward, loss, tape backward, Adam.  Returns (loss, correct)."""
         for p in self.params():
-            g = p.W.grad
-            if g is None:
-                if self.world == 1:
-                    continue
-                g = torch.zeros_like(p.W)
-            p.all_reduce_to_gradient(g)
-            p.learn_with_decay_Adam()
-            p.next()
+            p.zero_grad()
+        self.ctx.train()
+        out = self.Forward(seeds, True)
+        seeds_dev = self.subgraph.seeds().long()
+        loss = self.Loss(out, seeds_dev)
+        correct = (out.argmax(1) == self.L_GT.index_select(0, seeds_dev)).sum()
+        self.ctx.self_backward(self._retain_tape)
+        self.Update()
+        return loss.detach(), correct
 
     def evaluate(self, s):
         """Accuracy over mask == s from sampled forwards (no dropout, no update)."""
@@ -348,39 +412,34 @@ class _SampledRounds:
         return self._totals(correct)[0] / max(ids.numel(), 1)
 
     def _own_csc(self):
-        """(lo, hi, own_offsets, parts): this rank's destinations [lo, hi), the ownership offsets the per-layer tables
-        are built on, and the in-edge CSC pieces that cover [lo, hi) in order, as (column offsets [n + 1] int32,
-        row_indices, weight, edge_begin, edge_end) - a ShardedTopology's shards held in this process (all of them
-        after split()), or the slice [lo, hi) of the replicated single-partition CSC."""
-        from .sample import _DeviceArray
+        """(lo, hi, own_offsets, group, parts): this rank's destinations [lo, hi), the ownership offsets and process
+        group the per-layer tables are built on, and the in-edge CSC pieces that cover [lo, hi) in order, as (rows,
+        column offsets [n + 1] int32, row_indices, weight, edge_begin, edge_end), `rows` the piece's slice of [lo, hi)
+        counted from lo - a ShardedTopology's shards held in this process (all of them after split()), or the slice
+        [lo, hi) of the replicated single-partition CSC."""
         from .topology import ShardedTopology
         topo = self.sampler._graph
-        dev = self.device
-
-        def borrowed(ptr, n, typestr):
-            if n == 0:
-                return torch.empty(0, dtype=torch.float32 if typestr == "<f4" else torch.int32, device=dev)
-            return torch.as_tensor(_DeviceArray(ptr, n, typestr), device=dev)
-
+        group = None if self.table is None else self.table.group
         if isinstance(topo, ShardedTopology):
             if topo._buf is None:
                 raise _lib.NtsError("the topology is closed")
             off = [int(o) for o in topo.offsets]
             mine = range(len(off) - 1) if topo.world == 1 else [topo.rank]
+            lo, hi = off[mine[0]], off[mine[-1] + 1]
             parts = []
             for o in mine:
-                col = borrowed(topo.shard_arrays[0][o], off[o + 1] - off[o] + 1, "<i4")
+                col = _lib.borrowed(topo.shard_arrays[0][o], off[o + 1] - off[o] + 1, torch.int32, self.device)
                 n_edges = int(col[-1])
-                parts.append((col, borrowed(topo.shard_arrays[1][o], n_edges, "<i4"),
-                              borrowed(topo.shard_arrays[2][o], n_edges, "<f4"), 0, n_edges))
-            lo, hi = off[mine[0]], off[mine[-1] + 1]
-            return lo, hi, (off if topo.world > 1 else [0, off[-1]]), parts
+                parts.append((slice(off[o] - lo, off[o + 1] - lo), col,
+                              _lib.borrowed(topo.shard_arrays[1][o], n_edges, torch.int32, self.device),
+                              _lib.borrowed(topo.shard_arrays[2][o], n_edges, torch.float32, self.device), 0, n_edges))
+            return lo, hi, (off if topo.world > 1 else [0, off[-1]]), group, parts
         c_col, c_row, c_w = topo
         own = [0, self.sampler.V] if self.table is None else [int(o) for o in self.table.offsets]
         lo, hi = own[self.rank], own[self.rank + 1]
         col = c_col[lo:hi + 1]
         eb, ee = (int(e) & 0xFFFFFFFF for e in col[[0, -1]].tolist())
-        return lo, hi, own, [(col, c_row, c_w, eb, ee)]
+        return lo, hi, own, group, [(slice(0, hi - lo), col, c_row, c_w, eb, ee)]
 
     def evaluate_full(self, s):
         """Accuracy over mask == s from the model's infer(): each rank counts its own rows and the counts are summed
@@ -448,37 +507,14 @@ class GCNSampleImpl(_SampledRounds):
     def __init__(self, partitioned_graph, layers, features, labels, mask, fanout, batch_size, learn_rate=0.01,
                  weight_decay=0.0001, decay_rate=0.97, decay_epoch=100, drop_rate=0.5, seed=0, sample_seed=0,
                  gather_dtype=None):
-        self.layers = list(layers)
-        self.gather_dtype = ops._check_gather_dtype(gather_dtype)
-        if len(fanout) != len(self.layers) - 1:
-            raise _lib.NtsError("fanout needs one entry per layer (%d), got %d" % (len(self.layers) - 1, len(fanout)))
-        self.batch_size = int(batch_size)
-        if self.batch_size < 1:
-            raise _lib.NtsError("batch_size must be >= 1")
-        from .sample import NeighborSampler
-        self.sampler = NeighborSampler(partitioned_graph, fanout, self.batch_size)
-        self._init_features(features, self.sampler.V, partitioned_graph)
+        self._init_rounds(partitioned_graph, layers, features, labels, mask, fanout, batch_size, sample_seed,
+                          gather_dtype, include_dst=False, log_softmax_in_loss=True, retain_tape=False)
         self.features16 = None
         if self.gather_dtype is not None and self.table is None:
-            self.features16 = ops._bf16_rows(self.features, "minibatch_bf16_round")[0]
+            self.features16 = ops._bf16_rows(self.features, "minibatch_bf16_round")[:, :self.features.shape[1]]
         self.drop_rate = drop_rate
-        self.sample_seed = int(sample_seed)
-        self.step = 0
-        self.ctx = NtsContext()
-        gen = torch.Generator().manual_seed(seed)
-        self.P = []
-        for i in range(len(self.layers) - 1):
-            p = Parameter(self.layers[i], self.layers[i + 1], learn_rate, 0.9, 0.999, 1e-9, weight_decay,
-                          device=self.device, generator=gen)
-            p.init_parameter()
-            p.set_decay(decay_rate, decay_epoch)
-            self.P.append(p)
-        self.L_GT = labels.to(self.device)
-        mask = torch.as_tensor(mask).cpu()
-        self.nids = [(mask == s).nonzero().view(-1) for s in (0, 1, 2)]    # train / val / test ids, ascending
-        self.subgraph = None
-        self.loss = None
-        self.epoch = 0
+        self.P = _parameters(zip(self.layers, self.layers[1:]), seed, self.device, learn_rate, weight_decay,
+                             (decay_rate, decay_epoch))
 
     def params(self):
         return self.P
@@ -508,25 +544,6 @@ class GCNSampleImpl(_SampledRounds):
                 x = self.ctx.runVertexForward(lambda n, _l=l: torch.relu(self.P[_l].forward(n)), y)
         return x
 
-    def Loss(self, out, seeds_dev):
-        """GCN_CPU_SAMPLE.hpp:187-195: log_softmax + nll_loss over the batch's seeds."""
-        self.loss = torch.nn.functional.nll_loss(out.log_softmax(1), self.L_GT.index_select(0, seeds_dev))
-        self.ctx.appendNNOp(out, self.loss)
-        return self.loss
-
-    def train_step(self, seeds):
-        """One batch: zero the gradients, sample, forward, loss, tape backward, Adam.  Returns (loss, correct)."""
-        for p in self.P:
-            p.zero_grad()
-        self.ctx.train()
-        out = self.Forward(seeds, True)
-        seeds_dev = self.subgraph.seeds().long()
-        loss = self.Loss(out, seeds_dev)
-        correct = (out.argmax(1) == self.L_GT.index_select(0, seeds_dev)).sum()
-        self.ctx.self_backward(False)
-        self.Update()
-        return loss.detach(), correct
-
     @torch.no_grad()
     def infer(self):
         """Full-neighbour inference: collective over the ranks of the model's table.  Returns (lo, out), out the last
@@ -545,8 +562,7 @@ class GCNSampleImpl(_SampledRounds):
         any more; both are collective, and every table is closed before infer returns.  A rank without destinations
         joins every collective.  Neither the sampler, the step counter, the tape nor any gradient is touched."""
         from .feature_table import ShardedFeatureTable
-        lo, hi, own, parts = self._own_csc()
-        group = None if self.table is None else self.table.group
+        lo, hi, own, group, parts = self._own_csc()
         dtype = self.gather_dtype or torch.float32
         L = len(self.layers) - 1
         x = None
@@ -564,15 +580,12 @@ class GCNSampleImpl(_SampledRounds):
             else:
                 src = ShardedFeatureTable(x.contiguous(), own, group, dtype=dtype)
             y = torch.zeros((hi - lo, src.F), dtype=torch.float32, device=self.device)
-            row0 = 0
             scale = []
-            for col, rows, w, eb, ee in parts:
-                n = col.numel() - 1
-                src.aggregate(y[row0:row0 + n], col, rows, w, eb, ee)
+            for r, col, rows, w, eb, ee in parts:
+                src.aggregate(y[r], col, rows, w, eb, ee)
                 c = col.long() & 0xFFFFFFFF
                 deg = (c[1:] - c[:-1]).double()
                 scale.append(torch.where(deg > k, k / deg.clamp_min(1), torch.ones_like(deg)))
-                row0 += n
             if src is not self.table:
                 src.close()
             y.mul_(torch.cat(scale).float().unsqueeze(1))
@@ -582,7 +595,7 @@ class GCNSampleImpl(_SampledRounds):
         return lo, x
 
 
-class GATImpl:
+class GATImpl(_FullGraph):
     """Multi-head GAT on the fused aggregation path - the flow of toolkits/GAT_CPU_DIST_OPTM.hpp:196-241 (per-vertex
     attention scores -> [E, H] edge logits -> edge softmax -> DistAggregateDstFuseWeight) on the GPU operators, with
     H heads (the reference has one).  `layers` are total widths, e.g. [602, 64, 64, 41] with heads=8 gives hidden
@@ -605,22 +618,11 @@ class GATImpl:
             raise _lib.NtsError("GATImpl gather_dtype needs fused_kernel=True and two_pass_backward=True")
         self.layers = list(layers)
         self.device = features.device
-        self.heads = [heads] * (len(self.layers) - 2) + [1]
-        if self.gather_dtype is not None:
-            _refuse_bf16_gat_layers(self.layers, self.heads)
+        self.heads = _gat_heads(self.layers, heads, self.gather_dtype)
         self.ctx = NtsContext(sum_fanout_grads=sum_fanout_grads)
-        gen = torch.Generator().manual_seed(seed)
-        self.P, self.al, self.ar = [], [], []
-        for i in range(len(self.layers) - 1):
-            H = self.heads[i]
-            D = self.layers[i + 1] // H
-            assert H * D == self.layers[i + 1], "layer width must be a multiple of heads"
-            mk = lambda a, b: Parameter(a, b, learn_rate, 0.9, 0.999, 1e-9, weight_decay, device=self.device,
-                                        generator=gen)
-            for lst, shape in ((self.P, (self.layers[i], H * D)), (self.al, (H, D)), (self.ar, (H, D))):
-                prm = mk(*shape)
-                prm.init_parameter()
-                lst.append(prm)
+        # GATImpl's Adam keeps its defaults: no learning-rate decay
+        self.P, self.al, self.ar = _gat_parameters(self.layers, self.heads, seed, self.device, learn_rate,
+                                                   weight_decay)
         if exchange is None:
             from .exchange import GpuExchange
             exchange = GpuExchange(partitioned_graph)
@@ -639,15 +641,11 @@ class GATImpl:
     def Forward(self):
         ctx, pg = self.ctx, self.pg
         for i in range(len(self.layers) - 1):
-            H = self.heads[i]
-            D = self.layers[i + 1] // H
             last = i == len(self.layers) - 2
             X_trans = ctx.runVertexForward(lambda x, _i=i: self.P[_i].forward(x), self.X[i])
             mirror = ctx.runGraphOp(ops.DistGPUGetDepNbrOp, pg, None, X_trans.contiguous(), exchange=self.exchange)
-            src_att = ctx.runVertexForward(
-                lambda m, _i=i: (m.view(-1, H, D) * self.al[_i].W).sum(-1).contiguous(), mirror)
-            dst_att = ctx.runVertexForward(
-                lambda x, _i=i: (x.view(-1, H, D) * self.ar[_i].W).sum(-1).contiguous(), X_trans)
+            src_att = ctx.runVertexForward(lambda m, _i=i: _head_scores(m, self.al[_i].W), mirror)
+            dst_att = ctx.runVertexForward(lambda x, _i=i: _head_scores(x, self.ar[_i].W), X_trans)
             if self.fused_kernel:
                 nbr = ctx.runGraphOpN(ops.DistGPUFusedGATOp, pg, None, [mirror, src_att, dst_att],
                                       two_pass_backward=self.two_pass_backward, gather_dtype=self.gather_dtype)
@@ -663,20 +661,6 @@ class GATImpl:
             else:
                 self.X[i + 1] = ctx.runVertexForward(lambda t: torch.relu(t), nbr)
 
-    def Loss(self):
-        a = self.X[-1]
-        self.loss = torch.nn.functional.nll_loss(a.index_select(0, self.train_rows),
-                                                 self.L_GT.index_select(0, self.train_rows))
-        self.ctx.appendNNOp(a, self.loss)
-
-    def Update(self):
-        for p in self.params():
-            if p.W.grad is None:
-                continue
-            p.all_reduce_to_gradient(p.W.grad)
-            p.learn_with_decay_Adam()
-            p.next()
-
     def run_epoch(self):
         if self.epoch != 0:
             for p in self.params():
@@ -689,14 +673,37 @@ class GATImpl:
         return self.loss
 
 
-def _refuse_bf16_gat_layers(layers, heads):
-    """NtsError, before any device work, for the first layer whose shape a BF16 K7 entry refuses (the backward has no
-    fallback, so such a layer would otherwise run a whole forward and fail at its first backward)."""
+def _gat_heads(layers, heads, gather_dtype):
+    """The heads of each layer: `heads` on the hidden layers, one on the output layer.  NtsError, before any device
+    work, for a width that is not a multiple of its heads, and with BF16 gathers for the first layer whose shape a BF16
+    K7 entry refuses (the backward has no fallback, so such a layer would otherwise run a whole forward and fail at its
+    first backward)."""
+    heads = [heads] * (len(layers) - 2) + [1]
     for i, H in enumerate(heads):
-        why = ops.gat_bf16_shape_error(layers[i + 1], H)
-        if why is not None:
-            raise _lib.NtsError("layer %d (width %d, %d heads) cannot gather BF16 rows: %s"
-                                % (i, layers[i + 1], H, why))
+        if layers[i + 1] % H:
+            raise _lib.NtsError("layer width %d is not a multiple of %d heads" % (layers[i + 1], H))
+    if gather_dtype is not None:
+        for i, H in enumerate(heads):
+            why = ops.gat_bf16_shape_error(layers[i + 1], H)
+            if why is not None:
+                raise _lib.NtsError("layer %d (width %d, %d heads) cannot gather BF16 rows: %s"
+                                    % (i, layers[i + 1], H, why))
+    return heads
+
+
+def _gat_parameters(layers, heads, seed, device, learn_rate, weight_decay, decay=None):
+    """(P, al, ar): per layer the weight [in, H*D] and the source and destination attention vectors [H, D], drawn in
+    the order W_l, al_l, ar_l, layer by layer."""
+    shapes = []
+    for i, H in enumerate(heads):
+        shapes += [(layers[i], layers[i + 1]), (H, layers[i + 1] // H), (H, layers[i + 1] // H)]
+    params = _parameters(shapes, seed, device, learn_rate, weight_decay, decay)
+    return params[0::3], params[1::3], params[2::3]
+
+
+def _head_scores(t, a):
+    """Per-head scores <t[v, h], a[h]> of rows t [n, H*D] and attention vectors a [H, D], as a contiguous [n, H]."""
+    return (t.view(-1, *a.shape) * a).sum(-1).contiguous()
 
 
 def _minibatch_gat_op(sampled_subgraph, active, hop, gather_dtype=None):
@@ -739,41 +746,13 @@ class GATSampleImpl(_SampledRounds):
     def __init__(self, partitioned_graph, layers, features, labels, mask, fanout, batch_size, heads=8,
                  learn_rate=0.01, weight_decay=0.0001, decay_rate=0.97, decay_epoch=100, seed=0, sample_seed=0,
                  gather_dtype=None):
-        self.layers = list(layers)
-        if len(fanout) != len(self.layers) - 1:
-            raise _lib.NtsError("fanout needs one entry per layer (%d), got %d" % (len(self.layers) - 1, len(fanout)))
-        self.batch_size = int(batch_size)
-        if self.batch_size < 1:
-            raise _lib.NtsError("batch_size must be >= 1")
-        self.gather_dtype = ops._check_gather_dtype(gather_dtype)
-        self.heads = [heads] * (len(self.layers) - 2) + [1]
-        for i, H in enumerate(self.heads):
-            if self.layers[i + 1] % H:
-                raise _lib.NtsError("layer width %d is not a multiple of %d heads" % (self.layers[i + 1], H))
-        if self.gather_dtype is not None:
-            _refuse_bf16_gat_layers(self.layers, self.heads)
-        from .sample import NeighborSampler
-        self.sampler = NeighborSampler(partitioned_graph, fanout, self.batch_size, include_dst=True)
-        self._init_features(features, self.sampler.V, partitioned_graph)
-        self.sample_seed = int(sample_seed)
-        self.step = 0
-        self.ctx = NtsContext()
-        gen = torch.Generator().manual_seed(seed)
-        self.P, self.al, self.ar = [], [], []
-        for i in range(len(self.layers) - 1):
-            H = self.heads[i]
-            D = self.layers[i + 1] // H
-            for lst, shape in ((self.P, (self.layers[i], H * D)), (self.al, (H, D)), (self.ar, (H, D))):
-                prm = Parameter(*shape, learn_rate, 0.9, 0.999, 1e-9, weight_decay, device=self.device, generator=gen)
-                prm.init_parameter()
-                prm.set_decay(decay_rate, decay_epoch)
-                lst.append(prm)
-        self.L_GT = labels.to(self.device)
-        mask = torch.as_tensor(mask).cpu()
-        self.nids = [(mask == s).nonzero().view(-1) for s in (0, 1, 2)]    # train / val / test ids, ascending
-        self.subgraph = None
-        self.loss = None
-        self.epoch = 0
+        self.heads = _gat_heads(list(layers), heads, ops._check_gather_dtype(gather_dtype))
+        # Forward returns log-probabilities; the three NN segments of a layer share x_trans's autograd graph, so the
+        # tape's backward keeps it until the last of them has run
+        self._init_rounds(partitioned_graph, layers, features, labels, mask, fanout, batch_size, sample_seed,
+                          gather_dtype, include_dst=True, log_softmax_in_loss=False, retain_tape=True)
+        self.P, self.al, self.ar = _gat_parameters(self.layers, self.heads, seed, self.device, learn_rate,
+                                                   weight_decay, (decay_rate, decay_epoch))
 
     def params(self):
         return self.P + self.al + self.ar
@@ -789,8 +768,6 @@ class GATSampleImpl(_SampledRounds):
         for l in range(L):
             hop = L - 1 - l
             b = sg.blocks[hop]
-            H = self.heads[l]
-            D = self.layers[l + 1] // H
             if l == 0:
                 x = self._input_rows(b.src)
             x_trans = ctx.runVertexForward(lambda t, _l=l: self.P[_l].forward(t), x)
@@ -798,10 +775,8 @@ class GATSampleImpl(_SampledRounds):
             # input x_trans would otherwise chain onto x_trans's own tape entry (NtsContext.appendNNOp) and leave
             # d_x_trans without a producer to go to
             x_dst = x_trans.index_select(0, b.dst_pos.long())
-            dst_att = ctx.runVertexForward(
-                lambda t, _l=l, _H=H, _D=D: (t.view(-1, _H, _D) * self.ar[_l].W).sum(-1).contiguous(), x_dst)
-            src_att = ctx.runVertexForward(
-                lambda t, _l=l, _H=H, _D=D: (t.view(-1, _H, _D) * self.al[_l].W).sum(-1).contiguous(), x_trans)
+            dst_att = ctx.runVertexForward(lambda t, _l=l: _head_scores(t, self.ar[_l].W), x_dst)
+            src_att = ctx.runVertexForward(lambda t, _l=l: _head_scores(t, self.al[_l].W), x_trans)
             nbr = ctx.runGraphOpN(_minibatch_gat_op, sg, None, [x_trans, src_att, dst_att], hop=hop,
                                   gather_dtype=self.gather_dtype)
             if l == L - 1:
@@ -838,44 +813,21 @@ class GATSampleImpl(_SampledRounds):
             why = gat_shape_error(self.layers[l + 1], H, dtype)
             if why is not None:
                 raise _lib.NtsError("layer %d cannot run full-neighbour inference: %s" % (l, why))
-        lo, hi, own, parts = self._own_csc()
-        group = None if self.table is None else self.table.group
+        lo, hi, own, group, parts = self._own_csc()
         x = self.features[lo:hi] if self.table is None else self.table.gather(np.arange(lo, hi), torch.float32)
         L = len(self.layers) - 1
         for l in range(L):
             H = self.heads[l]
-            D = self.layers[l + 1] // H
             t = x.mm(self.P[l].W.detach())
-            s = (t.view(-1, H, D) * self.al[l].W.detach()).sum(-1).contiguous()
-            d = (t.view(-1, H, D) * self.ar[l].W.detach()).sum(-1).contiguous()
+            s = _head_scores(t, self.al[l].W.detach())
+            d = _head_scores(t, self.ar[l].W.detach())
             rows = ShardedFeatureTable(t, own, group, dtype=dtype)
             scores = ShardedFeatureTable(s, own, group)
-            y = torch.zeros((hi - lo, H * D), dtype=torch.float32, device=self.device)
-            row0 = 0
-            for col, ids, _, eb, ee in parts:
-                n = col.numel() - 1
-                rows.gat_aggregate(y[row0:row0 + n], scores, d[row0:row0 + n], col, ids, eb, ee, H)
-                row0 += n
+            y = torch.zeros((hi - lo, self.layers[l + 1]), dtype=torch.float32, device=self.device)
+            for r, col, ids, _, eb, ee in parts:
+                rows.gat_aggregate(y[r], scores, d[r], col, ids, eb, ee, H)
             rows.close()
             scores.close()
             x = torch.relu(y) if l < L - 1 else y.log_softmax(1)
         return lo, x
 
-    def Loss(self, out, seeds_dev):
-        self.loss = torch.nn.functional.nll_loss(out, self.L_GT.index_select(0, seeds_dev))
-        self.ctx.appendNNOp(out, self.loss)
-        return self.loss
-
-    def train_step(self, seeds):
-        """One batch: zero the gradients, sample, forward, loss, tape backward, Adam.  Returns (loss, correct)."""
-        for p in self.params():
-            p.zero_grad()
-        self.ctx.train()
-        out = self.Forward(seeds)
-        seeds_dev = self.subgraph.seeds().long()
-        loss = self.Loss(out, seeds_dev)
-        correct = (out.argmax(1) == self.L_GT.index_select(0, seeds_dev)).sum()
-        # the three NN segments of a layer share x_trans's autograd graph: keep it until the last of them has run
-        self.ctx.self_backward(True)
-        self.Update()
-        return loss.detach(), correct

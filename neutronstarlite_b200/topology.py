@@ -27,7 +27,6 @@ import torch
 
 from . import _lib
 from .feature_table import MAX_SHARDS, PeerShards, _group_rank_world
-from .sample import _DeviceArray, _stream
 
 
 def _align16(nbytes):
@@ -85,9 +84,7 @@ class ShardedTopology(PeerShards):
 
         def fill(dst):
             for p, t in zip(dst[0], (col, row, w)):
-                if t.numel():
-                    typestr = "<f4" if t.dtype == torch.float32 else "<i4"
-                    torch.as_tensor(_DeviceArray(p, t.numel(), typestr), device=self.device).copy_(t)
+                _lib.borrowed(p, t.numel(), t.dtype, self.device).copy_(t)
 
         self._build(off, group, col.device, [(col.numel() - 1, row.numel())], fill)
 
@@ -115,9 +112,7 @@ class ShardedTopology(PeerShards):
                 lo, e0, e1 = int(off[o]), bounds[o], bounds[o + 1]
                 local = (c[lo:lo + n_dst + 1] - e0).to(torch.int32)
                 for p, t in ((p_col, local), (p_row, row[e0:e1]), (p_w, w[e0:e1])):
-                    if t.numel():
-                        typestr = "<f4" if t.dtype == torch.float32 else "<i4"
-                        torch.as_tensor(_DeviceArray(p, t.numel(), typestr), device=self.device).copy_(t)
+                    _lib.borrowed(p, t.numel(), t.dtype, self.device).copy_(t)
 
         self = cls.__new__(cls)
         self._build(off, None, col.device, shards, fill, split=True)
@@ -145,7 +140,7 @@ class ShardedTopology(PeerShards):
             (p_col, p_row, p_w), = dst
             _lib.call("nts_merge_chunk_csc", ptrs("column_offset_gpu"), ptrs("row_indices_gpu"),
                       ptrs("edge_weight_forward_gpu"), P, n_dst, n_edges, p_col, p_row if n_edges else None,
-                      p_w if n_edges else None, _stream())
+                      p_w if n_edges else None, _lib.stream())
 
         self = cls.__new__(cls)
         self._build(pg.partition_offset, group, chunks[0].column_offset_gpu.device, [(n_dst, n_edges)], fill)

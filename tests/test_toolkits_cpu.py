@@ -229,6 +229,17 @@ def test_reference_tape_drops_the_fanout_gradient(fake_ops):
     assert not torch.allclose(grads[0], grads[1])
 
 
+def test_gat_refuses_a_width_that_is_not_a_multiple_of_its_heads(fake_ops):
+    """An NtsError, as GATSampleImpl raises it (not an assert, which python -O strips), before any device work."""
+    from neutronstarlite_b200 import _lib
+    from neutronstarlite_b200.toolkits import GATImpl
+    G = fake_ops
+    layers = [13, 12, 5]
+    feats, labels, mask = _data(G.V, layers[0], layers[-1])
+    with pytest.raises(_lib.NtsError, match="layer width 12 is not a multiple of 8 heads"):
+        GATImpl(G.pg, layers, feats, labels, mask, heads=8, exchange=object())
+
+
 @pytest.mark.parametrize("eager", [False, True])
 def test_input_buffer_can_be_swapped_between_epochs(fake_ops, eager):
     """A host-fed trainer alternates two input buffers (bench.py's end-to-end leg): same losses as a resident input."""
