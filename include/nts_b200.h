@@ -451,6 +451,23 @@ int nts_scatter_add_rows_atomic(float *dst, const float *src, const nts_vid_t *r
  * all-reduced gradient (Parameter::all_reduce_to_gradient, :719-722 - ncclAllReduce here instead of .cpu() + MPI). */
 int nts_adam_update(float *W, float *M, float *V, const float *grad, uint64_t n, float weight_decay, float beta1,
                     float beta2, float alpha, float epsilon, void *stream);
+/* K11: one row-sparse Adam step of an embedding table sharded by row ranges, on the owner of rows [row_lo, row_hi).
+ * Every one of the n_ranks (1..32) ranks q has an outbox at outboxes[q] (device array of pointers, local or peer
+ * memory, each 16-byte aligned) laid out as: a uint32 count n_q at byte 0; n_q <= capacity strictly ascending global
+ * row ids (uint32) from byte 16; n_q gradient rows of `pitch` floats from byte 16 + 16*ceil(capacity/4).  For every
+ * row g in [row_lo, row_hi) named by at least one outbox, the gradient is the sum of its contributors' rows in
+ * ascending rank order (the first contributor's row plus the next, and so on, in float32), and columns [0,
+ * feature_size) of rows[g - row_lo], adam_m[..] and adam_v[..] (rows of `pitch` floats, pitch % 4 == 0, >= feature_size,
+ * 16-byte aligned) get nts_adam_update's arithmetic with that gradient, bit for bit; every other row and every pad
+ * column keeps its bits.  Scratch of the owner: mask[row_hi - row_lo] (uint32, zero on entry and on return),
+ * positions[(row_hi - row_lo) * n_ranks] (uint32) and touched[1 + row_hi - row_lo] (uint32).  Two launches on
+ * `stream`, grid-stride over the device-side counts (the host needs no count).  The outboxes must be complete before
+ * the step starts and stay unchanged until it ends; no other rank may read rows [row_lo, row_hi) meanwhile.  An empty
+ * range launches nothing and looks at no pointer. */
+int nts_embedding_step(float *rows, float *adam_m, float *adam_v, uint32_t *mask, uint32_t *positions,
+                       uint32_t *touched, const void *const *outboxes, int n_ranks, nts_vid_t capacity,
+                       nts_vid_t row_lo, nts_vid_t row_hi, nts_vid_t pitch, nts_vid_t feature_size,
+                       float weight_decay, float beta1, float beta2, float alpha, float epsilon, void *stream);
 
 /* ---- peer memory (CUDA IPC) for the NVLink exchange ------------------------------------------------------ */
 #define NTS_IPC_HANDLE_BYTES 64

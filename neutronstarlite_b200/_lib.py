@@ -109,6 +109,7 @@ SIGNATURES = {
     "nts_ipc_open_handle": (_vp, [C.c_char_p]),
     "nts_ipc_close_handle": (_int, [_vp]),
     "nts_adam_update": (_int, [_vp, _vp, _vp, _vp, _u64] + [C.c_float] * 5 + [_vp]),
+    "nts_embedding_step": (_int, [_vp] * 7 + [_int, _u32, _u32, _u32, _u32, _u32] + [C.c_float] * 5 + [_vp]),
     "nts_signal_set": (_int, [_vp, _u32, _vp]),
     "nts_signal_wait_geq": (_int, [_vp, _u32, _vp]),
     "nts_host_degrees": (_int, [_vp, _u64, _u32, _vp, _vp]),

@@ -20,7 +20,7 @@ OBJDIR = os.path.join(LIBDIR, "obj")
 LIB = os.path.join(LIBDIR, "libnts_b200.so")
 
 CU_SOURCES = ["nts_runtime.cu", "nts_aggregate.cu", "nts_plan.cu", "nts_edge_ops.cu", "nts_exchange.cu", "nts_exchange_plan.cu",
-              "nts_graph_build.cu", "nts_sample.cu", "nts_infer.cu"]
+              "nts_graph_build.cu", "nts_sample.cu", "nts_infer.cu", "nts_embedding.cu"]
 CXX_SOURCES = ["nts_graph_host.cpp"]
 HEADERS = [os.path.join(CSRC, "nts_common.cuh"), os.path.join(ROOT, "include", "nts_b200.h")]
 

@@ -178,6 +178,20 @@ __device__ __forceinline__ void atomic_max_float(float *addr, float v) {
     atomicMin(reinterpret_cast<unsigned int *>(addr), __float_as_uint(v));
 }
 
+// One element of Parameter::learnC2G_with_decay_Adam (core/NtsScheduler.hpp:774-781), every operation explicitly
+// rounded, in the reference's order:
+//   W_g = W * weight_decay + grad;  M = beta1*M + (1-beta1)*W_g;  V = beta2*V + (1-beta2)*W_g*W_g;
+//   W   = W - alpha * M / (sqrt(V) + epsilon)
+// The dense update (nts_adam_update) and the embedding's row-sparse one (K11) both call it, so a row of either gets
+// the same bits from the same inputs.
+__device__ __forceinline__ void adam_element(float &w, float &m, float &v, float grad, float weight_decay, float beta1,
+                                             float beta2, float alpha, float epsilon) {
+  const float wg = __fadd_rn(__fmul_rn(w, weight_decay), grad);
+  m = __fadd_rn(__fmul_rn(beta1, m), __fmul_rn(__fsub_rn(1.f, beta1), wg));
+  v = __fadd_rn(__fmul_rn(beta2, v), __fmul_rn(__fmul_rn(__fsub_rn(1.f, beta2), wg), wg));
+  w = __fsub_rn(w, __fdiv_rn(__fmul_rn(alpha, m), __fadd_rn(__fsqrt_rn(v), epsilon)));
+}
+
 // Segment search: the largest r in [0, n_rows) with off[r] <= e  (requires off[0] <= e < off[n_rows])
 __device__ __forceinline__ uint32_t find_row(const uint32_t *__restrict__ off, uint32_t n_rows, uint32_t e) {
   uint32_t lo = 0, hi = n_rows; // invariant: off[lo] <= e < off[hi]

@@ -75,21 +75,17 @@ __global__ void signal_wait_kernel(const uint32_t *flag, uint32_t value) {
 }
 
 // Parameter::learnC2G_with_decay_Adam (core/NtsScheduler.hpp:774-781) in one pass: the reference issues six
-// element-wise libtorch ops (each a kernel and a temporary); same arithmetic, same order of operations per element:
-//   W_g = W * weight_decay + grad;  M = beta1*M + (1-beta1)*W_g;  V = beta2*V + (1-beta2)*W_g*W_g;
-//   W   = W - alpha * M / (sqrt(V) + epsilon)
+// element-wise libtorch ops (each a kernel and a temporary); same arithmetic, same order of operations per element
+// (adam_element, nts_common.cuh)
 __global__ void adam_update_kernel(float *__restrict__ W, float *__restrict__ M, float *__restrict__ V,
                                    const float *__restrict__ grad, uint64_t n, float weight_decay, float beta1,
                                    float beta2, float alpha, float epsilon) {
-  const float omb1 = 1.f - beta1, omb2 = 1.f - beta2;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    const float w = W[i];
-    const float wg = __fadd_rn(__fmul_rn(w, weight_decay), grad[i]);
-    const float m = __fadd_rn(__fmul_rn(beta1, M[i]), __fmul_rn(omb1, wg));
-    const float v = __fadd_rn(__fmul_rn(beta2, V[i]), __fmul_rn(__fmul_rn(omb2, wg), wg));
+    float w = W[i], m = M[i], v = V[i];
+    adam_element(w, m, v, grad[i], weight_decay, beta1, beta2, alpha, epsilon);
     M[i] = m;
     V[i] = v;
-    W[i] = __fsub_rn(w, __fdiv_rn(__fmul_rn(alpha, m), __fadd_rn(__fsqrt_rn(v), epsilon)));
+    W[i] = w;
   }
 }
 

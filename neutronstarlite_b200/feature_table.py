@@ -12,6 +12,9 @@ dtype=torch.bfloat16 stores the rows rounded to BF16 (nts_rows_to_bf16, round to
 8*ceil(F/8) values with zero pad columns: half the memory, and half the bytes per gathered row, local or remote.  Its
 gathers run nts_gather_rows_sharded_bf16 and return BF16 rows, or the same rows widened to float32 on request.
 
+`ShardedEmbedding` is the learnable twin: FP32 rows trained by row-sparse Adam (K11, nts_embedding_step), the ranks
+sending gradient rows to the rows' owners through outboxes mapped over the same CUDA IPC.
+
 Scope is one node: at most 32 ranks in one CUDA-IPC domain, as for the exchange engine (exchange.py).  With one rank
 (or no process group) the table is a single shard and `gather` is a local gather."""
 from __future__ import annotations
@@ -23,6 +26,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib
+from .adam import AdamSchedule
 
 MAX_SHARDS = 32
 
@@ -287,3 +291,137 @@ class ShardedFeatureTable(PeerShards):
                   self._shards.data_ptr(), self._offsets.data_ptr(), self.world, self.pitch, idp, n, self.F,
                   _lib.stream())
         return out[:, :self.F]
+
+
+class _Outbox(PeerShards):
+    """A ShardedEmbedding's outbox: one buffer per rank, mapped by every peer (nts_embedding_step's layout)."""
+
+    def __init__(self, owner, nbytes):
+        self.group, self.rank, self.world, self.device = owner.group, owner.rank, owner.world, owner.device
+        self._alloc(nbytes)
+
+
+class ShardedEmbedding(ShardedFeatureTable, AdamSchedule):
+    """A learnable float32 [V, F] table sharded like ShardedFeatureTable, trained by row-sparse Adam (K11,
+    nts_embedding_step): `step(ids, grad)` sends the gradient rows of some global ids, and the owner of each row sums
+    what every rank sent for it, in ascending rank order, and applies Parameter's update to the row and its Adam
+    moments.  The update is lazy, as in torch.optim.SparseAdam: a step's touched rows get the step-wide alpha, beta1
+    and beta2 of the schedule (adam.AdamSchedule, one next() per step, the models' defaults: Adam(0.9, 0.999, 1e-9)
+    with learn_rate, weight_decay and the decay of set_decay(decay_rate, decay_epoch)); untouched rows and their
+    moments keep their bits.  gather, aggregate, gat_aggregate and close work as for the base class, so they read the
+    learned rows.
+
+    The constructor is collective, like the base class's.  Besides the shard, each rank keeps the moments M and V of
+    its own rows ([hi - lo, pitch] float32, zero at first), K11's scratch (a uint32 mask and position per owned row and
+    rank, and a touched-row list), and an outbox of `capacity` (default V) ids and gradient rows at the shard's pitch,
+    exported over CUDA IPC once: every rank maps every peer's outbox at construction, not per step.  dtype must be
+    torch.float32 (BF16 storage would round every update away)."""
+
+    def __init__(self, local_rows, offsets, group=None, dtype=torch.float32, capacity=None, learn_rate=0.01,
+                 weight_decay=0.0001, decay_rate=0.97, decay_epoch=100):
+        if dtype != torch.float32:
+            raise _lib.NtsError("a learnable embedding stores torch.float32 rows, not %s" % (dtype,))
+        self._outbox = None
+        super().__init__(local_rows, offsets, group, dtype)
+        try:
+            self.capacity = self.rows if capacity is None else int(capacity)
+            if not 0 <= self.capacity < 2 ** 32:
+                raise _lib.NtsError("capacity must be in [0, 2^32), got %d" % self.capacity)
+            lo, hi = (int(o) for o in self.offsets[self.rank:self.rank + 2])
+            f32, i32 = dict(dtype=torch.float32, device=self.device), dict(dtype=torch.int32, device=self.device)
+            self.M = torch.zeros((hi - lo, self.pitch), **f32)
+            self.V = torch.zeros((hi - lo, self.pitch), **f32)
+            self._mask = torch.zeros(hi - lo, **i32)
+            self._positions = torch.empty((hi - lo) * self.world, **i32)
+            self._touched = torch.empty(1 + hi - lo, **i32)
+            rows_at = 16 + 16 * ((self.capacity + 3) // 4)
+            nbytes = rows_at + 4 * self.capacity * self.pitch
+            self._outbox = _Outbox(self, nbytes)
+            box = self._outbox._buf
+            whole = _lib.borrowed(box, nbytes // 4, torch.float32, self.device)
+            whole.zero_()      # the gradient rows' pad columns stay zero
+            self._count = _lib.borrowed(box, 1, torch.int32, self.device)
+            self._ids = _lib.borrowed(box + 16, self.capacity, torch.int32, self.device)
+            self._grad_rows = whole[rows_at // 4:].view(self.capacity, self.pitch)
+            ptrs, _ = self._outbox._share(None)
+            self._outboxes = torch.tensor(ptrs, dtype=torch.int64).to(self.device)
+        except Exception:
+            if self._outbox is not None:
+                self._outbox._release()
+            self._release()
+            raise
+        self._init_schedule(learn_rate, 0.9, 0.999, 1e-9, weight_decay)
+        self.set_decay(decay_rate, decay_epoch)
+
+    def step(self, ids, grad):
+        """Collective: one Adam step of the rows `ids` with gradient rows `grad`, on every rank once per round (a rank
+        with nothing to send passes empty ids and a [0, F] grad).  ids: int32 CUDA tensor of global ids, strictly
+        ascending, in [0, V), at most `capacity` of them; grad: float32 CUDA [len(ids), F].  A row several ranks send
+        gets the sum of their rows in ascending rank order.  Ids or grad of the wrong kind and a closed table raise
+        NtsError before any device work (the order and range checks read the ids back to the host).
+
+        The step writes this rank's outbox, fences, runs K11 on this rank's rows, and fences again; a fence is a
+        synchronise of this rank's current stream and then a barrier of the group.  The two fences are enough: every
+        rank's outbox is complete before the first fence's barrier, so no owner starts K11 before every outbox it
+        reads is written; every rank's earlier gathers of peer rows, issued on the same stream, also ended before that
+        barrier, so no owner updates a row a peer is still reading.  K11 has ended on every rank before the second
+        fence's barrier, so no rank's next gather reads a row mid-update and no rank overwrites its outbox (at its next
+        step) while an owner still reads it.  Between the fences a rank runs only K11, which reads the outboxes and
+        writes its own shard, moments and scratch.  With one rank, stream order alone does all this."""
+        self._check_open()
+        if not torch.is_tensor(ids) or not ids.is_cuda or ids.dtype != torch.int32 or ids.dim() != 1 or \
+                ids.device != self.device:
+            raise _lib.NtsError("ids must be a 1-D int32 tensor on %s" % self.device)
+        n = int(ids.numel())
+        if not torch.is_tensor(grad) or not grad.is_cuda or grad.dtype != torch.float32 or grad.device != self.device \
+                or tuple(grad.shape) != (n, self.F):
+            raise _lib.NtsError("grad must be a float32 [%d, %d] tensor on %s" % (n, self.F, self.device))
+        self._check_capacity(n)
+        if n:
+            u = ids.long() & 0xFFFFFFFF
+            unsorted, out_of_range = torch.stack([(u[1:] <= u[:-1]).any(), u[-1] >= self.rows]).tolist()
+            if unsorted:
+                raise _lib.NtsError("ids must be strictly ascending (distinct, sorted)")
+            if out_of_range:
+                raise _lib.NtsError("ids must be in [0, %d)" % self.rows)
+        self._step(ids, grad)
+
+    def _step(self, ids, grad):
+        """step() without the order and range checks, for ids known to be distinct, ascending and in [0, V): a
+        contiguous int32 device tensor holding uint32 values (a sampled block's src).  A closed table and more than
+        `capacity` ids still raise NtsError before any device work."""
+        self._check_open()
+        n = int(ids.numel())
+        self._check_capacity(n)
+        self._count.fill_(n)
+        if n:
+            self._ids[:n].copy_(ids)
+            self._grad_rows[:n, :self.F].copy_(grad)
+        self._fence()
+        lo, hi = (int(o) for o in self.offsets[self.rank:self.rank + 2])
+        _lib.call("nts_embedding_step", self._buf, self.M.data_ptr(), self.V.data_ptr(), self._mask.data_ptr(),
+                  self._positions.data_ptr(), self._touched.data_ptr(), self._outboxes.data_ptr(), self.world,
+                  self.capacity, lo, hi, self.pitch, self.F, float(self.weight_decay), float(self.beta1),
+                  float(self.beta2), float(self.alpha), float(self.epsilon), _lib.stream())
+        self._fence()
+        self.next()
+
+    def _check_open(self):
+        if self._buf is None:
+            raise _lib.NtsError("the feature table is closed")
+
+    def _check_capacity(self, n):
+        if n > self.capacity:
+            raise _lib.NtsError("%d rows in one step, the outbox holds %d (capacity)" % (n, self.capacity))
+
+    def _fence(self):
+        if self.world > 1:
+            torch.cuda.current_stream(self.device).synchronize()
+            dist.barrier(group=self.group)
+
+    def close(self):
+        """Collective: closes the outboxes, then the table (PeerShards.close)."""
+        if self._outbox is not None:
+            self._outbox.close()
+            self._outbox = None
+        super().close()

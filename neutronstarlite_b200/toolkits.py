@@ -23,11 +23,12 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from .adam import AdamSchedule
 from .context import NtsContext
 from . import _lib, ops
 
 
-class Parameter:
+class Parameter(AdamSchedule):
     def __init__(self, w, h, alpha, beta1, beta2, epsilon, weight_decay, device=None, generator=None):
         scale = math.sqrt(6.0 / (w + h))
         W = (2 * scale) * torch.rand((w, h), dtype=torch.float32, generator=generator) - scale
@@ -35,41 +36,18 @@ class Parameter:
         self.M = torch.zeros((w, h), dtype=torch.float32, device=device)
         self.V = torch.zeros((w, h), dtype=torch.float32, device=device)
         self.W_gradient = None
-        # the reference keeps every hyper-parameter in `ValueType` = float and does the schedule arithmetic in float
-        # (1 - 0.999f != 0.001: a 1.3e-5 relative difference in V that the golden vectors of tests/test_adam.py see)
-        f32 = np.float32
-        self.alpha = f32(alpha)
-        self.beta1, self.beta2, self.epsilon = f32(beta1), f32(beta2), f32(epsilon)
-        self.alpha_t, self.beta1_t, self.beta2_t = f32(alpha), f32(beta1), f32(beta2)
-        self.weight_decay = f32(weight_decay)
-        self.curr_epoch = 0
-        self.decay_rate, self.decay_epoch = 1, -1
+        self._init_schedule(alpha, beta1, beta2, epsilon, weight_decay)
 
     def init_parameter(self):
         """Network_simple::broadcast from rank 0 (comm/network.h:205-211)."""
         if dist.is_initialized() and dist.get_world_size() > 1:
             dist.broadcast(self.W.data, src=0)
 
-    def set_decay(self, decay_rate, decay_epoch):
-        # the reference stores both in `int` members (NtsScheduler.hpp:663-664): 0.97 truncates to 0
-        self.decay_rate, self.decay_epoch = int(decay_rate), int(decay_epoch)
-
     def all_reduce_to_gradient(self, grad):
         """SUM (not mean) over ranks, NtsScheduler.hpp:719-722 -> comm/network.h:198-203."""
         self.W_gradient = grad.detach().clone().contiguous()
         if dist.is_initialized() and dist.get_world_size() > 1:
             dist.all_reduce(self.W_gradient, op=dist.ReduceOp.SUM)
-
-    def next(self):
-        """NtsScheduler.hpp:727-736."""
-        if self.decay_epoch != -1 and self.curr_epoch != 0 and self.curr_epoch % self.decay_epoch == 0:
-            self.alpha_t *= self.decay_rate
-        one = np.float32(1)
-        self.alpha_t = np.float32(self.alpha_t)
-        self.alpha = np.float32(self.alpha_t * np.sqrt(one - self.beta2) / (one - self.beta1))
-        self.beta1 = np.float32(self.beta1 * self.beta1_t)
-        self.beta2 = np.float32(self.beta2 * self.beta2_t)
-        self.curr_epoch += 1
 
     def forward(self, x):
         return x.mm(self.W)
@@ -340,12 +318,22 @@ class _SampledRounds:
         self.table, self.features, self.device = features, None, features.device
         self.rank, self.world = features.rank, features.world
 
-    def _input_rows(self, src, dtype=torch.float32):
+    @property
+    def _learnable(self):
+        from .feature_table import ShardedEmbedding
+        return isinstance(self.table, ShardedEmbedding)
+
+    def _input_rows(self, src, dtype=torch.float32, training=False):
         """Features of the sampled sources `src` (global ids of a block, from the sampler: in range), as float32 rows,
-        or from a BF16 table with dtype=torch.bfloat16 as BF16 rows ([n, F] view of pitched rows)."""
+        or from a BF16 table with dtype=torch.bfloat16 as BF16 rows ([n, F] view of pitched rows).  Training on a
+        ShardedEmbedding, the rows are a leaf that requires a gradient, kept with src for Update's embedding step."""
         if self.table is None:
             return self.features.index_select(0, src.long())
-        return self.table._gather(src, dtype)
+        x = self.table._gather(src, dtype)
+        if training and self._learnable:
+            x.requires_grad_(True)
+            self._embedding_rows = (src, x)
+        return x
 
     def _batches(self, ids):
         """The seeds this rank runs in each round of a pass over `ids` (None in a round without a batch for it); sets
@@ -374,8 +362,17 @@ class _SampledRounds:
     def Update(self):
         """all_reduce_to_gradient, Adam and next() for every parameter.  At world 1 a parameter without a gradient is
         skipped; data-parallel, every rank reduces and steps every parameter (a missing gradient counts as zeros), so
-        that the collectives are the same on every rank."""
+        that the collectives are the same on every rank.  Then, on a ShardedEmbedding, one collective embedding step on
+        every rank: the gradient rows of this round's deepest-hop sources, or an empty contribution from a rank without
+        a batch."""
         _update(self.params(), self.world > 1)
+        if self._learnable:
+            rows, self._embedding_rows = getattr(self, "_embedding_rows", None), None
+            if rows is not None and rows[1].grad is not None:
+                self.table._step(rows[0], rows[1].grad)
+            else:
+                self.table._step(torch.empty(0, dtype=torch.int32, device=self.device),
+                                 torch.empty((0, self.table.F), dtype=torch.float32, device=self.device))
 
     def Loss(self, out, seeds_dev):
         """GCN_CPU_SAMPLE.hpp:187-195: nll_loss over the batch's seeds, after log_softmax where Forward returns
@@ -502,7 +499,12 @@ class GCNSampleImpl(_SampledRounds):
     option, nts_segment_gather_sum_bf16); activations, weights and gradients stay float32.  Tensor features are then
     stored once as pitched BF16 rows [V, 8*ceil(F/8)] (the caller's tensor is left alone), which the first layer reads
     by global id; a BF16 table hands its rows over as BF16, a float32 table's gathered rows are rounded once.  With
-    FP32 gathers a BF16 table's rows are widened exactly.  The reproducibility condition above holds as it is."""
+    FP32 gathers a BF16 table's rows are widened exactly.  The reproducibility condition above holds as it is.
+
+    features may be a feature_table.ShardedEmbedding: its gathered rows are then a leaf of the step, the tape also
+    back-propagates the first aggregation (MiniBatchFuseOp on the deepest hop), and Update() sends the rows' gradient
+    to the table (ShardedEmbedding._step) after the parameters' Adam, on every rank in every round.  Under BF16 gathers
+    the rows are rounded by the operator as for a float32 table; their gradient stays float32."""
 
     def __init__(self, partitioned_graph, layers, features, labels, mask, fanout, batch_size, learn_rate=0.01,
                  weight_decay=0.0001, decay_rate=0.97, decay_epoch=100, drop_rate=0.5, seed=0, sample_seed=0,
@@ -528,7 +530,12 @@ class GCNSampleImpl(_SampledRounds):
             x = self.features if self.features16 is None else self.features16
         else:
             bf16 = self.gather_dtype is not None and self.table.dtype == torch.bfloat16
-            x = self._input_rows(sg.blocks[L - 1].src, torch.bfloat16 if bf16 else torch.float32)
+            x = self._input_rows(sg.blocks[L - 1].src, torch.bfloat16 if bf16 else torch.float32, training)
+            if x.requires_grad:
+                # a learnable table's rows: recorded as an NN entry ahead of the first aggregation, so that the tape
+                # back-propagates that aggregation too (self_backward stops at a lone first graph op) and the rows'
+                # gradient lands in x.grad
+                self.ctx.appendNNOp(x, x)
         for l in range(L):
             hop = L - 1 - l
             if l != 0 and training and self.drop_rate > 0:
@@ -741,7 +748,8 @@ class GATSampleImpl(_SampledRounds):
     (_SampledRounds); the first layer then reads its sources' rows from the table (nts_gather_rows_sharded).  A
     bfloat16 table's rows are widened exactly to float32 (nts_gather_rows_sharded_bf16), since they feed x W.
     `partitioned_graph` is the whole graph as a single partition on every rank, or a topology.ShardedTopology as in
-    GCNSampleImpl."""
+    GCNSampleImpl.  A feature_table.ShardedEmbedding is trained as in GCNSampleImpl (its rows' gradient reaches them
+    through x W)."""
 
     def __init__(self, partitioned_graph, layers, features, labels, mask, fanout, batch_size, heads=8,
                  learn_rate=0.01, weight_decay=0.0001, decay_rate=0.97, decay_epoch=100, seed=0, sample_seed=0,
@@ -769,7 +777,7 @@ class GATSampleImpl(_SampledRounds):
             hop = L - 1 - l
             b = sg.blocks[hop]
             if l == 0:
-                x = self._input_rows(b.src)
+                x = self._input_rows(b.src, training=training)
             x_trans = ctx.runVertexForward(lambda t, _l=l: self.P[_l].forward(t), x)
             # the destination score reads the destinations' own rows; it is recorded before the source score, whose
             # input x_trans would otherwise chain onto x_trans's own tape entry (NtsContext.appendNNOp) and leave
